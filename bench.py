@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — tokens/s of greedy caption decoding (BASELINE.json metric) on N B200s, plus the other BASELINE configs as blocks.
+"""bench.py — tokens/s of greedy caption decoding (BASELINE.json metric) on N H100s, plus the other BASELINE configs as blocks.
 
 A "step" is one pass of the hot path over one batch of synthetic clips: prologue (region / frame feature encoding, object
 interaction) + the 20-step greedy loop, i.e. one ``forward(..., 'sample')`` of the reference (misc/model.py:492-624) for B=100 clips
@@ -10,8 +10,8 @@ of 10x100x2048 fc6 RoIs and T frame rows (BASELINE configs[1]).
   e2e            the same through the C-ABI host-buffer entry point gvd_sample_greedy_host (pinned host inputs -> H2D -> prologue ->
                  loop -> D2H of ids / logits / similarity), every step
   loop_only      the 20-step greedy loop alone (gvd_decode_greedy: one CUDA-graph replay), timed directly with events
-  roofline       dominant kernel family of the step (tcgen05 GEMMs of the prologue) against the measured dense tensor peak
-  roofline_decode  attention kernel / whole decode step against the measured HBM peak (SURVEY.md 8d algorithmic bytes)
+  roofline       dominant kernel family of the step (wgmma GEMMs of the prologue) against the dense tensor peak
+  roofline_decode  attention kernel / whole decode step against the HBM peak (SURVEY.md 8d algorithmic bytes)
   stages_ms_per_step  per-stage CUDA-event times recorded on the launching stream by the library's profiler in a SEPARATE pass (the
                  profiled pass enqueues the loop kernel by kernel instead of replaying the graph)
   t480           the reference-default T=480 frame rows (opts.py:50)
@@ -59,6 +59,8 @@ def parse():
     ap.add_argument("--only", default="", help="comma list of extra blocks to run (t480,beam,train,gpu_reference,transformer); default: all")
     ap.add_argument("--no-gpu-reference-tfm", action="store_true", help="skip the eager-PyTorch timing inside the transformer block")
     ap.add_argument("--train-steps", type=int, default=3)
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write what the last timed step of the headline leg returned (token ids, their log-probs, region attention) as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -68,12 +70,11 @@ def peaks():
         p = json.load(open(path))
         return dict(hbm_gbs=float(p["hbm_gbs"]), bf16_tflops=float(p.get("bf16_tflops_sustained", p["bf16_tflops"])),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1400.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, source="NVIDIA H100 SXM data sheet (700 W card; not measured)")
 
 
 def ncu_traffic():
-    """dram bytes per launch of the named kernels from the committed ncu captures of this round (profiles/traffic.json, written by
-    tools/ncu_traffic.py from `ncu --set full` reports); {} when no capture has been committed."""
+    """dram bytes per launch of the named kernels from a profiler capture (profiles/traffic.json); {} when there is none."""
     path = os.path.join(ROOT, "profiles", "traffic.json")
     try:
         return json.load(open(path))
@@ -82,7 +83,7 @@ def ncu_traffic():
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -223,7 +224,8 @@ def measure_decode(ctx, args, T, full):
     l0 = capi.kernel_launches()
     ms, (seq, logp, att2) = ctx.timed(step_dev, K)
     launches = capi.kernel_launches() - l0
-    r = dict(opt=opt, sd=sd, ms=ms, launches=launches, uniq=int(len(torch.unique(seq))), B=B, K=K, W=W, T=T)
+    r = dict(opt=opt, sd=sd, ms=ms, launches=launches, uniq=int(len(torch.unique(seq))), B=B, K=K, W=W, T=T,
+             outputs={"seq": seq, "logp": logp, "att2": att2})
     if args.quick:
         r["clocks"] = None
         return r
@@ -471,12 +473,35 @@ def gpu_reference(opt, sd, B, T):
             "(fp32, allow_tf32=False, cudnn.benchmark=True), eager", "torch": torch.__version__}
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(path, outputs):
+    """The arrays the caller of the timed path received in its last step, one float .npy each (token ids as float64: exact), at most 64 MB
+    in all: an array over its share of the limit is stored as a fixed, seeded sample of its rows (first axis), with the row indices next to
+    it as <name>_rows.npy."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    share = DUMP_LIMIT_BYTES // max(1, len(outputs))
+    for name, t in outputs.items():
+        a = t.detach().cpu()
+        a = a.to(torch.float32 if a.is_floating_point() else torch.float64).numpy()
+        if a.nbytes > share:
+            keep = max(1, int(share // (a.nbytes // a.shape[0] + 8)))           # (+8: the float64 index of the row)
+            rows = np.sort(np.random.default_rng(20240229).choice(a.shape[0], size=keep, replace=False))
+            np.save(os.path.join(path, name + "_rows.npy"), rows.astype(np.float64))
+            a = a[rows]
+        np.save(os.path.join(path, name + ".npy"), a)
+
+
 def run_ours(args):
     ctx = Ctx(args)
     only = set(x for x in args.only.split(",") if x) or {"t480", "beam", "train", "gpu_reference", "transformer"}
     T = args.frames
     r = measure_decode(ctx, args, T, True)
     opt, B, K, W = r["opt"], r["B"], r["K"], r["W"]
+    if args.dump_outputs and ctx.rank == 0:
+        dump_outputs(args.dump_outputs, r["outputs"])
     world = ctx.world
     tokens = world * B * opt.seq_length * K
     pk = peaks()
@@ -531,10 +556,10 @@ def run_ours(args):
         fl_k = 2.0 * B * R_ * per_row
         n_launch = kg[1] / K
         k_ms = kg[0] / K
-        tr_k = traffic.get("f16ss_persistent_kernel", {})
+        tr_k = traffic.get("wg_gemm_kernel", {})
         ach = fl_k / (k_ms / 1e3) / 1e12
         line["roofline"] = {
-            "kernel": "f16ss_persistent_kernel<256> (conversion-free persistent tcgen05 GEMM, both operands fp16x3 images; %d launches per step: fc7, "
+            "kernel": "wg_gemm_kernel<fp16x3> (conversion-free wgmma GEMM, both operands fp16x3 images; %d launches per step: fc7, "
                       "similarity, region embedding, Q|K|V, Wo, FFN x2 per encoder layer, ctx2pool; %.0f%% of the step)" % (round(n_launch), 100 * k_ms / (r["ms"] / K)),
             "bound": "tensor", "achieved": ach, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": ach / pk["bf16_tflops"],
             "frac_of_3pass_ceiling": ach / (pk["bf16_tflops"] / 3),
@@ -548,8 +573,8 @@ def run_ours(args):
         fl = prologue_flops(opt, B, T)
         ach = fl / (gemm_ms / 1e3) / 1e12
         line["roofline_prologue_family"] = {
-            "kernels": "every dense contraction of the prologue: f16ss_persistent_kernel, tc2_gemm_kernel (frame branch, clip vector), tc_astat_kernel + "
-                       "tc_pv_kernel (self-attention pair), gru_step_f16_kernel, and the remaining activation packing passes",
+            "kernels": "every dense contraction of the prologue: wg_gemm_kernel in its modes (operand-image GEMMs, frame branch, clip vector, "
+                       "self-attention pair, GRU step), and the remaining activation packing passes",
             "achieved": ach, "peak": pk["bf16_tflops"], "unit": "TFLOP/s", "frac": ach / pk["bf16_tflops"], "algorithmic_flops_per_step": fl,
             "ms_per_step": gemm_ms, "share_of_step": gemm_ms / (r["ms"] / K), "note": note,
         }
@@ -613,13 +638,16 @@ def run_reference(args):
     inp = synth.make_inputs(opt, n, seed=1234, masked=False)
     pick_cpu_threads(opt, sd, inp)
     K, W = args.steps, max(0, min(args.warmup, 2))
+    out = None
     with torch.no_grad():
         for _ in range(W):
             O.sample_greedy(sd, opt, inp)
         t0 = time.perf_counter()
         for _ in range(K):
-            O.sample_greedy(sd, opt, inp)
+            out = O.sample_greedy(sd, opt, inp)
         dt = time.perf_counter() - t0
+    if args.dump_outputs and out is not None:
+        dump_outputs(args.dump_outputs, {"seq": out[0], "logp": out[1], "att2": out[2]})
     v = n * opt.seq_length * K / dt
     # the same workload object as our arm; the arm-specific facts (CPU algorithm, bounded sample, one host process) sit next to it
     cfg = workload_config(args.batch, T, opt.seq_length, max(1, int(os.environ.get("WORLD_SIZE", args.gpus))))

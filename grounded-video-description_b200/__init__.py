@@ -1,7 +1,7 @@
-"""gvd-b200: B200-native caption-decode hot path of grounded-video-description.
+"""gvd-b200: H100-native caption-decode hot path of grounded-video-description.
 
 Layout:
-  csrc/     hand-written sm_100a CUDA kernels + the C-ABI (include/gvd_b200.h)
+  csrc/     hand-written sm_90a CUDA kernels + the C-ABI (include/gvd_b200.h)
   capi.py   ctypes binding of the C-ABI (raw device pointers, sizes, stream)
   misc/     host-side mirror of the reference's nn.Module surface
             (misc/AttModel.py, misc/model.py, misc/CaptionModelBU.py)

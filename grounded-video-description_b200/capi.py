@@ -1,4 +1,4 @@
-"""ctypes binding of the C-ABI in include/gvd_b200.h (libgvd_b200.so, hand-written sm_100a CUDA).
+"""ctypes binding of the C-ABI in include/gvd_b200.h (libgvd_b200.so, hand-written sm_90a CUDA).
 
 PyTorch is used here only for device memory, streams and dtype bookkeeping: every entry point
 receives raw device pointers (``tensor.data_ptr()``), sizes and the current CUDA stream.
@@ -47,7 +47,7 @@ def lib():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise GvdError("%s not found: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                       "(nvcc, sm_100a). gvd_b200 has no CPU or PyTorch fallback." % LIB_PATH)
+                       "(nvcc, sm_90a). gvd_b200 has no CPU or PyTorch fallback." % LIB_PATH)
     L = ctypes.CDLL(LIB_PATH)
     vp, ci, sz, i64 = ctypes.c_void_p, ctypes.c_int, ctypes.c_size_t, ctypes.c_int64
     L.gvd_last_error.restype = ctypes.c_char_p
@@ -483,7 +483,7 @@ class TransformerCaptioner:
 
 
 def set_backend(flags):
-    """0 = fp32 CUDA cores, 1 = tcgen05 3xTF32 tensor cores for every GEMM-shaped stage."""
+    """0 = fp32 CUDA cores, 1 = wgmma 3xTF32 tensor cores for every GEMM-shaped stage."""
     lib().gvd_set_backend(int(flags))
 
 
@@ -525,7 +525,7 @@ def op_linear_f16ss(A, W, bias=None, act=0, want_img=False, want_c=True):
 
 
 def op_scores_tc(A, W, nh, hs):
-    """C[b,h] = A[b][:, h*hs:(h+1)*hs] @ W[b][:, h*hs:(h+1)*hs].T through the A-stationary tcgen05 kernel."""
+    """C[b,h] = A[b][:, h*hs:(h+1)*hs] @ W[b][:, h*hs:(h+1)*hs].T through the tensor-core score product."""
     nb, M, ld = A.shape
     N = W.shape[1]
     C = torch.empty(nb, nh, M, N, dtype=torch.float32, device="cuda")
@@ -535,7 +535,7 @@ def op_scores_tc(A, W, nh, hs):
 
 
 def op_self_attention_tc(qkv, nh, hs, scale, debug=False, E=None, F=None, stages=3):
-    """concat_h softmax(Q_h K_h^T * scale) V_h for qkv [nb, R, 3*HP] through the fused tcgen05 attention pair.
+    """concat_h softmax(Q_h K_h^T * scale) V_h for qkv [nb, R, 3*HP] through the fused wgmma attention pair.
     debug=True also returns the softmax as stored: numerators E [nb,nh,R,R] and group factors F [nb,nh,ceil(R/32),R];
     stages=1 runs only the score kernel, stages=2 only P.V on caller-provided E / F."""
     nb, R, three_hp = qkv.shape

@@ -26,15 +26,16 @@ void gvd_count_launch() { g_launches.fetch_add(1, std::memory_order_relaxed); }
 long long gvd_launch_count() { return g_launches.load(); }
 void gvd_launch_count_add(long long n) { g_launches.fetch_add(n, std::memory_order_relaxed); }
 extern "C" GVD_API const char* gvd_last_error(void) { return g_err; }
-extern "C" GVD_API const char* gvd_version(void) { return "gvd-b200 0.1.0 (sm_100a)"; }
+extern "C" GVD_API const char* gvd_version(void) { return "gvd-b200 0.1.0 (sm_90a)"; }
 extern "C" GVD_API int gvd_op_kernel_launches(void) { return (int)g_launches.load(); }
-// backend switches (gvd_set_backend): bit 0 tcgen05 tensor cores for every GEMM-shaped stage (0 = fp32 CUDA cores); bit 1 fused self-attention
-// pair; bit 2 (4) 256-column prologue tiles (measured: no gain, off); bit 3 (8) operand-swapped split-K decode products with fused
-// reduce + sampler; bit 4 (16) fp16x3 instead of 3xTF32 in the forward GEMMs (pre-split constant weights); bit 5 (32) persistent GRU layer
-// kernel (measured: no gain, off); bit 6 (64) programmatic dependent launch in the decode loop (measured: no gain, off); bit 7 (128)
-// conversion-free persistent GEMMs for the prologue (activations packed into the fp16x3 image, both operands straight from TMA); bit 8 (256)
+// backend switches (gvd_set_backend): bit 0 wgmma tensor cores for every GEMM-shaped stage (0 = fp32 CUDA cores); bit 1 fused self-attention
+// pair; bit 2 (4) inert (it selected 256-column tiles of a kernel that needed tensor memory); bit 3 (8) operand-swapped split-K decode products
+// with fused reduce + sampler; bit 4 (16) fp16x3 instead of 3xTF32 in the forward GEMMs (pre-split constant weights); bit 5 (32) cooperative
+// GRU layer kernel (off); bit 6 (64) programmatic dependent launch in the decode loop (off); bit 7 (128) conversion-free GEMMs for the
+// prologue (activations packed into the fp16x3 image, both operands straight from TMA); bit 8 (256)
 // fp16x3 images instead of tf32 planes in the fused self-attention pair; bit 9 (512) pack fusion: the producer of a prologue activation (GEMM
-// epilogue / row kernel) stores the fp16x3 operand image the next GEMM streams, instead of a separate pack pass.
+// epilogue / row kernel) stores the fp16x3 operand image the next GEMM streams, instead of a separate pack pass; bit 10 (1024) inert (it
+// selected CTA pairs).  Bits 2 and 10 are accepted so that stored flag values keep working; nothing reads them.
 // Default 923 = 1 + 2 + 8 + 16 + 128 + 256 + 512.
 static std::atomic<int> g_backend{923};
 int gvd_backend() { return g_backend.load(std::memory_order_relaxed); }
@@ -571,8 +572,8 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     gvd_attn_chunks(R, T, w.RC, w.TC, &w.nch_r, &w.nch_t);
     w.clip_chunk = std::max(1, std::min(B, (int)(100000000ll / ((long long)m->nheads * R * R * 4 + 1))));   // S chunk ~<= 100 MB (L2)
     // the attention kernels run one CTA per (clip, head, 128 query rows) and one CTA per SM: a chunk that is one full wave
-    // (148 SMs -> 3 clips x 6 heads x 8 row blocks = 144 CTAs at R = 1000) has no partial second wave
-    w.clip_chunk = std::max(1, std::min(w.clip_chunk, 148 / std::max(1, m->nheads * ((R + 127) / 128))));
+    // (132 SMs -> 2 clips x 6 heads x 8 row blocks = 96 CTAs at R = 1000) has no partial second wave
+    w.clip_chunk = std::max(1, std::min(w.clip_chunk, 132 / std::max(1, m->nheads * ((R + 127) / 128))));
     {
         static const int env_chunk = getenv("GVD_CLIP_CHUNK") ? atoi(getenv("GVD_CLIP_CHUNK")) : 0;
         if (env_chunk > 0) w.clip_chunk = std::min(B, env_chunk);
@@ -639,10 +640,10 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     w.xt = (float*)take(BD * d.input_encoding_size * 4);
     w.sk_ldp = (int)rup(BD, 4);
     w.xcat_att = w.xcat_lang = w.sk_part = w.xp_att = w.xp_lang = nullptr;
-    if (BD <= 128) {    // operand-swapped split-K path (experimental, backend bit 3): at most 148 (weight-row tile, K split) pairs per product
+    if (BD <= 128) {    // operand-swapped split-K path (experimental, backend bit 3): at most 132 (weight-row tile, K split) pairs per product
         w.xcat_att = (float*)take(BD * (size_t)(d.input_encoding_size + H) * 4);
         w.xcat_lang = (float*)take(BD * (size_t)3 * H * 4);
-        w.sk_part = (float*)take((size_t)148 * 128 * w.sk_ldp * 4 + (size_t)BD * 64);      // [S][B][ldp], S * ceil(Nw/128) <= 148, ldp <= Nw + 3
+        w.sk_part = (float*)take((size_t)132 * 128 * w.sk_ldp * 4 + (size_t)BD * 64);      // [S][B][ldp], S * ceil(Nw/128) <= 132, ldp <= Nw + 3
         w.xp_att = (float*)take(BD * (size_t)(d.input_encoding_size + H) * 4);
         w.xp_lang = (float*)take(BD * (size_t)3 * H * 4);
         w.q_part = (float*)take((size_t)4 * BD * 2 * A * 4);
@@ -733,7 +734,7 @@ static int check_ws(const gvd_model* m, int B, int T, void* workspace, size_t by
 
 // ------------------------------------------------------------------------------------ prologue
 // C = act(A W^T + bias) for a constant, registered weight W.  Backend bit 7: pack the activation operand into the fp16x3 image (one
-// element-wise pass: 4 B read + 4 B written per element) and run the conversion-free kernel (f16ss_kernel: TMA -> tcgen05 SS MMAs);
+// element-wise pass: 4 B read + 4 B written per element) and run the conversion-free kernel (MODE_SS of wg_gemm_kernel: TMA -> wgmma on two operand images);
 // otherwise the conversion kernel (tc2_gemm_kernel) on the fp32 operand.
 // Pack fusion: the producer of an activation can store its operand image directly (A_img: the image of A, pitch rup32(K), already
 // written by whoever produced A; C_img: have THIS GEMM's epilogue store the image of its output, pitch rup32(N)) — the pack pass and
@@ -746,10 +747,7 @@ static bool linear_w_f16ss(const WS& w, const float* W, long long ldw, int M, in
     if (ldwp) *ldwp = l;
     return ok;
 }
-static bool pack_fusion() {
-    static const bool off = getenv("GVD_SS_NO_PERSIST") != nullptr;      // (the image is stored by the persistent kernel's epilogue)
-    return !off && (gvd_backend() & 512) != 0;                            // backend bit 9
-}
+static bool pack_fusion() { return (gvd_backend() & 512) != 0; }      // backend bit 9
 static int linear_w(const WS& w, const float* A, long long lda, const float* W, long long ldw, const float* bias, float* C, long long ldc, int M, int N,
                     int K, int act, cudaStream_t st, const float* scale2 = nullptr, const float* shift2 = nullptr, const float* A_img = nullptr,
                     float* C_img = nullptr) {
@@ -817,9 +815,8 @@ static int obj_interact_fwd(const gvd_model* m, const WS& w0, int c0, int B, cud
             // V^T per clip (the P.V product is then again an NT GEMM with K = R contiguous)
             GVD_STAGE("interact.v_transpose", gvd_transpose(w.qk + 2 * HP, w.vT, B, R, HP, 3 * HP, st));
         }
-        // The P.V epilogue stores the operand image of the output projection's input (no fp32 att_o, no pack pass).  Through the staged, coalesced
-        // epilogue (session 38): P.V 1.98 -> 2.12 ms per step, Wo + pack 1.75 -> 1.30 ms.  (Thread-per-row stores of the image words, session 36:
-        // P.V 2.60 ms — slower than the pack pass it removed.)  GVD_NO_ATT_O_IMG restores the pack pass.
+        // The P.V epilogue stores the operand image of the output projection's input (no fp32 att_o, no pack pass).
+        // GVD_NO_ATT_O_IMG restores the pack pass.
         static const bool no_o_img = getenv("GVD_NO_ATT_O_IMG") != nullptr;
         const long long HPi = (HP + 31) / 32 * 32;
         const bool o_img = fuse && att16 && !no_o_img && HS % 4 == 0 && linear_w_f16ss(w, m->wo[l], HP, (int)BR, H, HP);
@@ -909,7 +906,7 @@ static int frame_branch_fwd(const gvd_model* m, const WS& w0, int B, int T, cons
         }
         GVD_CHECK_CUDA(cudaMemsetAsync(w.hstate, 0, (size_t)2 * 2 * B * G * sizeof(float), st));
         {
-            // tensor-core step kernel (bit 4): gh = W_hh h on tcgen05 from two pre-split operands with the gate math in the epilogue — one
+            // tensor-core step kernel (bit 4): gh = W_hh h on wgmma from two pre-split operands with the gate math in the epilogue — one
             // launch per time step instead of a CUDA-core GEMM + a pointwise kernel
             static const bool old_gru = getenv("GVD_GRU_OLD") != nullptr;
             const float* Wimg = nullptr;
@@ -990,17 +987,15 @@ static int frame_stages(const gvd_model* m, const WS& w, int B, int T, const flo
     return 0;
 }
 
-// The frame stages next to the region stages (P2-P6) instead of behind them: the bi-GRU is 2 * 2 * T dependent launches on 32 SMs (17.7 us
-// each: 17 ms at the reference-default T = 480) that nothing else in the prologue depends on.  They run on a second stream;
-// while they do, the persistent GEMMs of the region stages launch 32 CTAs fewer (gvd_sm_reserve), otherwise every GRU step would wait
-// for a whole GEMM to drain.  Off under the stage profiler (its per-stage times are meant to be serial) or with GVD_NO_FRAME_OVERLAP.
+// The frame stages next to the region stages (P2-P6) instead of behind them: the bi-GRU is 2 * 2 * T dependent launches of a few CTAs
+// that nothing else in the prologue depends on.  They run on a second stream; no GEMM here is persistent, so the chain's CTAs find SMs as
+// the region kernels' CTAs retire.  Off under the stage profiler (its per-stage times are meant to be serial) or with GVD_NO_FRAME_OVERLAP.
 static bool frame_overlap_on() { return g_prof_on.load(std::memory_order_relaxed) == 0 && getenv("GVD_NO_FRAME_OVERLAP") == nullptr; }
 static int frame_fork(gvd_model* m, cudaStream_t st) {
     if (!m->frame_stream) {
         int lo = 0, hi = 0;
         GVD_CHECK_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-        // default priority: measured (B = 100, T = 480, tools/overlap_diag.py) prologue 38.2 ms serial, 30.5 ms with this stream at the default
-        // priority; at the highest priority the programmatically serialized GRU chain holds back every region kernel until it ends (39.0 ms)
+        // lowest priority by default: at the highest one the GRU chain can hold back every region kernel until it ends
         GVD_CHECK_CUDA(cudaStreamCreateWithPriority(&m->frame_stream, cudaStreamNonBlocking, getenv("GVD_FRAME_PRIO_HIGH") ? hi : lo));
         GVD_CHECK_CUDA(cudaEventCreateWithFlags(&m->ev_fork, cudaEventDisableTiming));
         GVD_CHECK_CUDA(cudaEventCreateWithFlags(&m->ev_join, cudaEventDisableTiming));
@@ -1014,28 +1009,6 @@ static int frame_join(gvd_model* m, cudaStream_t st) {
     GVD_CHECK_CUDA(cudaStreamWaitEvent(st, m->ev_join, 0));
     return 0;
 }
-// Clips of the region stages that run with the SM reserve: about as many as the GRU chain lasts (measured: 17.7 us per GRU step, 0.21 ms per
-// clip of region stages on 148 SMs), whole attention sub-batches; short clips (T < 64: chain < 2.3 ms) run without a reserve.
-// (one GRU step = 2 directions x G / 32 CTAs, one per SM; GVD_FRAME_RESERVE_SMS overrides — more leaves room for the next step's CTAs, which
-// programmatic stream serialization schedules early to prefetch their W_hh tiles)
-static int frame_reserve_sms(const gvd_model* m) {
-    const char* e = getenv("GVD_FRAME_RESERVE_SMS");
-    return e ? std::max(0, std::min(120, atoi(e))) : 2 * (m->G / 32);
-}
-static int frame_reserve_clips(const gvd_model* m, const WS& w, int B, int T) {
-    if (T < 64) return 0;
-    const double gru_ms = 2.0 * T * 0.0177 + 0.3, clip_ms = 0.21 * 148.0 / (148.0 - frame_reserve_sms(m));
-    const double scale = getenv("GVD_FRAME_RESERVE_SCALE") ? atof(getenv("GVD_FRAME_RESERVE_SCALE")) : 1.0;
-    if (frame_reserve_sms(m) == 0 || scale <= 0.0) return 0;
-    const int n = (int)(scale * gru_ms / clip_ms) + 1;
-    return std::min(B, (n + w.clip_chunk - 1) / w.clip_chunk * w.clip_chunk);
-}
-struct SmReserveScope {
-    int old;
-    explicit SmReserveScope(int n) : old(gvd_sm_reserve(n)) {}
-    ~SmReserveScope() { gvd_sm_reserve(old); }
-};
-
 extern "C" GVD_API int gvd_prologue_fwd(gvd_model_t* m, int B, int T, const float* segs_feat, const float* ppls, const int64_t* num,
                                 const float* ppls_feat, const int64_t* sample_idx, const uint8_t* pnt_mask, void* workspace,
                                 size_t workspace_bytes, float* sim_mat_out, void* stream) {
@@ -1066,15 +1039,7 @@ extern "C" GVD_API int gvd_prologue_fwd(gvd_model_t* m, int B, int T, const floa
                                  sim_mat_out ? sim_mat_out + (size_t)c0 * m->NC * R : nullptr, st);
         }
     } else {
-        // P2-P6: the first n_res clips next to the GRU chain with the SM reserve, the rest on the whole GPU
-        const int n_res = overlap ? frame_reserve_clips(m, w, B, T) : 0;
-        if (n_res > 0) {
-            SmReserveScope rs(frame_reserve_sms(m));
-            rc = region_prologue(m, w, 0, n_res, ppls, ppls_feat, pnt_mask, sim_mat_out, st);
-        }
-        if (rc == 0 && n_res < B)
-            rc = region_prologue(m, w, n_res, B - n_res, ppls + (size_t)n_res * R * 7, ppls_feat + (size_t)n_res * R * d.att_feat_size,
-                                 pnt_mask + (size_t)n_res * (R + 1), sim_mat_out ? sim_mat_out + (size_t)n_res * m->NC * R : nullptr, st);
+        rc = region_prologue(m, w, 0, B, ppls, ppls_feat, pnt_mask, sim_mat_out, st);          // P2-P6
     }
     if (otrace) GVD_CHECK_CUDA(cudaEventRecord(te[2], st));
     if (overlap) GVD_TRY(frame_join(m, st));
@@ -1083,8 +1048,7 @@ extern "C" GVD_API int gvd_prologue_fwd(gvd_model_t* m, int B, int T, const floa
         float a = 0.f, b = 0.f;
         cudaEventElapsedTime(&a, te[0], te[1]);
         cudaEventElapsedTime(&b, te[0], te[2]);
-        fprintf(stderr, "[gvd] overlap trace: frame stream done %.2f ms, region stages done %.2f ms after the fork (reserve %d SMs for %d clips)\n", a, b,
-                frame_reserve_sms(m), frame_reserve_clips(m, w, B, T));
+        fprintf(stderr, "[gvd] overlap trace: frame stream done %.2f ms, region stages done %.2f ms after the fork\n", a, b);
         for (auto& e : te) cudaEventDestroy(e);
     }
     return rc;
@@ -1263,9 +1227,8 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
     GVD_TRY(gvd_decode_reset_state(m, B, T, workspace, workspace_bytes, (void*)st));
     GVD_CHECK_CUDA(cudaMemsetAsync(w.it, 0, (size_t)B * sizeof(long long), st));            // <bos> = 0 (model.py:587-588)
     // The pick kernel also writes the next step's xt = ReLU(embed[token]) (no separate embedding launch).  Folding the whole
-    // sampler into the vocabulary-head GEMM epilogue (mode 2 of tc2_gemm_kernel, last-CTA merge of 154 per-CTA partials) is
-    // implemented and parity-tested but measured SLOWER (168 us vs 62 us per step: the merge is a serial chain on one CTA),
-    // so it is only used when GVD_FUSED_PICK is set.
+    // sampler into the vocabulary-head GEMM epilogue (MODE_PICK of wg_gemm_kernel, last-CTA merge of the per-CTA partials) is
+    // implemented and parity-tested; its merge is a serial chain on one CTA, so it is only used when GVD_FUSED_PICK is set.
     const bool tc = (gvd_backend() & 1) != 0 && H % 8 == 0;
     static const bool fused_pick = getenv("GVD_FUSED_PICK") != nullptr;
     const bool fused = tc && fused_pick && B <= 128;
@@ -1310,7 +1273,7 @@ extern "C" GVD_API int gvd_decode_greedy(gvd_model_t* m, int B, int T, void* wor
     GVD_REQUIRE(pnt_mask && seq_out && att2_logits_out, "decode_greedy: null argument");
     cudaStream_t st = (cudaStream_t)stream;
     const int L = m->d.seq_length, R = m->R;
-    // Direct enqueue when the stage profiler is on (its events cannot be captured) or when asked (GVD_NO_GRAPH: per-kernel ncu runs)
+    // Direct enqueue when the stage profiler is on (its events cannot be captured) or when asked (GVD_NO_GRAPH: per-kernel profiling)
     static const bool no_graph = getenv("GVD_NO_GRAPH") != nullptr;
     if (no_graph || g_prof_on.load(std::memory_order_relaxed) != 0)
         return decode_greedy_enqueue(m, w, B, T, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_logits_out, st);
@@ -1465,11 +1428,9 @@ extern "C" GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_si
     return 0;
 }
 
-// Clip chunks of the host-buffer entry point.  The persistent GEMMs walk 128-row tiles on 148 CTAs, so a chunk costs whole waves: 9 / 18 / 27 clips
-// (71 / 141 / 211 row tiles) fill their last wave to > 93 %, 12 clips (94 tiles) only to 64-80 %.  The pipeline starts with one attention
-// sub-batch (`unit` clips: the first kernel waits for the first copy) and grows 1, 2, 3, 6, 9, 12, 12 ... units while the copy engine stays ahead
-// (copy 0.16 ms per clip, compute 0.21 ms per clip); a short remainder joins the last chunk.  B = 100: 3, 6, 9, 18, 27, 37 clips — measured
-// (tools/overlap_sweep.py, session 30) 27.55 ms end to end against 30.6 ms for uniform 12-clip chunks and 25.0 ms with the inputs resident.
+// Clip chunks of the host-buffer entry point.  The pipeline starts with one attention sub-batch (`unit` clips: the first kernel waits for the
+// first copy) and grows 1, 2, 3, 6, 9, 12, 12 ... units, so that the copy engine stays ahead of the compute stream; a short remainder joins
+// the last chunk.  The growth rule has not been re-tuned for the H100.
 // GVD_H2D_SCHED="3,6,9,..." (clips per chunk; a short list repeats its last entry) or GVD_H2D_CHUNK=n (uniform) override the rule.
 static std::vector<int> h2d_schedule(int B, int unit) {
     std::vector<int> s;
@@ -1529,9 +1490,9 @@ extern "C" GVD_API int gvd_sample_greedy_host(gvd_model_t* m, int B, int T, cons
     }
     cudaEvent_t ev_start = m->events[nchunks], ev_sim = m->events[nchunks + 1], ev_segs = m->events[nchunks + 2];
     // Frame stages (P1 + P7) on their own stream next to the region stages (see frame_fork).  Long clips (reference default T = 480: 590 MB of
-    // frame features, a 17 ms GRU chain): the frame features cross PCIe after the first ~30 % of the region chunks — early enough for the
-    // chain to end with the region stages, late enough for those to have work while the features travel; the chunks enqueued behind them run
-    // with the SM reserve for about as long as the chain lasts.  Without the second stream they travel last and the frame stages run last.
+    // frame features, a long GRU chain): the frame features cross PCIe after the first ~30 % of the region chunks — early enough for the
+    // chain to end with the region stages, late enough for those to have work while the features travel.  Without the second stream they
+    // travel last and the frame stages run last.
     const bool overlap = frame_overlap_on();
     const bool big_segs = BT * (size_t)FC * 4 > ((size_t)64 << 20);
     int segs_after = 0;                                   // chunks copied before the frame features (big_segs only)
@@ -1544,8 +1505,6 @@ extern "C" GVD_API int gvd_sample_greedy_host(gvd_model_t* m, int B, int T, cons
             while (segs_after < nchunks && acc < want) acc += sched[segs_after++];
         }
     }
-    const int res_sms = frame_reserve_sms(m);
-    int res_left = (overlap && big_segs) ? frame_reserve_clips(m, w, B, T) : 0;     // clips still to run with the reserve once the chain has started
     const bool trace = getenv("GVD_TRACE") != nullptr;
     const auto t_begin = std::chrono::steady_clock::now();
     auto ms_since = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(); };
@@ -1593,9 +1552,6 @@ extern "C" GVD_API int gvd_sample_greedy_host(gvd_model_t* m, int B, int T, cons
             if (big_segs && overlap && c == segs_after && !frame_done) { rc = run_frame(); if (rc) break; }
             const int cb = sched[c];
             GVD_CHECK_CUDA(cudaStreamWaitEvent(st, m->events[c], 0));
-            const bool reserve = frame_done && overlap && big_segs && res_left > 0;
-            SmReserveScope rs(reserve ? res_sms : 0);
-            if (reserve) res_left -= cb;
             rc = region_prologue(m, w, c0, cb, w.in_ppls + (size_t)c0 * R * 7, w.in_feat + (size_t)c0 * R * d.att_feat_size,
                                  w.in_mask + (size_t)c0 * (R + 1), h_sim_mat_out ? w.out_sim + (size_t)c0 * m->NC * R : nullptr, st);
             c0 += cb;
@@ -1660,7 +1616,7 @@ extern "C" GVD_API int gvd_op_linear_tc(const float* A, int64_t lda, const float
     g.M = M; g.N = N; g.K = K; g.nh = 1; g.act = act; g.alpha = 1.f;
     return gvd_gemm_nt_tc(g, 1, (cudaStream_t)stream);
 }
-// The conversion-free prologue GEMM (f16ss_persistent_kernel) on its own: both operands are packed into fp16x3 images here (scratch from the
+// The conversion-free prologue GEMM (MODE_SS of wg_gemm_kernel) on its own: both operands are packed into fp16x3 images here (scratch from the
 // stream-ordered allocator), optionally with the fp16x3 image of the output (img_out [M, rup32(N)] words) next to / instead of C.  Test hook.
 extern "C" GVD_API int gvd_op_linear_f16ss(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias, float* C, int64_t ldc,
                                            float* img_out, int M, int N, int K, int act, void* stream) {
@@ -1677,7 +1633,7 @@ extern "C" GVD_API int gvd_op_linear_f16ss(const float* A, int64_t lda, const fl
     cudaFreeAsync(Wi, st);
     return rc;
 }
-// One LSTMCell step from up to two dense input segments [x0 | x1] (weights w0 [4H,K0], w1 [4H,K1]); backend 0 = CUDA cores, 1 = tcgen05
+// One LSTMCell step from up to two dense input segments [x0 | x1] (weights w0 [4H,K0], w1 [4H,K1]); backend 0 = CUDA cores, 1 = wgmma
 extern "C" GVD_API int gvd_op_lstm_step(int B, int H, const float* x0, int K0, const float* w0, int64_t ldw0, const float* x1, int K1,
                                         const float* w1, int64_t ldw1, const float* bias1, const float* bias2, const float* c_prev,
                                         float* h_out, float* c_out, int backend, void* stream) {
@@ -1701,7 +1657,7 @@ extern "C" GVD_API int gvd_op_scores_tc(const float* A, const float* W, float* C
     return gvd_gemm_nt_astat(g, nb * nh, (cudaStream_t)stream);
 }
 // Self-attention core of one encoder layer on a packed projection buffer qkv [nb, R, 3*HP] (Q | K | V, heads of width hs at
-// column h*hs):  out[nb, R, HP] = concat_h softmax(Q_h K_h^T * scale) V_h through the fused tcgen05 pair.  Test hook: the
+// column h*hs):  out[nb, R, HP] = concat_h softmax(Q_h K_h^T * scale) V_h through the fused wgmma pair.  Test hook: the
 // scratch buffers are allocated here.  E [nb,nh,R,R] (numerators) and F [nb,nh,ceil(R/32),R] (group factors) are caller
 // buffers; stages: bit 0 = scores (writes E, F), bit 1 = P.V (reads E, F, writes out).
 extern "C" GVD_API int gvd_op_self_attention_tc(const float* qkv, float* out, int nb, int nh, int R, int hs, int HP, float scale, float* E,

@@ -1,4 +1,4 @@
-// gvd-b200: shared device/host helpers for the sm_100a kernels.
+// gvd-b200: shared device/host helpers for the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -91,7 +91,7 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 __device__ __forceinline__ float sigmoid_acc(float x) { return 1.f / (1.f + expf(-x)); }
 
-// ---------------------------------------------------------------- fp16x3 operand image (gvd_tcgemm.cu: skinny_f16_kernel, pre-split weights)
+// ---------------------------------------------------------------- fp16x3 operand image (gvd_wgmma.cu: skinny_f16_kernel, pre-split weights)
 // A row of K fp32 values is stored as K 32-bit words: per 32-wide K slice 16 words of hi pairs (k = 2p, 2p + 1 in word p, low half = even k)
 // followed by 16 words of lo pairs; hi = the value rounded to 11 significant bits (exact in fp16), lo = fp16(value - hi); values are
 // multiplied by a power-of-two scale first.  word index of the hi pair of column k (even): (k / 32) * 32 + (k % 32) / 2, lo pair: + 16.

@@ -1,4 +1,4 @@
-// gvd-b200: decode-step kernels — TopDownCore.forward (misc/AttModel.py:134-164) rebuilt for sm_100a.
+// gvd-b200: decode-step kernels — TopDownCore.forward (misc/AttModel.py:134-164) rebuilt for sm_90a.
 //
 //   lstm_step_kernel     : both LSTMCells (AttModel.py:139,160): gate GEMM over up to three
 //                          K-segments (no concat is ever materialised; the token embedding is

@@ -1,4 +1,4 @@
-// gvd-b200: register-tiled fp32 NT GEMM (see gvd_gemm.cuh).  sm_100a, no tensor cores:
+// gvd-b200: register-tiled fp32 NT GEMM (see gvd_gemm.cuh).  sm_90a, no tensor cores:
 // BMxBN CTA tile, BK=16 slices staged k-major in double-buffered shared memory, TMxTN
 // accumulators per thread, 128-bit global loads along K, 128-bit shared loads, 128-bit stores.
 #include "gvd_gemm.cuh"
@@ -159,9 +159,9 @@ int gvd_gemm_nt(const GemmArgs& g, int batch, cudaStream_t stream) {
     GVD_REQUIRE(g.sAb % 4 == 0 && g.sAh % 4 == 0 && g.sWb % 4 == 0 && g.sWh % 4 == 0, "gemm: batch strides must be multiples of 4");
     GVD_REQUIRE(g.act != GVD_ACT_RELU_AFFINE_RELU || (g.scale2 && g.shift2), "gemm: act=2 needs scale2/shift2");
     GVD_REQUIRE(batch >= 1 && batch <= 65535 && g.nh >= 1, "gemm: bad batch %d", batch);
-    // tile choice: fill 148 SMs; skinny problems take narrower N tiles
+    // tile choice: fill 132 SMs; skinny problems take narrower N tiles
     const long long ctas_big = (long long)gvd_cdiv(g.M, 128) * gvd_cdiv(g.N, 128) * batch;
-    if (g.M > 64 && ctas_big >= 148) return launch<128, 128, 8, 8>(g, batch, stream);
+    if (g.M > 64 && ctas_big >= 132) return launch<128, 128, 8, 8>(g, batch, stream);
     if (g.M > 64) {
         const long long ctas_mid = (long long)gvd_cdiv(g.M, 128) * gvd_cdiv(g.N, 64) * batch;
         if (ctas_mid >= 120) return launch<128, 64, 8, 4>(g, batch, stream);

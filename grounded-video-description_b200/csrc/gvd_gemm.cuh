@@ -21,9 +21,6 @@ struct GemmArgs {
     int nh;                // heads per batch entry (blockIdx.z = b * nh + h)
     int act;               // 0 none, 1 relu, 2 relu->affine->relu
     float alpha;
-    int force_bn;          // tensor-core path only: 0 = pick the N tile by problem size, else 32 | 64 | 128
-    int pdl;               // tensor-core path only: programmatic-dependent-launch hints: bit 1 the A operand, bit 2 the W operand is constant data
-                           // (weights / prologue features) that may be streamed before the predecessor kernel has finished
     int trans_c;           // tensor-core path only: store C transposed, C[n * ldc + m] (no bias / activation): the split-K partials of the
                            // operand-swapped skinny products come out batch-major, so every later pass reads them along the contiguous dimension
 };

@@ -1,7 +1,6 @@
 // Persistent bidirectional GRU layer (model.py:150-154,562: nn.GRU(H, H/2, 2, bidirectional=True); SURVEY 8 row P7).
 //
-// Round 1 ran the recurrence as 2 launches per time step (a batched W_hh GEMM on the CUDA cores + a pointwise kernel): 4.T launches
-// for the two layers, i.e. 1920 launches and +23.7 ms per batch at the reference default T = 480.  Here ONE cooperative launch runs a
+// Run as launches per time step the recurrence needs thousands of launches per batch at the reference default T = 480.  Here ONE cooperative launch runs a
 // whole layer (both directions): CTA (c, d) owns 8 hidden units of direction d and keeps its 24 rows of W_hh (r, z, n gates) in
 // shared memory for all T steps; per step it computes gh = W_hh h(t-1) + b_hh for its units and every clip (fp32 FFMA, h staged through
 // shared memory in K chunks), applies the gate math, writes h(t) to a ping-pong global buffer and the layer output row, then meets

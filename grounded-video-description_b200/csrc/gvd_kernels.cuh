@@ -83,7 +83,7 @@ int gvd_row_argmax(const float* z, long long ld, int rows, int R, int* out, cuda
 int gvd_beam_finish(const BeamBufs& bb, const int* bos_att, int B, int K, int L, long long* seq_out, float* lp_out, long long* att_out,
                     cudaStream_t st);
 
-// ---- tcgen05 / TMEM / TMA GEMM (gvd_tcgemm.cu)
+// ---- wgmma / TMA GEMM (gvd_wgmma.cu)
 int gvd_backend();   // gvd_set_backend flags (gvd_api.cu)
 // operand-swapped split-K path for the skinny decode-step products (gvd_skinny.cu; backend bit 3)
 int gvd_skinny_splits(int Nw, int Ktot, int B);
@@ -91,7 +91,7 @@ int gvd_skinny_splitk(const float* W, int Nw, int Ktot, const float* X, long lon
 int gvd_reduce_lstm(const float* part, int S, int ldp, const float* pre, int pre_div, const float* bias1, const float* bias2, const float* c_prev,
                     float* c_out, float* h0, long long ldh0, float* h1, long long ldh1, float* h2, long long ldh2, int B, int H, cudaStream_t st,
                     float* pk1 = nullptr, long long ldpk1 = 0, float* pk2 = nullptr, long long ldpk2 = 0);
-// conversion-free fp16x3 product of two operand images (gvd_tcgemm.cu: skinny_f16_kernel)
+// conversion-free fp16x3 product of two operand images (gvd_wgmma.cu: MODE_TRANS with split K)
 int gvd_skinny_f16(const float* Wp, long long ldw, int Nw, const float* Xp, long long ldx, int B, int Ktot, int S, float* part, int ldp,
                    cudaStream_t st);
 int gvd_reduce_bias(const float* part, int S, int Nw, int ldp, const float* bias, float* out, long long ld_out, int B, cudaStream_t st);
@@ -99,7 +99,7 @@ int gvd_reduce_pick(const float* part, int S, int ldp, const float* bias, int B,
                     float* logp_out, long long out_stride, const float* embed, float* xt, long long ld_xt, int E, float* logits_out,
                     long long ld_logits, cudaStream_t st, float* xt_pk = nullptr, long long ld_xt_pk = 0);
 int gvd_gemm_nt_tc(const GemmArgs& g, int batch, cudaStream_t stream);
-int gvd_gemm_nt_astat(const GemmArgs& g, int batch, cudaStream_t stream);   // short-K (<= 192), A block stationary in TMEM
+int gvd_gemm_nt_astat(const GemmArgs& g, int batch, cudaStream_t stream);   // short-K (<= 192), one K pass
 // self-attention pair (W operands pre-split into tf32 hi / lo planes): softmax-numerator scores + group factors F, then (F (.) E) V
 int gvd_attn_scores_tc(const GemmArgs& g, const float* W_lo, float* F, float smx_scale, int batch, cudaStream_t stream, int f16 = 0);
 int gvd_attn_pv_tc(const GemmArgs& g, const float* W_lo, const float* F, int batch, cudaStream_t stream, int f16 = 0, float* img = nullptr,
@@ -137,13 +137,13 @@ int gvd_gru_layer(const float* gi, const float* whh, const float* bhh, float* hb
 int gvd_gru_layer_f16(const float* gi, const float* Whh_img, const float* bhh, float* hstate, float* h_img, float* out, const long long* sample_idx, int B,
                       int T, int G, cudaStream_t st);
 
-// fp16x3 operand images for the fused self-attention: per-head key image, transposed value image (scales must match gvd_tcgemm.cu)
+// fp16x3 operand images for the fused self-attention: per-head key image, transposed value image (scales must match gvd_wgmma.cu)
 #define GVD_ATT_SK_HOST 16.f
 #define GVD_ATT_SV_HOST 16.f
 int gvd_pack_heads_f16x3(const float* in, long long ld_in, long long rows, int nh, int hs_in, int hs, int KH, float scale, float* out, cudaStream_t st);
 int gvd_transpose_pack_f16x3(const float* in, float* out, int B, int R, int C, int ld_in, int Rp, float scale, cudaStream_t st);
 
-// fp16x3 precision scope (backend bit 4): inside a scope the tcgen05 GEMMs launched by this thread may use the fp16 hi/lo split
+// fp16x3 precision scope (backend bit 4): inside a scope the wgmma GEMMs launched by this thread may use the fp16 hi/lo split
 // (kind::f16, half the MMAs of 3xTF32).  Only forward inference stages with O(1) operands open a scope (prologue, decode step);
 // gradient products stay on 3xTF32 (fp16's exponent range is too narrow for unscaled gradients).
 bool gvd_gemm_f16();
@@ -152,10 +152,9 @@ void gvd_f16_scope(int delta);
 #define GVD_F16_SW 256.f
 // registry of pre-split constant weights (filled by gvd_model_finalize): fp32 weight pointer -> packed image (gvd_pack_f16x3)
 int gvd_pack_f16x3(const float* W, long long ldw, int N, int K, float* out, long long Kp, cudaStream_t st, float scale = GVD_F16_SW);
-// conversion-free GEMM on two operand images (gvd_tcgemm.cu: f16ss_kernel)
-// Q|K|V projection epilogue of the region encoder (f16ss_persistent_kernel): Q as fp32, K as the per-head fp16x3 image, V as the image of V^T per clip
+// conversion-free GEMM on two operand images (gvd_wgmma.cu: MODE_SS)
+// Q|K|V projection epilogue of the region encoder (MODE_SS): Q as fp32, K as the per-head fp16x3 image, V as the image of V^T per clip
 struct GvdQkvImages { int HP, HS, KH, nh, R, Rp; float *k_img, *vt_img; float sk, sv; };
-int gvd_sm_reserve(int n);   // persistent GEMMs leave n SMs free from now on (returns the previous value); see gvd_tcgemm.cu
 int gvd_gemm_f16ss(const float* Ap, long long lda, const float* Wp, long long ldw, const float* bias, const float* scale2, const float* shift2, int act,
                    float* C, long long ldc, int M, int N, int K, cudaStream_t st, float* img = nullptr, long long ld_img = 0,
                    const GvdQkvImages* qkv = nullptr);

@@ -1,16 +1,13 @@
 // Skinny (M = batch <= 128 rows) contractions of the decode step, operand-swapped and split along K (backend bit 3).
 //
-// Why: a tcgen05.mma with its A operand in TMEM costs ~45 cycles + 128.N/256 (profiles/r1_ncu_summary.md).  The decode-step GEMMs
-// (B = 100 rows of activations against 4096 x 3072 LSTM weights, the 4905 x 1024 vocabulary head, the 1024 x 1024 attention queries)
-// as 128 x 32 tiles put the (padded) batch on the 128-row M side, so every MMA covers only 32 weight rows.  Swapped, the WEIGHT rows
-// are the M side and the whole batch is one N = 128 tile (2.2x fewer tensor cycles per weight element).  The swap leaves only Nw/128
-// CTAs per launch (32 for an LSTM), so K is split across CTAs as well: split s owns the columns [s.Ks, (s+1).Ks) of both operands —
-// a "batch" of the batched NT GEMM whose batch stride is Ks ELEMENTS ALONG K for both operands (the tensor-map trick of the attention
-// heads).  Measured (ncu, B=100): the four products take 79 us per step instead of 191 us.
+// Why: with the (padded) batch on the 128-row M side of a tile, every MMA of a decode-step GEMM (B = 100 rows of activations against
+// 4096 x 3072 LSTM weights, the 4905 x 1024 vocabulary head, the 1024 x 1024 attention queries) would cover few weight rows.  Swapped, the
+// WEIGHT rows are the M side and the batch the N side (two 64-column tiles).  The swap leaves only Nw/128 row blocks per launch (32 for an
+// LSTM), so K is split across CTAs as well: split s owns the columns [s.Ks, (s+1).Ks) of both operands — a "batch" of the batched NT GEMM
+// whose batch stride is Ks ELEMENTS ALONG K for both operands (the tensor-map trick of the attention heads).
 //
 // The partial sums leave the GEMM TRANSPOSED (GemmArgs::trans_c): part[s][b][n] with the weight-row index n contiguous, so the
-// reductions below are plain coalesced element-wise passes (round 1's [s][n][b] layout needed a shared-memory transpose and cost
-// 25 us per LSTM):
+// reductions below are plain coalesced element-wise passes:
 //   reduce_lstm      gates partials -> + pre + biases -> LSTMCell pointwise -> h (up to three destinations: the state buffer and the
 //                    slots of the concatenated inputs of the next products), c                                (AttModel.py:139,160)
 //   reduce_bias      out[b][n] = sum_s part[s][b][n] + bias[n]                                                 (attention queries)
@@ -170,11 +167,11 @@ __global__ void __launch_bounds__(PICK_NT) reduce_pick_kernel(const float* __res
 }  // namespace
 
 // Number of K splits for a skinny product with Nw weight rows and Ktot columns (0 = shape not supported by this path):
-// as many CTAs as fit in one wave of the 148 SMs, every split a whole number of 32-wide K slices and at least two of them.
+// as many CTAs as fit in one wave of the 132 SMs, every split a whole number of 32-wide K slices and at least two of them.
 int gvd_skinny_splits(int Nw, int Ktot, int B) {
     if (B < 1 || B > 128 || Nw < 128 || Ktot % 32 != 0) return 0;
     const int mt = gvd_cdiv(Nw, 128);
-    int S = 148 / mt;
+    int S = 132 / mt;
     if (S < 1) return 0;
     if (S > Ktot / 64) S = Ktot / 64;
     while (S > 1 && Ktot % (S * 32) != 0) --S;
@@ -191,9 +188,7 @@ int gvd_skinny_splitk(const float* W, int Nw, int Ktot, const float* X, long lon
     g.W = X; g.ldw = ldx; g.sWb = Ks;
     g.C = part; g.ldc = ldp; g.sCb = (long long)B * ldp;
     g.M = Nw; g.N = B; g.K = Ks; g.nh = 1; g.act = GVD_ACT_NONE; g.alpha = 1.f;
-    g.force_bn = 128;                              // the whole batch is ONE 128-column tile (the point of the swap)
     g.trans_c = 1;                                 // partials come out batch-major
-    g.pdl = 2;                                     // the A operand is a weight matrix: its tiles may stream before the predecessor kernel ends
     return gvd_gemm_nt_tc(g, S, st);
 }
 

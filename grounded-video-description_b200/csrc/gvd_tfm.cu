@@ -6,7 +6,7 @@
 // result over the layer's encoder output, feed-forward, each in a ResidualBlock with the custom LayerNorm (:79-88,66-77); then the
 // vocabulary head (tied with the embedding, :207,222) and an argmax.  It RE-PROJECTS the constant encoder output with wk / wv at every
 // step (MultiHead.forward, :117-119) and re-projects every earlier position of the self-attention too; both are the same numbers each time,
-// so this file projects the encoder output once per batch (tcgen05 GEMM) and caches the self-attention keys / values per position.
+// so this file projects the encoder output once per batch (wgmma GEMM) and caches the self-attention keys / values per position.
 //
 // The step is HBM-bound: the attention over the R = 1000 region rows streams K and V of every clip once (2 * R * H * 4 B per clip-step =
 // 8.19 MB at H = 1024; 819 MB at B = 100) against ~30 MFLOP of products per clip.  tfm_cross_partial_kernel is that stream (flash-decoding
@@ -366,7 +366,7 @@ struct TfmWs {
 
 int tfm_chunking(int B, int n, int* rows) {
     // enough CTAs to cover the machine a few times over, at most TFM_RC rows each
-    int chunks = std::max(1, std::min(gvd_cdiv(n, 8), gvd_cdiv(148 * 6, std::max(B, 1))));
+    int chunks = std::max(1, std::min(gvd_cdiv(n, 8), gvd_cdiv(132 * 6, std::max(B, 1))));
     int r = gvd_cdiv(n, chunks);
     r = std::min(r, TFM_RC);
     *rows = r;
@@ -377,7 +377,7 @@ inline int rup4i(int x) { return (x + 3) / 4 * 4; }
 
 // split-K planes of one skinny product (0: generic path, one plane)
 int tfm_splits(int Nw, int K, int B) {
-    if ((gvd_backend() & 9) != 9) return 0;                  // tcgen05 + split-K decode products (backend bits 0 and 3)
+    if ((gvd_backend() & 9) != 9) return 0;                  // wgmma + split-K decode products (backend bits 0 and 3)
     return gvd_skinny_splits(Nw, K, B);
 }
 size_t tfm_part_floats(int Nw, int K, int B) { return (size_t)std::max(1, gvd_skinny_splits(Nw, K, B)) * B * rup4i(Nw); }
@@ -434,11 +434,11 @@ int tfm_check(const gvd_tfm_weights_t* w, int B, int L, int n0, int n1) {
     return 0;
 }
 
-// part[s][b][n] = partial sums of X[b, :] . W[n, :]: operand-swapped split-K tcgen05 product when the shape allows it (the weight rows fill the
+// part[s][b][n] = partial sums of X[b, :] . W[n, :]: operand-swapped split-K wgmma product when the shape allows it (the weight rows fill the
 // 128-row MMA tile, the batch is the N tile; S planes), else the generic GEMM into one plane.  Returns the plane count through *S.
 // With backend bit 4 and the weight's fp16x3 image at hand (Wimg; Ximg = scratch for the image of X): one small pack pass over the B activation
-// rows, then the conversion-free kernel of the greedy LSTM path (skinny_f16_kernel: TMA -> tcgen05 SS MMAs on both images, no conversion warps,
-// no TMEM operand slots) — the products of this loop are 2-20 MB of weights each, so their time is the fixed latency of the kernel.
+// rows, then the conversion-free kernel of the greedy LSTM path (skinny_f16_kernel: TMA -> wgmma on both operand images, no conversion,
+// ) — the products of this loop are 2-20 MB of weights each, so their time is the fixed latency of the kernel.
 bool tfm_f16() { return (gvd_backend() & 16) != 0 && getenv("GVD_TFM_NO_F16") == nullptr; }
 int tfm_product(const float* W, int Nw, int K, const float* X, long long ldx, int B, float* part, int ldp, int* S, cudaStream_t st,
                 const float* Wimg = nullptr, float* Ximg = nullptr, const float* Xready = nullptr) {

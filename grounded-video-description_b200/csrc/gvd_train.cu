@@ -1,7 +1,7 @@
 // Primitive set of the training step (gvd_b200/train.py; SURVEY 8 rows T7 / D1): the element-wise, row-wise and reduction
-// kernels of the explicit backward.  The dense products go through the tcgen05 GEMM (gvd_op_linear / gvd_tr_gemm_nt_batched).
+// kernels of the explicit backward.  The dense products go through the wgmma GEMM (gvd_op_linear / gvd_tr_gemm_nt_batched).
 //
-// EXPERIMENTAL: written after the device budget of round 1 was spent — not yet run on a device.  Every function here has its
+// Every function here has its
 // mathematical definition in tests/ops_ref.py (same name) and a per-primitive device test in tests/test_gpu_zz_train.py.
 // All tensors fp32, contiguous.  Reductions are deterministic (fixed summation order, no float atomics except cls_nll's scatter of
 // equal addends).
@@ -394,7 +394,7 @@ __global__ void adam_first_step_kernel(const float* __restrict__ w, const float*
 
 // ---------------------------------------------------------------- flat-buffer optimiser (main.py:265-266,660-677)
 // Global gradient norm of the flat fp32 gradient buffer, deterministic: fixed grid, per-block double partials, one finishing block.
-constexpr int SQ_BLOCKS = 1184;      // 8 x 148 SMs
+constexpr int SQ_BLOCKS = 1056;      // 8 x 132 SMs
 __global__ void __launch_bounds__(256) sumsq_partial_kernel(const float* __restrict__ g, long long n, double* __restrict__ part) {
     __shared__ double red[8];
     double s = 0.0;
@@ -505,12 +505,12 @@ GVD_API int gvd_tr_outer_rows(const float* a, const float* v, float* out, int B,
 GVD_API int gvd_tr_outer_rows_acc(const float* a, const float* v, float* acc, int B, int N, int H, void* st) {
     GVD_REQUIRE(a && v && acc && H % 4 == 0, "tr_outer_rows_acc: H must be a multiple of 4");
     const long long total4 = (long long)B * N * (H / 4);
-    outer_rows_acc_kernel<<<(unsigned)std::min<long long>(148 * 16, (total4 + TB - 1) / TB), TB, 0, ST(st)>>>(a, v, acc, N, H, total4);
+    outer_rows_acc_kernel<<<(unsigned)std::min<long long>(132 * 16, (total4 + TB - 1) / TB), TB, 0, ST(st)>>>(a, v, acc, N, H, total4);
     LAUNCH_OK();
 }
 GVD_API int gvd_tr_colsum(const float* x, float* out, int batch, long long M, int N, void* st) {
     const int nb = gvd_cdiv(N, 32);
-    long long RB = std::min<long long>(std::max<long long>(1, 1184 / ((long long)nb * batch)), std::max<long long>(1, M / 64));
+    long long RB = std::min<long long>(std::max<long long>(1, 1056 / ((long long)nb * batch)), std::max<long long>(1, M / 64));
     if (RB <= 1) {
         colsum_kernel<<<dim3(nb, batch, 1), dim3(32, 8), 0, ST(st)>>>(x, out, M, N, M, 0);
         LAUNCH_OK();
@@ -659,7 +659,7 @@ GVD_API int gvd_tr_adam_first_step(const float* w, const float* g, float coef, f
 GVD_API int gvd_tr_dropout(const float* x, float* y, long long n, float p, long long seed, int site, long long step, void* st) {
     GVD_REQUIRE(x && y && n >= 0 && p >= 0.f && p < 1.f, "tr_dropout: bad arguments (p = %f)", (double)p);
     if (n == 0) return 0;
-    const unsigned grid = (unsigned)std::min<long long>(148 * 16, (((n + 3) >> 2) + TB - 1) / TB);
+    const unsigned grid = (unsigned)std::min<long long>(132 * 16, (((n + 3) >> 2) + TB - 1) / TB);
     dropout_kernel<<<grid, TB, 0, ST(st)>>>(x, y, n, p, 1.f / (1.f - p), (uint32_t)(seed & 0xffffffffll), (uint32_t)((unsigned long long)seed >> 32),
                                             (uint32_t)site, (uint32_t)(step & 0xffffffffll), (uint32_t)((unsigned long long)step >> 32));
     LAUNCH_OK();
@@ -679,7 +679,7 @@ GVD_API int gvd_tr_adam_flat(float* w, float* g, float* m, float* v, long long n
                              const float* norm, float b1, float b2, float eps, float weight_decay, int t, void* st) {
     GVD_REQUIRE(w && g && m && v && seg_end && seg_lr && nseg >= 1 && n > 0 && t >= 1, "tr_adam_flat: bad arguments");
     const float bc1 = (float)(1.0 - pow((double)b1, (double)t)), bc2s = (float)sqrt(1.0 - pow((double)b2, (double)t));
-    adam_flat_kernel<<<148 * 8, 256, 0, ST(st)>>>(w, g, m, v, n, (const long long*)seg_end, seg_lr, nseg, norm, b1, b2, eps, weight_decay, bc1, bc2s);
+    adam_flat_kernel<<<132 * 8, 256, 0, ST(st)>>>(w, g, m, v, n, (const long long*)seg_end, seg_lr, nseg, norm, b1, b2, eps, weight_decay, bc1, bc2s);
     LAUNCH_OK();
 }
 // C[z] = A[z] W[z]^T  (A [batch, M, K], W [batch, N, K], C [batch, M, N]; row pitches lda / ldw / ldc, batch strides in elements)

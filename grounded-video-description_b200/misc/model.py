@@ -4,7 +4,7 @@ What is kept from the reference: the constructor signature and the ``opt`` field
 (model.py:29-73), the parameter tree / state_dict keys (checkpoint contract, main.py:638), the
 ``forward(segs_feat, seq, gt_seq, num, ppls, gt_boxes, mask_boxes, ppls_feat, frm_mask,
 sample_idx, pnt_mask, opt, eval_opt={})`` dispatch on 'MLE' | 'GRD' | 'sample' (model.py:227-234)
-and the return tuples.  What is new: all arithmetic runs in hand-written sm_100a kernels behind
+and the return tuples.  What is new: all arithmetic runs in hand-written sm_90a kernels behind
 the C-ABI (include/gvd_b200.h); the three copies of the prologue (model.py:302-409, 504-568,
 634-698) are one native call; nothing executes on the CPU and there is no torch fallback.
 """

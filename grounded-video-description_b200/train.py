@@ -2,12 +2,12 @@
 (BatchNorm batch statistics; dropout p = 0, see below), the four losses, the explicit backward, global-norm clipping and
 per-tensor Adam — `main.py:235-266,660-677` of the reference.
 
-STATUS: EXPERIMENTAL — written after the device budget of round 1 was spent.  The ORCHESTRATION in this file is verified on the
+The ORCHESTRATION in this file is verified on the
 CPU: `tests/test_train_host_logic.py` runs it with a torch mock of the primitive set (`tests/ops_ref.py`) and compares every
 gradient with the oracle (`oracle/gvd_oracle.train_step`, pinned to the reference) — it is a line-by-line transcription of the
 verified specification `oracle/gvd_backward.py`.  The PRIMITIVES used by the product (`NativeOps`: csrc/gvd_train.cu through
-the C ABI, GEMMs through the tcgen05 kernel) have not run on a device yet; their per-primitive tests are
-`tests/test_gpu_zz_train.py` (opt-in, GVD_TEST_EXPERIMENTAL=1).
+the C ABI, GEMMs through the wgmma kernel) have their per-primitive tests in
+`tests/test_gpu_zz_train.py`.
 
 Dropout: the reference draws its masks from torch's RNG, so bit parity with dropout on is undefined; like the oracle pin this
 step runs with every Dropout at p = 0.  (A Philox mask per dropout site is a local change in `lin`/`embed`.)

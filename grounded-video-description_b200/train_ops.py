@@ -1,5 +1,5 @@
 """NativeOps: the primitive set of gvd_b200.train.TrainStep on the device — every method is one (or a fixed few) C-ABI call(s) into
-csrc/gvd_train.cu, dense products through the tcgen05 GEMM.  torch is used for device memory only (allocation, views, cat/stack,
+csrc/gvd_train.cu, dense products through the wgmma GEMM.  torch is used for device memory only (allocation, views, cat/stack,
 dtype conversion of masks), never for arithmetic on float data.
 
 EXPERIMENTAL: not yet run on a device (see train.py).  The mathematical definition of each method is the method of the same name
@@ -111,7 +111,7 @@ class NativeOps:
     def cat(self, ts, dim): return torch.cat([t for t in ts], dim=dim)
     def stack1(self, ts): return torch.stack(list(ts), dim=1)
 
-    # ---- dense algebra (tcgen05 / CUDA-core GEMM of the library; contraction length padded to a multiple of 4 with zeros)
+    # ---- dense algebra (wgmma / CUDA-core GEMM of the library; contraction length padded to a multiple of 4 with zeros)
     def _gemm(self, A, W, batch):
         """A [batch, M, K], W [batch, N, K] -> [batch, M, N]"""
         A, W = _pad_last(_f(A)), _pad_last(_f(W))

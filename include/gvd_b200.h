@@ -1,4 +1,4 @@
-/* gvd-b200 C-ABI: B200-native caption-decode hot path of grounded-video-description.
+/* gvd-b200 C-ABI: H100-native caption-decode hot path of grounded-video-description.
  *
  * The reference has NO native interface: its boundary for this path is the Python nn.Module
  * surface misc/AttModel.py:167-171 (TopDownModel(opt)) / misc/model.py:227-234 (forward) /
@@ -156,32 +156,32 @@ GVD_API int gvd_plan_skinny_splits(int weight_rows, int k_total, int batch_rows)
    whole batch in one piece).  `unit` = clips per self-attention sub-batch; writes at most `cap` chunk sizes to `chunks_out`, returns their number
    (the sizes sum to batch_clips), or -1 with gvd_last_error() set.  Honours GVD_H2D_SCHED / GVD_H2D_CHUNK like the entry point itself. */
 GVD_API int gvd_plan_h2d_chunks(int batch_clips, int unit, int* chunks_out, int cap);
-/* the same contraction on the tcgen05 tensor cores (3xTF32, fp32-faithful) */
+/* the same contraction on the wgmma tensor cores (3xTF32, fp32-faithful) */
 GVD_API int gvd_op_linear_tc(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias, float* C, int64_t ldc,
                   int M, int N, int K, int act, void* stream);
 /* batched short-K (hs <= 192) product C[b,h] = A[b][:, h*hs:(h+1)*hs] . W[b][:, h*hs:(h+1)*hs]^T — the self-attention
-   score shape of transformer.py:111 — through the A-stationary tcgen05 kernel; A [nb,M,ld], W [nb,N,ld], C [nb,nh,M,N] */
+   score shape of transformer.py:111 — through the tensor-core score product; A [nb,M,ld], W [nb,N,ld], C [nb,nh,M,N] */
 GVD_API int gvd_op_scores_tc(const float* A, const float* W, float* C, int nb, int nh, int M, int N, int hs, int64_t ld, void* stream);
 /* self-attention core of one region-encoder layer (transformer.py:84-118) on a packed projection buffer qkv [nb, R, 3*HP]
    (Q | K | V; head h = columns [h*hs, (h+1)*hs)): out[nb, R, HP] = concat_h softmax(Q_h K_h^T * scale) V_h through the fused
-   tcgen05 pair.  stages bit 0: A-stationary scores with the softmax-numerator epilogue -> numer [nb,nh,R,R] and per-(row,
+   wgmma pair.  stages bit 0: A-stationary scores with the softmax-numerator epilogue -> numer [nb,nh,R,R] and per-(row,
    32-key group) factors factor [nb,nh,ceil(R/32),R] (softmax = numer * factor); bit 1: the row-scaled P.V -> out */
 GVD_API int gvd_op_self_attention_tc(const float* qkv, float* out, int nb, int nh, int R, int hs, int HP, float scale,
                   float* numer, float* factor, int stages, void* stream);
-/* the conversion-free persistent prologue GEMM on its own (operands packed into fp16x3 images inside the call); img_out: optional fp16x3 image of
+/* the conversion-free prologue GEMM on its own (operands packed into fp16x3 images inside the call); img_out: optional fp16x3 image of
    the output, [M, rup32(N)] 32-bit words (what the next GEMM would stream), C may then be NULL */
 GVD_API int gvd_op_linear_f16ss(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias, float* C, int64_t ldc,
                   float* img_out, int M, int N, int K, int act, void* stream);
-/* one LSTMCell step (AttModel.py:139,160) from up to two dense input segments; backend 0 = CUDA cores, 1 = tcgen05 */
+/* one LSTMCell step (AttModel.py:139,160) from up to two dense input segments; backend 0 = CUDA cores, 1 = wgmma */
 GVD_API int gvd_op_lstm_step(int B, int H, const float* x0, int K0, const float* w0, int64_t ldw0, const float* x1, int K1,
                   const float* w1, int64_t ldw1, const float* bias1, const float* bias2, const float* c_prev,
                   float* h_out, float* c_out, int backend, void* stream);
-/* arithmetic backend switches: bit 0 tcgen05 tensor cores for every GEMM-shaped stage (0 = fp32 CUDA cores); bit 1 fused self-attention pair;
-   bit 2 (4) 256-column tiles in the conversion kernel (measured: no gain); bit 3 (8) operand-swapped split-K decode products with fused
+/* arithmetic backend switches: bit 0 wgmma tensor cores for every GEMM-shaped stage (0 = fp32 CUDA cores); bit 1 fused self-attention pair;
+   bit 2 (4) inert; bit 3 (8) operand-swapped split-K decode products with fused
    reduce + sampler; bit 4 (16) fp16x3 instead of 3xTF32 in the forward GEMMs, pre-split weights, conversion-free decode step, tensor-core GRU;
-   bit 5 (32) persistent GRU layer kernel (no gain); bit 6 (64) programmatic dependent launch in the decode loop (no gain); bit 7 (128)
-   conversion-free persistent prologue GEMMs; bit 8 (256) fp16x3 key / value images in the self-attention pair; bit 9 (512) pack fusion
-   (producers store the operand image of the next GEMM).  Default 923 = 1 + 2 + 8 + 16 + 128 + 256 + 512.  Every combination in
+   bit 5 (32) cooperative GRU layer kernel (off); bit 6 (64) programmatic dependent launch in the decode loop (off); bit 7 (128)
+   conversion-free prologue GEMMs; bit 8 (256) fp16x3 key / value images in the self-attention pair; bit 9 (512) pack fusion
+   (producers store the operand image of the next GEMM); bit 10 (1024) inert.  Default 923 = 1 + 2 + 8 + 16 + 128 + 256 + 512.  Every combination in
    tests/test_gpu_tcgen05.py meets the same parity bar. */
 GVD_API int gvd_set_backend(int flags);
 GVD_API int gvd_get_backend(void);
@@ -198,7 +198,7 @@ GVD_API const char* gvd_profile_entry(int i, double* total_ms, long long* count)
 /* ---------------------------------------------------------------------------------------------------------------------------
  * Training-step primitives (main.py:235-266: teacher-forced forward in train mode, explicit backward, clip, Adam) — the
  * element-wise / row-wise / reduction kernels the host orchestration in gvd_b200/train.py is written over; dense products go
- * through gvd_op_linear and gvd_tr_gemm_nt_batched.  EXPERIMENTAL: not yet run on a device (round 1 ended first); definitions of
+ * through gvd_op_linear and gvd_tr_gemm_nt_batched.  Definitions of
  * every primitive: tests/ops_ref.py.  All tensors fp32 and contiguous unless noted; masks uint8; indices int64.
  * ------------------------------------------------------------------------------------------------------------------------- */
 /* op: 0 a+b, 1 a*b, 2 a*s, 3 relu(a), 4 relu backward (a = dy, b = y), 5 mask ? s : a */

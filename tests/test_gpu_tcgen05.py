@@ -1,4 +1,4 @@
-"""tcgen05 (3xTF32) path: the tensor-core GEMM / LSTM kernels against fp64 references and against the
+"""Tensor-core (wgmma, 3xTF32 / fp16x3) path: the tensor-core GEMM / LSTM kernels against fp64 references and against the
 CUDA-core kernels, then the whole greedy decode with the tensor-core backend against the oracle."""
 import os
 
@@ -26,7 +26,7 @@ def _restore_backend():
 @pytest.mark.parametrize("act", [0, 1])
 @pytest.mark.parametrize("backend", [3, 19])
 def test_linear_tc(M, N, K, act, backend):
-    """backend 3: 3xTF32 (kind::tf32, hi/lo planes); 19 = +16: fp16x3 (kind::f16, fp16 hi/lo with power-of-two operand scales)."""
+    """backend 3: 3xTF32 (tf32 wgmma, hi/lo planes); 19 = +16: fp16x3 (f16 wgmma, fp16 hi/lo with power-of-two operand scales)."""
     capi.set_backend(backend)
     g = torch.Generator().manual_seed(M * 7 + N)
     A = torch.randn(M, K, generator=g)
@@ -71,11 +71,10 @@ experimental = pytest.mark.skipif(os.environ.get("GVD_TEST_EXPERIMENTAL", "0") i
 
 @pytest.mark.parametrize("wide_backend", [7, 23])
 @pytest.mark.parametrize("M,N,K", [(20000, 256, 32), (20000, 512, 1024), (20000, 3096, 1024), (40000, 432, 2048), (10000, 1024, 2780),
-                                   (10000, 2048, 544)])       # every shape gives >= 148 wide CTAs, i.e. takes the BN = 256 path
+                                   (10000, 2048, 544)])       # large M with narrow, wide and ragged N
 @pytest.mark.parametrize("act", [0, 1])
 def test_linear_tc_wide_tiles(M, N, K, act, wide_backend):
-    """backend bit 2: whole 256-column tiles through tc2_gemm_kernel<256> (single accumulator, drain every 16 slices),
-    the column tail through the regular path."""
+    """backend bit 2 (inert: it selected 256-column tiles) must not change the result of large products."""
     capi.set_backend(wide_backend)
     g = torch.Generator().manual_seed(M + N)
     A = torch.randn(M, K, generator=g)
@@ -102,9 +101,9 @@ def _decode_f16x3(img, N, scale):
 @pytest.mark.parametrize("act", [0, 1])
 @pytest.mark.parametrize("ss_backend", [923, 1947])
 def test_linear_f16ss_persistent(M, N, K, act, ss_backend):
-    """The conversion-free persistent prologue GEMM (backend bit 7) on its own, against fp64: C, the fp16x3 image of C its epilogue writes for the
-    next GEMM (backend bit 9: 22 significant bits of the fp32 value, zero padding columns), and the image-only mode.  1947 = 923 + bit 10: the
-    256 x 256 tiles of the CTA-pair kernel (tcgen05 cta_group::2) wherever the single-CTA kernel would use 256-column tiles."""
+    """The conversion-free prologue GEMM (backend bit 7) on its own, against fp64: C, the fp16x3 image of C its epilogue writes for the
+    next GEMM (backend bit 9: 22 significant bits of the fp32 value, zero padding columns), and the image-only mode.  1947 = 923 + bit 10:
+    the same product with the (unused on Hopper) CTA-pair switch set: it must not change the result."""
     capi.set_backend(ss_backend)
     g = torch.Generator().manual_seed(M + 3 * N)
     A = torch.randn(M, K, generator=g)
@@ -188,9 +187,9 @@ def test_fused_self_attention_repeated_launches(att_backend):
 @pytest.mark.parametrize("backend", [0, 1, 3, 7, 11, 15, 19, 27, 31, 59, 91, 155, 411, 923, 1947])
 @pytest.mark.parametrize("name", ["greedy_T10_B4", "greedy_T480_B2", "greedy_small_B5", "greedy_T10_B2_nointeract"])
 def test_greedy_with_both_backends(name, backend):
-    """backend 3 (tcgen05 3xTF32 + fused self-attention, the default), 1 (tcgen05, unfused attention) and 0 (fp32 CUDA
-    cores) all meet the parity bar, and so do the switches on top: bit 2 (+4, 256-column prologue tiles), bit 3 (+8, operand-swapped
-    split-K decode products with the fused reduce + sampler), bit 4 (+16, fp16x3 instead of 3xTF32 in the forward GEMMs), bit 7 (+128, conversion-free persistent prologue GEMMs), bit 8 (+256, fp16x3 images
+    """backend 3 (wgmma 3xTF32 + fused self-attention), 1 (wgmma, unfused attention) and 0 (fp32 CUDA
+    cores) all meet the parity bar, and so do the switches on top: bit 2 (+4, inert), bit 3 (+8, operand-swapped
+    split-K decode products with the fused reduce + sampler), bit 4 (+16, fp16x3 instead of 3xTF32 in the forward GEMMs), bit 7 (+128, conversion-free prologue GEMMs), bit 8 (+256, fp16x3 images
     in the attention pair), bit 9 (+512, producers store the operand image of the next GEMM: 923 is the default)."""
     capi.set_backend(backend)
     opt, sd, inp = build_case(CASES[name])
@@ -204,9 +203,8 @@ def test_greedy_with_both_backends(name, backend):
 
 @pytest.mark.parametrize("backend", [3, 19])
 def test_gemm_repeated_launches_stress(backend):
-    """Ring hand-off stress (ADVICE r1: mbarrier parity aliasing when a ring length is not a multiple of the conversion-group count —
-    closed by static_assert(NRA % NG == 0 && NRB % NG == 0)): 200 launches each of a BN = 128 problem (several waves of CTAs) and of the
-    BN = 32 LSTM-mode kernel at full size, EVERY result checked against fp64 on the device and against the first launch bit for bit."""
+    """Ring hand-off stress (mbarrier phase accounting of the TMA ring): 200 launches each of a large problem (several waves of CTAs) and of the
+    LSTM-mode kernel at full size, EVERY result checked against fp64 on the device and against the first launch bit for bit."""
     capi.set_backend(backend)
     g = torch.Generator().manual_seed(11)
     A = torch.randn(4000, 2048, generator=g).cuda()

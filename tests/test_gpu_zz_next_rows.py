@@ -1,5 +1,5 @@
 """Rows of SURVEY.md 8(f) ("next") built so far, through the C ABI.  The file name sorts last on purpose: these tests were added
-after the last device session of round 1 and must not mask the parity suite if one of them fails."""
+late and must not mask the parity suite if one of them fails."""
 import os
 
 import numpy as np

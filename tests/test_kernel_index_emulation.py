@@ -1,6 +1,5 @@
-"""Thread-level emulation (numpy, on the CPU) of the INDEX ARITHMETIC of the kernels that were written after the last device session
-(csrc/gvd_train.cu, the two grounding kernels of csrc/gvd_losses.cu; the split-K reductions of csrc/gvd_skinny.cu were rewritten in round 2
-and are covered by the device tests instead).  Each emulation below is a literal
+"""Thread-level emulation (numpy, on the CPU) of the INDEX ARITHMETIC of kernels whose indexing is easy to get wrong
+(csrc/gvd_train.cu, the two grounding kernels of csrc/gvd_losses.cu, the epilogues of csrc/gvd_wgmma.cu).  Each emulation below is a literal
 transliteration of the kernel body — same flattened-index expressions, same block / thread decomposition, same shared-memory tile
 phases — run for every (block, thread) of a small launch and compared with the primitive's mathematical definition.  It cannot find
 device-only problems (synchronisation, alignment), but a wrong stride, a swapped axis or an off-by-one tile is caught here instead of
@@ -219,79 +218,67 @@ def test_split_k_as_batch_axis_is_the_full_contraction():
     assert np.allclose(part.sum(0), W @ X.T, atol=1e-4)
 
 
-# ----------------------------------------------------------------------------- round 2, sessions 37 / 38: staged epilogues of the self-attention pair
+# ----------------------------------------------------------------------------- epilogues of wg_gemm_kernel (csrc/gvd_wgmma.cu)
 def _f16x3_word(k_even):
     """gvd_common.cuh::f16x3_word: word of the hi half of the fp16 pair (k, k + 1) inside a row image (32-wide K slices: 16 hi words | 16 lo words)."""
     return (k_even >> 5) * 32 + ((k_even & 31) >> 1)
 
 
-def test_scores_epilogue_staging_is_a_conflict_free_bijection():
-    """tc_astat_kernel's staged epilogue: lane = row writes its 8 sixteen-byte chunks XOR-swizzled by the row, then 8 instructions read 4 rows x 8
-    chunks each.  Every (row, chunk) written is read back exactly once from the same address, and neither phase has a bank conflict inside a
-    quarter-warp (the unit in which 128-bit shared accesses are served)."""
-    tile = {}
-    for lane in range(32):                                   # phase 1: sts128(stg + lane * 128 + ((c ^ (lane & 7)) << 4), v[4c .. 4c + 3])
-        for c in range(8):
-            addr = lane * 128 + ((c ^ (lane & 7)) << 4)
-            assert addr not in tile
-            tile[addr] = (lane, c)
-        # (per instruction c, a quarter-warp's 8 lanes must hit 8 different 16-byte bank groups)
-    for c in range(8):
-        for qw in range(4):
-            groups = {((lane * 128 + ((c ^ (lane & 7)) << 4)) >> 4) & 7 for lane in range(qw * 8, qw * 8 + 8)}
-            assert len(groups) == 8
-    seen = set()
-    for i in range(8):                                        # phase 2: rr = i * 4 + (lane >> 3), chunk c = lane & 7
-        for qw in range(4):
-            groups = set()
-            for lane in range(qw * 8, qw * 8 + 8):
-                rr, c = i * 4 + (lane >> 3), lane & 7
-                addr = rr * 128 + ((c ^ (rr & 7)) << 4)
-                assert tile[addr] == (rr, c)                  # the chunk this lane stores is row rr, columns [4c, 4c + 4)
-                seen.add((rr, c))
-                groups.add((addr >> 4) & 7)
-            assert len(groups) == 8
-    assert len(seen) == 32 * 8
+def test_fragment_to_row_exchange_is_a_bijection():
+    """wg_gemm_kernel's exchange of the wgmma accumulator fragments through shared memory: thread (warpgroup, warp, lane) writes, for each of the
+    8 column blocks j, float2 pairs at rows r0 and r0 + 8; together the 256 consumer threads write every element of the 128 x 64 tile exactly once
+    (pitch 68 words, 8-byte aligned), and the row-per-thread readers (row = (warp & 3) * 32 + lane, column half = warp >> 2) read all of it."""
+    LDS, tile = 68, {}
+    for warp in range(8):
+        wg = warp >> 2
+        for lane in range(32):
+            r0, c0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), 2 * (lane & 3)
+            for j in range(8):
+                for rr, e0 in ((r0, 4 * j), (r0 + 8, 4 * j + 2)):
+                    addr = rr * LDS + 8 * j + c0
+                    assert addr % 2 == 0
+                    for e in range(2):
+                        assert addr + e not in tile
+                        tile[addr + e] = (rr, 8 * j + c0 + e, e0 + e)
+    assert len(tile) == 128 * 64 and all(a == r * LDS + c for a, (r, c, _) in tile.items())
+    read = set()
+    for warp in range(8):
+        for lane in range(32):
+            row, cbeg = (warp & 3) * 32 + lane, (warp >> 2) * 32
+            for j in range(0, 32, 4):
+                assert (row * LDS + cbeg + j) % 4 == 0        # float4 reads
+                read.update(row * LDS + cbeg + j + e for e in range(4))
+    assert read == set(tile)
 
 
 def test_pv_epilogue_image_covers_every_word_of_the_row_once():
-    """tc_pv_kernel's image epilogue (reference-size heads: 6 heads of 171 / 169 columns in slots of 172, tile width 176 in two halves of 88): over
-    all (head, column half, 4-column chunk) the stores of one row write every word of the Wo operand image row [0, rup32(6 * 172) = 1056) exactly once —
-    head columns through the chunk loop, the K padding through the zeroing loop of the last head — with 8-byte aligned word pairs that never straddle
-    a 32-wide K slice; pad columns (n >= N) carry zeros."""
+    """The P.V image epilogue of wg_gemm_kernel (reference-size heads: 6 heads of 171 / 169 columns in slots of 172, padded width 176 = three
+    64-column tiles of two 32-column halves): over all (head, tile, column half, 4-column chunk) the stores of one row write every word of the Wo
+    operand image row [0, rup32(6 * 172) = 1056) exactly once — head columns through the chunk loop, the K padding through the zeroing loop of
+    the last head's first tile — with 8-byte aligned word pairs that never straddle a 32-wide K slice; pad columns (n >= N) carry zeros."""
     nh, sCh, bn, img_ld = 6, 172, 176, 1056
     N = [171] * 5 + [169]
-    half, written, zero_cols = bn // 2, {}, set()
+    slot, written, zero_cols = min(bn, sCh), {}, set()
     for zh in range(nh):
-        for grp in range(2):
-            c0 = grp * half
-            nchunk = half >> 2
-            for ch in range(nchunk):                          # phase 2 of the staged epilogue: chunk ch of this warp's row
-                n = c0 + ch * 4
-                if n >= min(bn, sCh):
-                    continue                                  # columns past the slot belong to the next head's CTA
-                gc = zh * sCh + n
-                assert gc % 4 == 0 and (gc & 31) + 4 <= 32    # the chunk sits inside one K slice
-                w = _f16x3_word(gc)
-                assert w % 2 == 0                             # uint2 stores: 8-byte aligned
-                for d in (w, w + 1, w + 16, w + 17):
-                    assert d not in written and 0 <= d < img_ld
-                    written[d] = (zh, n)
-                zero_cols.update(zh * sCh + n + e for e in range(4) if n + e >= N[zh])
-        if zh == nh - 1:                                      # K padding of the Wo operand: zeros
-            for gc in range(nh * sCh, img_ld, 4):
-                w = _f16x3_word(gc)
-                for d in (w, w + 1, w + 16, w + 17):
-                    assert d not in written
-                    written[d] = "pad"
+        for bx in range(-(-bn // 64)):
+            for cbeg in (0, 32):
+                if zh == nh - 1 and bx == 0 and cbeg == 0:        # K padding of the Wo operand: zeros
+                    for gc in range(nh * sCh, img_ld, 4):
+                        w = _f16x3_word(gc)
+                        for d in (w, w + 1, w + 16, w + 17):
+                            assert d not in written
+                            written[d] = "pad"
+                for j in range(0, 32, 4):
+                    n = bx * 64 + cbeg + j
+                    if n >= slot:
+                        continue                                  # columns past the slot belong to the next head's CTA
+                    gc = zh * sCh + n
+                    assert gc % 4 == 0 and (gc & 31) + 4 <= 32    # the chunk sits inside one K slice
+                    w = _f16x3_word(gc)
+                    assert w % 2 == 0                             # uint2 stores: 8-byte aligned
+                    for d in (w, w + 1, w + 16, w + 17):
+                        assert d not in written and 0 <= d < img_ld
+                        written[d] = (zh, n)
+                    zero_cols.update(zh * sCh + n + e for e in range(4) if n + e >= N[zh])
     assert sorted(written) == list(range(img_ld))
     assert zero_cols == {zh * sCh + n for zh in range(nh) for n in range(N[zh], sCh)}
-    # the staging pitch of phase 1 (half + 4 words) keeps a quarter-warp's 16-byte row writes on 8 different bank groups
-    pitch = half + 4
-    for cc in range(0, half, 4):
-        for qw in range(4):
-            assert len({((lane * pitch + cc) >> 2) & 7 for lane in range(qw * 8, qw * 8 + 8)}) == 8
-    # phase 2 walks the tile as a flat chunk index: every (row, chunk) exactly once
-    nchunk = half >> 2
-    flat = [(f // nchunk, f - (f // nchunk) * nchunk) for lane in range(32) for f in range(lane, 32 * nchunk, 32)]
-    assert sorted(flat) == [(r, c) for r in range(32) for c in range(nchunk)]

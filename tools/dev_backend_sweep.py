@@ -1,8 +1,8 @@
-"""Round-2 bring-up: step time and stage times of the B=100, T=10 greedy decode under the backend switches
-(3 = validated default, +4 = 256-column prologue tiles, +8 = operand-swapped split-K decode products), plus token equality with
-the default.  Usage: python tools/dev_backend_sweep.py 3 7 11 15"""
-import sys, time
-sys.path.insert(0, '/root/repo')
+"""Step time and stage times of the B=100, T=10 greedy decode under the backend switches
+(+8 = operand-swapped split-K decode products), plus token equality with
+the default.  Usage: python tools/dev_backend_sweep.py 3 11 923"""
+import os, sys, time
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from gvd_b200 import capi, synth
 import os

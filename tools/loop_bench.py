@@ -2,7 +2,7 @@
 Process-level switches (GVD_ATTN_RC, GVD_ATTN_TC, GVD_CLIP_CHUNK ...) are read when the workspace is laid out: one process per setting."""
 import os
 import sys
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from gvd_b200 import capi, synth
 B, T = 100, int(sys.argv[1]) if len(sys.argv) > 1 else 10

@@ -1,6 +1,6 @@
 """Profiling aid: B=100, T=10 prologue once, then the greedy loop a few times (kernel-by-kernel with GVD_NO_GRAPH=1).  argv[1] = backend flags."""
-import sys
-sys.path.insert(0, '/root/repo')
+import os, sys
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from gvd_b200 import capi, synth
 be = int(sys.argv[1]) if len(sys.argv) > 1 else 3

@@ -1,6 +1,6 @@
 """Profiling aid: B=100, T=10 prologue once, then the transformer captioner's greedy decode (gvd_tfm_decode_greedy) argv[1] times."""
-import sys
-sys.path.insert(0, '/root/repo')
+import os, sys
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from gvd_b200 import capi, synth
 B, T = 100, 10

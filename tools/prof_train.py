@@ -1,6 +1,6 @@
-"""Profiling aid: one training step (B=100, T=10, dropout off) under ncu's launch list; argv[1] = number of steps after one warm-up."""
-import sys
-sys.path.insert(0, '/root/repo')
+"""Profiling aid: one training step (B=100, T=10, dropout off) (for use under a profiler); argv[1] = number of steps after one warm-up."""
+import os, sys
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 from gvd_b200 import synth
 from gvd_b200.train import Trainer
