@@ -19,7 +19,8 @@ EXPORTS = [
     "gvd_workspace_tensor", "gvd_prologue_fwd", "gvd_decode_greedy", "gvd_decode_step_fwd",
     "gvd_decode_reset_state", "gvd_sample_greedy_host", "gvd_op_linear", "gvd_op_tanh", "gvd_op_kernel_launches",
     "gvd_profile_enable", "gvd_profile_reset", "gvd_profile_count", "gvd_profile_entry",
-    "gvd_op_linear_tc", "gvd_op_linear_f16ss", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
+    "gvd_op_linear_tc", "gvd_op_linear_f16ss", "gvd_op_skinny_partials", "gvd_op_reduce_lstm", "gvd_op_reduce_bias", "gvd_op_reduce_pick",
+    "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
     "gvd_tfm_workspace_bytes", "gvd_tfm_decode_greedy", "gvd_tfm_teacher_fwd",
     "gvd_grounding_extract", "gvd_grounding_eval", "gvd_plan_skinny_splits", "gvd_plan_h2d_chunks", "gvd_workspace_bytes_beam", "gvd_beam_decode", "gvd_workspace_bytes_teacher", "gvd_teacher_fwd",
     # training-step primitives (csrc/gvd_train.cu; bound in train_ops.py)
@@ -86,6 +87,13 @@ def lib():
     L.gvd_plan_h2d_chunks.argtypes = [ci, ci, vp, ci]
     L.gvd_grounding_eval.argtypes = [vp, vp, vp, ci, ci, ci, ctypes.c_float, vp, vp, vp]
     L.gvd_op_lstm_step.argtypes = [ci, ci, vp, ci, vp, i64, vp, ci, vp, i64, vp, vp, vp, vp, vp, ci, vp]
+    L.gvd_op_skinny_partials.argtypes = [vp, ci, ci, vp, i64, ci, ci, ci, vp, ci, vp]
+    L.gvd_op_reduce_lstm.argtypes = [vp, ci, ci, vp, ci, vp, vp, vp, vp, vp, i64, vp, i64, vp, i64, ci, ci, vp, i64, vp, i64, vp]
+    L.gvd_op_reduce_bias.argtypes = [vp, ci, ci, ci, vp, vp, i64, ci, vp]
+    L.gvd_op_reduce_pick.argtypes = [vp, ci, ci, vp, ci, ci, ci, vp, vp, vp, i64, vp, vp, i64, ci, vp, i64, vp, i64, vp]
+    L.gvd_op_greedy_pick.argtypes = [vp, i64, ci, ci, ci, vp, vp, vp, i64, vp, vp, i64, ci, vp]
+    L.gvd_op_logit_pick_tc.argtypes = [vp, i64, vp, i64, vp, ci, ci, ci, ci, vp, ci, vp, vp, vp, i64, vp, vp]
+    L.gvd_op_gru_layer.argtypes = [ci, vp, vp, vp, vp, ci, ci, ci, vp, vp]
     L.gvd_set_backend.argtypes = [ci]
     L.gvd_tfm_workspace_bytes.argtypes = [vp, ci, ci, ci, ci]
     L.gvd_tfm_workspace_bytes.restype = sz
@@ -499,6 +507,91 @@ def op_lstm_step(x0, w0, x1, w1, b1, b2, c_prev, backend):
     check(lib().gvd_op_lstm_step(B, H, p(x0), x0.shape[1], p(w0), w0.stride(0), p(x1), x1.shape[1] if x1 is not None else 0,
                                  p(w1), w1.stride(0) if w1 is not None else 0, p(b1), p(b2), p(c_prev), p(h), p(c), backend, _stream()))
     return h, c
+
+
+def _ptr(t):
+    return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def _pitch(t):
+    """Row pitch of a 2-D view whose rows are dense (a column window of a wider buffer); 0 for None."""
+    if t is None:
+        return 0
+    if t.dim() != 2 or t.stride(1) != 1:
+        raise GvdError("expected a 2-D tensor with dense rows")
+    return t.stride(0)
+
+
+def op_skinny_partials(W, X, S=0, f16_images=False, ldp=None, fill=float("nan")):
+    """Split-K partial planes part [S, B, ldp] of X @ W.T (W [Nw,K] dense, X [B,K] with any row pitch), pre-filled with `fill` so
+    that a caller can see which elements the product wrote.  S = 0: the planned number of splits."""
+    Nw, K = W.shape
+    B = X.shape[0]
+    if S == 0:
+        S = int(lib().gvd_plan_skinny_splits(Nw, K, B))
+        if S < 1:
+            raise GvdError("no split plan for %d x %d weights and %d rows" % (Nw, K, B))
+    ldp = int(ldp or Nw)
+    part = torch.full((S, B, ldp), fill, dtype=torch.float32, device="cuda")
+    check(lib().gvd_op_skinny_partials(_dev(W, torch.float32, "W"), Nw, K, _ptr(X), _pitch(X), B, S, int(bool(f16_images)), _ptr(part), ldp,
+                                       _stream()))
+    return part
+
+
+def op_reduce_lstm(part, c_prev, c_out, h0, h1=None, h2=None, pre=None, bias1=None, bias2=None, pk1=None, pk2=None, pre_div=1):
+    """LSTMCell from partial planes part [S, B, ldp]; h0 / h1 / h2 (fp32) and pk1 / pk2 (fp16x3 words) are [B, H] column windows."""
+    S, B, ldp = part.shape
+    H = c_prev.shape[1]
+    check(lib().gvd_op_reduce_lstm(_ptr(part), S, ldp, _ptr(pre), pre_div, _ptr(bias1), _ptr(bias2), _ptr(c_prev), _ptr(c_out), _ptr(h0), _pitch(h0),
+                                   _ptr(h1), _pitch(h1), _ptr(h2), _pitch(h2), B, H, _ptr(pk1), _pitch(pk1), _ptr(pk2), _pitch(pk2), _stream()))
+
+
+def op_reduce_bias(part, Nw, bias, out):
+    S, B, ldp = part.shape
+    check(lib().gvd_op_reduce_bias(_ptr(part), S, Nw, ldp, _ptr(bias), _ptr(out), _pitch(out), B, _stream()))
+
+
+def _strided_outputs(seq, logp):
+    """seq / logp: 1-D views (a column of a [B, L] buffer) sharing one element stride."""
+    stride = seq.stride(0) if seq is not None else (logp.stride(0) if logp is not None else 1)
+    if seq is not None and logp is not None and seq.stride(0) != logp.stride(0):
+        raise GvdError("seq and logp destinations must share their stride")
+    return stride
+
+
+def op_reduce_pick(part, bias, V, unk, it, seq=None, logp=None, embed=None, xt=None, logits_out=None, xt_pk=None):
+    S, B, ldp = part.shape
+    E = embed.shape[1] if embed is not None else 0
+    check(lib().gvd_op_reduce_pick(_ptr(part), S, ldp, _ptr(bias), B, V, unk, _ptr(it), _ptr(seq), _ptr(logp), _strided_outputs(seq, logp), _ptr(embed),
+                                   _ptr(xt), _pitch(xt), E, _ptr(logits_out), _pitch(logits_out), _ptr(xt_pk), _pitch(xt_pk), _stream()))
+
+
+def op_greedy_pick(logits, unk, it, seq=None, logp=None, embed=None, xt=None):
+    B, V = logits.shape
+    E = embed.shape[1] if embed is not None else 0
+    check(lib().gvd_op_greedy_pick(_ptr(logits), _pitch(logits), B, V, unk, _ptr(it), _ptr(seq), _ptr(logp), _strided_outputs(seq, logp), _ptr(embed),
+                                   _ptr(xt), _pitch(xt), E, _stream()))
+
+
+def op_logit_pick_tc(h, W, bias, unk, it, seq=None, logp=None, embed=None, xt=None):
+    """Vocabulary head h [B,K] @ W [V,K].T + bias with the sampler fused into the GEMM epilogue; xt [B,E] dense."""
+    B, K = h.shape
+    V = W.shape[0]
+    E = embed.shape[1] if embed is not None else 0
+    if xt is not None and _pitch(xt) != E:
+        raise GvdError("logit_pick_tc writes xt with pitch E")
+    check(lib().gvd_op_logit_pick_tc(_ptr(h), _pitch(h), _ptr(W), _pitch(W), _ptr(bias), B, V, K, unk, _ptr(embed), E, _ptr(it), _ptr(seq), _ptr(logp),
+                                     _strided_outputs(seq, logp), _ptr(xt), _stream()))
+
+
+def op_gru_layer(path, gi, Whh, bhh, sample_idx=None):
+    """One bidirectional GRU layer from gi [B,T,6G]; returns out [B,T,2G] (pre-filled with NaN: the layer writes every element)."""
+    B, T, G6 = gi.shape
+    G = G6 // 6
+    out = torch.full((B, T, 2 * G), float("nan"), dtype=torch.float32, device="cuda")
+    check(lib().gvd_op_gru_layer(int(path), _dev(gi, torch.float32, "gi"), _dev(Whh, torch.float32, "Whh"), _dev(bhh, torch.float32, "bhh"),
+                                 _dev(sample_idx, torch.int64, "sample_idx") if sample_idx is not None else None, B, T, G, _ptr(out), _stream()))
+    return out
 
 
 def op_linear(A, W, bias=None, act=0, tc=False):

@@ -874,6 +874,25 @@ static int obj_interact_fwd(const gvd_model* m, const WS& w0, int c0, int B, cud
     return 0;
 }
 
+// One bidirectional GRU layer step by step: gh = W_hh h(t-1) + b_hh of both directions in one batched GEMM, then the pointwise cell.
+// hstate [2 parity][2 dir][B][G] zeroed by the caller, gh [2 dir][B][3G] scratch, whh [2][3G][G], bhh [2][3G].
+static int gru_layer_steps(const float* gi, const float* whh, const float* bhh, float* hstate, float* gh, float* out,
+                           const long long* sample_idx, int B, int T, int G, cudaStream_t st) {
+    for (int s = 0; s < T; ++s) {
+        float* h_prev = hstate + (size_t)(s & 1) * 2 * B * G;
+        float* h_new = hstate + (size_t)((s + 1) & 1) * 2 * B * G;
+        GemmArgs g{};
+        g.A = h_prev; g.lda = G; g.sAb = (long long)B * G;
+        g.W = whh; g.ldw = G; g.sWb = (long long)3 * G * G;
+        g.bias = bhh; g.sBb = 3 * G;
+        g.C = gh; g.ldc = 3 * G; g.sCb = (long long)B * 3 * G;
+        g.M = B; g.N = 3 * G; g.K = G; g.nh = 1; g.alpha = 1.f;
+        GVD_STAGE("frame.gru_hh", gvd_gemm_nt(g, 2, st));
+        GVD_STAGE("frame.gru_pointwise", gvd_gru_pointwise(gi, gh, h_prev, h_new, out, sample_idx, B, T, G, s, st));
+    }
+    return 0;
+}
+
 static int frame_branch_fwd(const gvd_model* m, const WS& w0, int B, int T, const float* segs, const long long* sample_idx,
                             cudaStream_t st) {
     GvdF16Scope f16;
@@ -916,18 +935,7 @@ static int frame_branch_fwd(const gvd_model* m, const WS& w0, int B, int T, cons
                 continue;
             }
         }
-        for (int s = 0; s < T; ++s) {
-            float* h_prev = w.hstate + (size_t)(s & 1) * 2 * B * G;
-            float* h_new = w.hstate + (size_t)((s + 1) & 1) * 2 * B * G;
-            GemmArgs g{};
-            g.A = h_prev; g.lda = G; g.sAb = (long long)B * G;
-            g.W = m->gru_whh[l]; g.ldw = G; g.sWb = (long long)3 * G * G;
-            g.bias = m->gru_bhh[l]; g.sBb = 3 * G;
-            g.C = w.gh; g.ldc = 3 * G; g.sCb = (long long)B * 3 * G;
-            g.M = B; g.N = 3 * G; g.K = G; g.nh = 1; g.alpha = 1.f;
-            GVD_STAGE("frame.gru_hh", gvd_gemm_nt(g, 2, st));
-            GVD_STAGE("frame.gru_pointwise", gvd_gru_pointwise(w.gi, w.gh, h_prev, h_new, out, l == 1 ? sample_idx : nullptr, B, T, G, s, st));
-        }
+        GVD_TRY(gru_layer_steps(w.gi, m->gru_whh[l], m->gru_bhh[l], w.hstate, w.gh, out, l == 1 ? sample_idx : nullptr, B, T, G, st));
     }
     GVD_STAGE("frame.ctx2att", gvd_linear(w.conv, H, m->P("ctx2att.weight"), H, m->P("ctx2att.bias"), w.p_conv, A, (int)BT, A, H, GVD_ACT_NONE, st));
     return 0;
@@ -1228,7 +1236,8 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
     GVD_CHECK_CUDA(cudaMemsetAsync(w.it, 0, (size_t)B * sizeof(long long), st));            // <bos> = 0 (model.py:587-588)
     // The pick kernel also writes the next step's xt = ReLU(embed[token]) (no separate embedding launch).  Folding the whole
     // sampler into the vocabulary-head GEMM epilogue (MODE_PICK of wg_gemm_kernel, last-CTA merge of the per-CTA partials) is
-    // implemented and parity-tested; its merge is a serial chain on one CTA, so it is only used when GVD_FUSED_PICK is set.
+    // implemented and compared with the two other samplers and an fp64 reference in tests/test_gpu_decode_ops.py (through
+    // gvd_op_logit_pick_tc); its merge is a serial chain on one CTA, so the loop only uses it when GVD_FUSED_PICK is set.
     const bool tc = (gvd_backend() & 1) != 0 && H % 8 == 0;
     static const bool fused_pick = getenv("GVD_FUSED_PICK") != nullptr;
     const bool fused = tc && fused_pick && B <= 128;
@@ -1645,6 +1654,95 @@ extern "C" GVD_API int gvd_op_lstm_step(int B, int H, const float* x0, int K0, c
     if (x1) a.seg[1] = LstmSeg{x1, K1, nullptr, 0, w1, ldw1, K1};
     a.bias1 = bias1; a.bias2 = bias2; a.c_prev = c_prev; a.h_out = h_out; a.c_out = c_out; a.B = B; a.H = H;
     return backend ? gvd_lstm_step_tc(a, (cudaStream_t)stream) : gvd_lstm_step(a, (cudaStream_t)stream);
+}
+// The decode step's operand-swapped split-K product on its own: part[s][b][n] = sum over the K range of split s of W[n][k] X[b][k].
+// f16_images = 0: gvd_skinny_splitk (operands split in the kernel, 3xTF32 or fp16x3 by backend bit 4); 1: both operands packed into fp16x3
+// images here and multiplied by the conversion-free gvd_skinny_f16.  S = 0 takes the plan of gvd_skinny_splits.  Test hook.
+extern "C" GVD_API int gvd_op_skinny_partials(const float* W, int Nw, int K, const float* X, int64_t ldx, int B, int S, int f16_images,
+                                              float* part, int ldp, void* stream) {
+    GVD_REQUIRE(W && X && part && Nw > 0 && K > 0 && B >= 1 && B <= 128 && S >= 0, "op_skinny_partials: bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    if (S == 0) S = gvd_skinny_splits(Nw, K, B);
+    GVD_REQUIRE(S >= 1, "op_skinny_partials: no split plan for %d x %d weights and %d rows", Nw, K, B);
+    GvdF16Scope f16;
+    if (!f16_images) return gvd_skinny_splitk(W, Nw, K, X, ldx, B, S, part, ldp, st);
+    GVD_REQUIRE(K % 32 == 0, "op_skinny_partials: operand images need K %% 32 == 0");
+    float *Wi = nullptr, *Xi = nullptr;
+    GVD_CHECK_CUDA(cudaMallocAsync((void**)&Wi, (size_t)Nw * K * 4, st));
+    GVD_CHECK_CUDA(cudaMallocAsync((void**)&Xi, (size_t)B * K * 4, st));
+    int rc = gvd_pack_f16x3(W, K, Nw, K, Wi, K, st, GVD_F16_SW);
+    if (!rc) rc = gvd_pack_f16x3(X, ldx, B, K, Xi, K, st, GVD_F16_SA);
+    if (!rc) rc = gvd_skinny_f16(Wi, K, Nw, Xi, K, B, K, S, part, ldp, st);
+    cudaFreeAsync(Wi, st);
+    cudaFreeAsync(Xi, st);
+    return rc;
+}
+// The three reductions of the split-K partial planes and the CUDA-core sampler with their launchers' own arguments.  Test hooks.
+extern "C" GVD_API int gvd_op_reduce_lstm(const float* part, int S, int ldp, const float* pre, int pre_div, const float* bias1, const float* bias2,
+                                          const float* c_prev, float* c_out, float* h0, int64_t ldh0, float* h1, int64_t ldh1, float* h2,
+                                          int64_t ldh2, int B, int H, float* pk1, int64_t ldpk1, float* pk2, int64_t ldpk2, void* stream) {
+    GVD_REQUIRE(part && c_prev && c_out && h0 && S >= 1 && B >= 1 && H >= 1, "op_reduce_lstm: bad arguments");
+    return gvd_reduce_lstm(part, S, ldp, pre, pre_div, bias1, bias2, c_prev, c_out, h0, ldh0, h1, ldh1, h2, ldh2, B, H, (cudaStream_t)stream, pk1, ldpk1,
+                           pk2, ldpk2);
+}
+extern "C" GVD_API int gvd_op_reduce_bias(const float* part, int S, int Nw, int ldp, const float* bias, float* out, int64_t ld_out, int B,
+                                          void* stream) {
+    GVD_REQUIRE(part && out && S >= 1 && B >= 1 && Nw >= 1, "op_reduce_bias: bad arguments");
+    return gvd_reduce_bias(part, S, Nw, ldp, bias, out, ld_out, B, (cudaStream_t)stream);
+}
+extern "C" GVD_API int gvd_op_reduce_pick(const float* part, int S, int ldp, const float* bias, int B, int V, int unk_idx, int64_t* it_out,
+                                          int64_t* seq_out, float* logp_out, int64_t out_stride, const float* embed, float* xt, int64_t ld_xt,
+                                          int E, float* logits_out, int64_t ld_logits, float* xt_pk, int64_t ld_xt_pk, void* stream) {
+    GVD_REQUIRE(part && S >= 1 && B >= 1 && (!xt || embed), "op_reduce_pick: bad arguments");
+    return gvd_reduce_pick(part, S, ldp, bias, B, V, unk_idx, (long long*)it_out, (long long*)seq_out, logp_out, out_stride, embed, xt, ld_xt, E,
+                           logits_out, ld_logits, (cudaStream_t)stream, xt_pk, ld_xt_pk);
+}
+extern "C" GVD_API int gvd_op_greedy_pick(const float* logits, int64_t ld, int B, int V, int unk_idx, int64_t* it_out, int64_t* seq_out,
+                                          float* logp_out, int64_t out_stride, const float* embed, float* xt, int64_t ld_xt, int E, void* stream) {
+    GVD_REQUIRE(logits && it_out && B >= 1 && (!xt || embed), "op_greedy_pick: bad arguments");
+    return gvd_greedy_pick(logits, ld, B, V, unk_idx, (long long*)it_out, (long long*)seq_out, logp_out, out_stride, embed, xt, E,
+                           (cudaStream_t)stream, ld_xt);
+}
+// Vocabulary head with the sampler in the GEMM epilogue (MODE_PICK of wg_gemm_kernel): the per-CTA partials and the zeroed ticket are
+// allocated here.  Test hook.
+extern "C" GVD_API int gvd_op_logit_pick_tc(const float* h, int64_t ldh, const float* W, int64_t ldw, const float* bias, int B, int V, int K,
+                                            int unk_idx, const float* embed, int E, int64_t* it_out, int64_t* seq_out, float* logp_out,
+                                            int64_t out_stride, float* xt, void* stream) {
+    GVD_REQUIRE(h && W && bias && it_out && B >= 1 && V >= 2 && K > 0 && (!xt || embed), "op_logit_pick_tc: bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    GvdF16Scope f16;
+    const size_t part_bytes = (size_t)gvd_cdiv(V, 64) * B * 8 * sizeof(float);
+    float* part = nullptr;
+    GVD_CHECK_CUDA(cudaMallocAsync((void**)&part, part_bytes + 16, st));
+    int* ticket = reinterpret_cast<int*>(reinterpret_cast<char*>(part) + part_bytes);
+    int rc = 0;
+    if (cudaMemsetAsync(part, 0, part_bytes + 16, st) != cudaSuccess) { gvd_set_error("op_logit_pick_tc: memset failed"); rc = 2; }
+    if (!rc) rc = gvd_logit_pick_tc(h, ldh, W, ldw, bias, B, V, K, unk_idx, part, ticket, (long long*)it_out, (long long*)seq_out, logp_out, out_stride,
+                                    embed, xt, E, st);
+    cudaFreeAsync(part, st);
+    return rc;
+}
+// One bidirectional GRU layer (model.py:150-154) from given input projections gi [B,T,6G]: path 1 = the tensor-core layer (W_hh packed
+// into its fp16x3 image here), path 0 = the per-step GEMM + pointwise loop (gvd_gemm_nt follows the backend switch).  Test hook.
+extern "C" GVD_API int gvd_op_gru_layer(int path, const float* gi, const float* Whh, const float* bhh, const int64_t* sample_idx, int B, int T,
+                                        int G, float* out, void* stream) {
+    GVD_REQUIRE(gi && Whh && bhh && out && B >= 1 && T >= 1 && G >= 4 && G % 4 == 0 && (path == 0 || path == 1), "op_gru_layer: bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    GvdF16Scope f16;
+    const size_t state = (size_t)2 * 2 * B * G, nw = (size_t)6 * G * G, ngh = (size_t)2 * B * 3 * G;
+    float* buf = nullptr;                                           // hstate | h image or gh | W_hh image
+    GVD_CHECK_CUDA(cudaMallocAsync((void**)&buf, (2 * state + (path ? nw : ngh)) * sizeof(float), st));
+    float *hstate = buf, *h_img = buf + state, *tail = buf + 2 * state;
+    int rc = 0;
+    if (path) {
+        rc = gvd_pack_f16x3(Whh, G, 6 * G, G, tail, G, st, GVD_F16_SW);
+        if (!rc) rc = gvd_gru_layer_f16(gi, tail, bhh, hstate, h_img, out, (const long long*)sample_idx, B, T, G, st);
+    } else {
+        if (cudaMemsetAsync(hstate, 0, state * sizeof(float), st) != cudaSuccess) { gvd_set_error("op_gru_layer: memset failed"); rc = 2; }
+        if (!rc) rc = gru_layer_steps(gi, Whh, bhh, hstate, tail, out, (const long long*)sample_idx, B, T, G, st);
+    }
+    cudaFreeAsync(buf, st);
+    return rc;
 }
 // Batched short-K product C[b,h] = A[b,:,h*hs:(h+1)*hs] . W[b,:,h*hs:(h+1)*hs]^T through the A-stationary kernel (the attention-score shape)
 extern "C" GVD_API int gvd_op_scores_tc(const float* A, const float* W, float* C, int nb, int nh, int M, int N, int hs, int64_t ld, void* stream) {

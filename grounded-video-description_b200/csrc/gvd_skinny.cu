@@ -216,6 +216,8 @@ int gvd_reduce_pick(const float* part, int S, int ldp, const float* bias, int B,
                     float* logp_out, long long out_stride, const float* embed, float* xt, long long ld_xt, int E, float* logits_out,
                     long long ld_logits, cudaStream_t st, float* xt_pk, long long ld_xt_pk) {
     GVD_REQUIRE(V >= 2 && V <= PICK_NT * 6 && bias && it_out, "reduce_pick: vocabulary of 2..6144 entries");
+    GVD_REQUIRE(!xt_pk || (xt && E % 2 == 0 && ld_xt_pk % 32 == 0 && ld_xt_pk >= (E + 31) / 32 * 32),
+                "reduce_pick: the packed xt needs an even E and a 32-multiple pitch covering E");
     const long long plane = (long long)B * ldp;
     if (V <= PICK_NT * 2) GVD_CHECK_CUDA(gvd_launch(reduce_pick_kernel<2>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, unk_idx, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, logits_out, ld_logits, xt_pk, ld_xt_pk, GVD_F16_SA));
     else if (V <= PICK_NT * 5) GVD_CHECK_CUDA(gvd_launch(reduce_pick_kernel<5>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, unk_idx, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, logits_out, ld_logits, xt_pk, ld_xt_pk, GVD_F16_SA));

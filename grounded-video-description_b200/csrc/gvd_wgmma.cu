@@ -631,7 +631,8 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                                 const float* pp = p.pk_part + ((long long)cta * p.M + m) * 8;
                                 const float4 a4 = __ldcg(reinterpret_cast<const float4*>(pp));
                                 const float2 b2 = __ldcg(reinterpret_cast<const float2*>(pp + 4));
-                                if (a4.x > M) { S = S * expf(M - a4.x) + a4.y; M = a4.x; } else { S = fmaf(a4.y, expf(a4.x - M), S); }
+                                if (a4.x > M) { S = S * expf(M - a4.x) + a4.y; M = a4.x; }
+                                else if (a4.x > -INFINITY) { S = fmaf(a4.y, expf(a4.x - M), S); }   // a tile of -inf logits adds nothing (its own sum is NaN)
                                 const float cv[2] = {a4.z, b2.x};
                                 const int ci[2] = {__float_as_int(a4.w), __float_as_int(b2.y)};
 #pragma unroll
@@ -642,7 +643,8 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                             }
                             const float lse = M + logf(S);
                             const bool keep = j1 != p.pk_unk;
-                            const long long it = keep ? j1 : j2;
+                            long long it = keep ? j1 : j2;
+                            if ((unsigned long long)it >= (unsigned long long)p.N) it = 0;   // every logit NaN: stay inside the embedding table
                             p.pk_it[m] = it;
                             if (p.pk_seq) p.pk_seq[(long long)m * p.pk_stride] = it;
                             if (p.pk_logp) p.pk_logp[(long long)m * p.pk_stride] = (keep ? t1 : t2) - lse;
@@ -997,6 +999,7 @@ int gvd_gemm_nt_tc(const GemmArgs& g, int batch, cudaStream_t stream) {
     CUtensorMap mA[3], mW[3];
     TcParams p{};
     set_precision(p);
+    if (g.trans_c) std::swap(p.sa, p.sw);   // operand-swapped product: the M side holds the weights, so it takes the weight scale
     GVD_TRY(make_map(&mA[0], g.A, g.K, g.M, g.lda, g.nh, g.sAh, nb, g.sAb, TC_BM, &p.a_mul_h, &p.a_mul_b));
     {
         // fp16x3: a registered constant weight has a pre-split copy (hi | lo halves per 32-wide K slice, gvd_pack_f16x3): stream that one and
@@ -1027,6 +1030,7 @@ int gvd_logit_pick_tc(const float* h, long long ldh, const float* W, long long l
                       const float* embed, float* xt, int E, cudaStream_t stream) {
     GVD_REQUIRE(B >= 1 && B <= TC_BM, "logit_pick: at most %d rows per launch (got %d)", TC_BM, B);
     GVD_REQUIRE(bias && part && ticket && it_out, "logit_pick: null argument");
+    GVD_REQUIRE(!xt || (embed && E % 4 == 0), "logit_pick: the embedding row is copied in 16-byte pieces (E=%d)", E);
     CUtensorMap mA[3], mW[3];
     TcParams p{};
     set_precision(p);

@@ -176,6 +176,35 @@ GVD_API int gvd_op_linear_f16ss(const float* A, int64_t lda, const float* W, int
 GVD_API int gvd_op_lstm_step(int B, int H, const float* x0, int K0, const float* w0, int64_t ldw0, const float* x1, int K1,
                   const float* w1, int64_t ldw1, const float* bias1, const float* bias2, const float* c_prev,
                   float* h_out, float* c_out, int backend, void* stream);
+/* ---- the decode step's default path op by op (tests/test_gpu_decode_ops.py): operand-swapped split-K product, its three reductions,
+ * the three greedy samplers and one bidirectional GRU layer.
+ * Partial planes: part[s][b][n], row pitch ldp >= Nw (ldp % 4 == 0), plane stride B * ldp; columns [Nw, ldp) are never written.
+ * f16_images 0: operands split in the kernel (3xTF32, or fp16x3 with backend bit 4); 1: both operands packed into fp16x3 images first
+ * (the conversion-free product of the default backend).  S = 0: the plan of gvd_plan_skinny_splits.  fp16x3 holds |x| <= 16376 and
+ * |w| <= 255; larger values overflow to inf. */
+GVD_API int gvd_op_skinny_partials(const float* W, int Nw, int K, const float* X, int64_t ldx, int B, int S, int f16_images, float* part,
+                  int ldp, void* stream);
+/* sum of the S planes (ascending s) + pre + biases -> LSTMCell; h to up to three fp32 destinations and two fp16x3 images (H % 32 == 0) */
+GVD_API int gvd_op_reduce_lstm(const float* part, int S, int ldp, const float* pre, int pre_div, const float* bias1, const float* bias2,
+                  const float* c_prev, float* c_out, float* h0, int64_t ldh0, float* h1, int64_t ldh1, float* h2, int64_t ldh2, int B, int H,
+                  float* pk1, int64_t ldpk1, float* pk2, int64_t ldpk2, void* stream);
+GVD_API int gvd_op_reduce_bias(const float* part, int S, int Nw, int ldp, const float* bias, float* out, int64_t ld_out, int B, void* stream);
+/* Samplers (model.py:590-615): top-2 with ties to the lower index, the runner-up if the winner is unk_idx, log-prob of the token taken;
+ * it_out [B]; seq_out / logp_out element b at [b * out_stride] (NULL to skip); xt [B, ld_xt] = ReLU(embed[token]) (NULL to skip), xt_pk
+ * its fp16x3 image.  A row without any finite comparison (all NaN) yields token 0.  reduce_pick: 2 <= V <= 6144. */
+GVD_API int gvd_op_reduce_pick(const float* part, int S, int ldp, const float* bias, int B, int V, int unk_idx, int64_t* it_out,
+                  int64_t* seq_out, float* logp_out, int64_t out_stride, const float* embed, float* xt, int64_t ld_xt, int E,
+                  float* logits_out, int64_t ld_logits, float* xt_pk, int64_t ld_xt_pk, void* stream);
+GVD_API int gvd_op_greedy_pick(const float* logits, int64_t ld, int B, int V, int unk_idx, int64_t* it_out, int64_t* seq_out, float* logp_out,
+                  int64_t out_stride, const float* embed, float* xt, int64_t ld_xt, int E, void* stream);
+/* vocabulary head h [B,K] . W [V,K]^T + bias with the sampler in the GEMM epilogue; B <= 128, E % 4 == 0, xt [B,E] */
+GVD_API int gvd_op_logit_pick_tc(const float* h, int64_t ldh, const float* W, int64_t ldw, const float* bias, int B, int V, int K, int unk_idx,
+                  const float* embed, int E, int64_t* it_out, int64_t* seq_out, float* logp_out, int64_t out_stride, float* xt, void* stream);
+/* one bidirectional GRU layer (model.py:150-154) from its input projections gi [B,T,6G] (b_ih included): Whh [2,3G,G], bhh [2,3G],
+ * sample_idx [B,2] or NULL (output rows t outside [lo, hi) are 0), out [B,T,2G].  path 0: GEMM + pointwise kernel per step (the GEMM
+ * follows the backend switch); path 1: tensor-core layer kernel (B <= 128, G % 32 == 0). */
+GVD_API int gvd_op_gru_layer(int path, const float* gi, const float* Whh, const float* bhh, const int64_t* sample_idx, int B, int T, int G,
+                  float* out, void* stream);
 /* arithmetic backend switches: bit 0 wgmma tensor cores for every GEMM-shaped stage (0 = fp32 CUDA cores); bit 1 fused self-attention pair;
    bit 2 (4) inert; bit 3 (8) operand-swapped split-K decode products with fused
    reduce + sampler; bit 4 (16) fp16x3 instead of 3xTF32 in the forward GEMMs, pre-split weights, conversion-free decode step, tensor-core GRU;
