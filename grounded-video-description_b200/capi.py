@@ -16,11 +16,11 @@ LIB_PATH = os.path.join(_HERE, "libgvd_b200.so")
 EXPORTS = [
     "gvd_last_error", "gvd_version", "gvd_model_create", "gvd_model_destroy", "gvd_model_set_param",
     "gvd_model_num_params", "gvd_model_param_key", "gvd_model_finalize", "gvd_workspace_bytes",
-    "gvd_workspace_tensor", "gvd_prologue_fwd", "gvd_decode_greedy", "gvd_decode_step_fwd",
+    "gvd_workspace_tensor", "gvd_prologue_fwd", "gvd_decode_greedy", "gvd_decode_sample", "gvd_decode_step_fwd",
     "gvd_decode_reset_state", "gvd_sample_greedy_host", "gvd_op_linear", "gvd_op_tanh", "gvd_op_kernel_launches",
     "gvd_profile_enable", "gvd_profile_reset", "gvd_profile_count", "gvd_profile_entry",
     "gvd_op_linear_tc", "gvd_op_linear_f16ss", "gvd_op_skinny_partials", "gvd_op_reduce_lstm", "gvd_op_reduce_bias", "gvd_op_reduce_pick",
-    "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
+    "gvd_op_reduce_sample", "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
     "gvd_tfm_workspace_bytes", "gvd_tfm_decode_greedy", "gvd_tfm_teacher_fwd",
     "gvd_grounding_extract", "gvd_grounding_eval", "gvd_plan_skinny_splits", "gvd_plan_h2d_chunks", "gvd_workspace_bytes_beam", "gvd_beam_decode", "gvd_workspace_bytes_teacher", "gvd_teacher_fwd",
     # training-step primitives (csrc/gvd_train.cu; bound in train_ops.py)
@@ -73,6 +73,7 @@ def lib():
     L.gvd_workspace_tensor.restype = vp
     L.gvd_prologue_fwd.argtypes = [vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, sz, vp, vp]
     L.gvd_decode_greedy.argtypes = [vp, ci, ci, vp, sz, vp, vp, vp, vp, vp]
+    L.gvd_decode_sample.argtypes = [vp, ci, ci, vp, sz, vp, ctypes.c_uint64, ctypes.c_float, vp, vp, vp, vp]
     L.gvd_decode_step_fwd.argtypes = [vp, ci, ci, vp, sz, ci, vp, vp, vp, vp, i64, vp, vp]
     L.gvd_decode_reset_state.argtypes = [vp, ci, ci, vp, sz, vp]
     L.gvd_sample_greedy_host.argtypes = [vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp]
@@ -92,6 +93,7 @@ def lib():
     L.gvd_op_reduce_bias.argtypes = [vp, ci, ci, ci, vp, vp, i64, ci, vp]
     L.gvd_op_reduce_pick.argtypes = [vp, ci, ci, vp, ci, ci, ci, vp, vp, vp, i64, vp, vp, i64, ci, vp, i64, vp, i64, vp]
     L.gvd_op_greedy_pick.argtypes = [vp, i64, ci, ci, ci, vp, vp, vp, i64, vp, vp, i64, ci, vp]
+    L.gvd_op_reduce_sample.argtypes = [vp, ci, ci, vp, ci, ci, ctypes.c_float, ctypes.c_uint64, ci, vp, vp, vp, i64, vp, vp, i64, ci, vp, i64, vp]
     L.gvd_op_logit_pick_tc.argtypes = [vp, i64, vp, i64, vp, ci, ci, ci, ci, vp, ci, vp, vp, vp, i64, vp, vp]
     L.gvd_op_gru_layer.argtypes = [ci, vp, vp, vp, vp, ci, ci, ci, vp, vp]
     L.gvd_set_backend.argtypes = [ci]
@@ -297,6 +299,19 @@ class NativeModel:
         att2 = torch.empty(B, L, self.R, dtype=torch.float32, device="cuda")
         check(self._L.gvd_decode_greedy(self._h, B, T, ctypes.c_void_p(ws.data_ptr()), ws.numel(),
                                         _dev(pnt_mask, torch.uint8, "pnt_mask"), ctypes.c_void_p(seq.data_ptr()),
+                                        ctypes.c_void_p(logp.data_ptr()), ctypes.c_void_p(att2.data_ptr()), _stream()))
+        return seq, logp, att2
+
+    def decode_sample(self, B, T, pnt_mask, seed, temperature=1.0):
+        """Multinomial sampling (sample_max=0): the token of every step drawn from softmax(logits / temperature) with counter-based
+        noise keyed by (seed, row, step); the same shapes as decode_greedy, log-probs untempered.  See gvd_decode_sample."""
+        ws = self.workspace(B, T)
+        L = self.dims.seq_length
+        seq = torch.empty(B, L, dtype=torch.int64, device="cuda")
+        logp = torch.empty(B, L, dtype=torch.float32, device="cuda")
+        att2 = torch.empty(B, L, self.R, dtype=torch.float32, device="cuda")
+        check(self._L.gvd_decode_sample(self._h, B, T, ctypes.c_void_p(ws.data_ptr()), ws.numel(), _dev(pnt_mask, torch.uint8, "pnt_mask"),
+                                        int(seed) & 0xFFFFFFFFFFFFFFFF, float(temperature), ctypes.c_void_p(seq.data_ptr()),
                                         ctypes.c_void_p(logp.data_ptr()), ctypes.c_void_p(att2.data_ptr()), _stream()))
         return seq, logp, att2
 
@@ -564,6 +579,15 @@ def op_reduce_pick(part, bias, V, unk, it, seq=None, logp=None, embed=None, xt=N
     E = embed.shape[1] if embed is not None else 0
     check(lib().gvd_op_reduce_pick(_ptr(part), S, ldp, _ptr(bias), B, V, unk, _ptr(it), _ptr(seq), _ptr(logp), _strided_outputs(seq, logp), _ptr(embed),
                                    _ptr(xt), _pitch(xt), E, _ptr(logits_out), _pitch(logits_out), _ptr(xt_pk), _pitch(xt_pk), _stream()))
+
+
+def op_reduce_sample(part, bias, V, temperature, seed, step, it, seq=None, logp=None, embed=None, xt=None, xt_pk=None):
+    """The multinomial sampler on partial planes part [S, B, ldp] (+ bias or None) at decode step `step`."""
+    S, B, ldp = part.shape
+    E = embed.shape[1] if embed is not None else 0
+    check(lib().gvd_op_reduce_sample(_ptr(part), S, ldp, _ptr(bias), B, V, float(temperature), int(seed) & 0xFFFFFFFFFFFFFFFF, int(step), _ptr(it),
+                                     _ptr(seq), _ptr(logp), _strided_outputs(seq, logp), _ptr(embed), _ptr(xt), _pitch(xt), E, _ptr(xt_pk),
+                                     _pitch(xt_pk), _stream()))
 
 
 def op_greedy_pick(logits, unk, it, seq=None, logp=None, embed=None, xt=None):

@@ -3,6 +3,7 @@
 #include <atomic>
 #include <mutex>
 #include <chrono>
+#include <cmath>
 #include <cstdarg>
 #include <cstdlib>
 #include <cstring>
@@ -181,6 +182,7 @@ __global__ void bn_affine_kernel(const float* w, const float* b, const float* me
 
 // ------------------------------------------------------------------------------------ model
 struct Param { std::string key; size_t numel; size_t off; bool set; };
+struct LoopKey { int B, T, backend; void* ws; size_t ws_bytes; };   // what a captured decode loop depends on
 
 struct gvd_model {
     gvd_dims_t d;
@@ -211,8 +213,13 @@ struct gvd_model {
     // cudaGraphLaunch (no per-launch host cost, back-to-back scheduling on the device)
     cudaStream_t capture_stream = nullptr;
     cudaGraphExec_t greedy_exec = nullptr;
-    struct { int B, T, backend; void* ws; size_t ws_bytes; } greedy_key{0, 0, 0, nullptr, 0};
+    LoopKey greedy_key{0, 0, 0, nullptr, 0};
     long long greedy_nodes = 0;      // kernel launches inside one replay (counted while capturing)
+    // the multinomial-sampling loop has a graph of its own (alternating greedy and sampling calls re-capture neither); its seed and
+    // temperature are read from the workspace, so a new draw replays the same graph
+    cudaGraphExec_t sample_exec = nullptr;
+    LoopKey sample_key{0, 0, 0, nullptr, 0};
+    long long sample_nodes = 0;
 
     float* P(const std::string& k) const {
         auto it = index.find(k);
@@ -364,6 +371,7 @@ extern "C" GVD_API void gvd_model_destroy(gvd_model_t* m) {
     if (m->ev_fork) cudaEventDestroy(m->ev_fork);
     if (m->ev_join) cudaEventDestroy(m->ev_join);
     if (m->greedy_exec) cudaGraphExecDestroy(m->greedy_exec);
+    if (m->sample_exec) cudaGraphExecDestroy(m->sample_exec);
     if (m->capture_stream) cudaStreamDestroy(m->capture_stream);
     delete m;
 }
@@ -531,6 +539,7 @@ struct WS {
     float* h_img;                      // [2 parity][2 dir][B][G] words: fp16x3 images of the GRU state (tensor-core step kernel)
     int* ticket;                       // [rows] last-CTA tickets of the fused attention combine
     float* pk_part; int* pk_ticket;    // fused vocabulary head + greedy pick: per-CTA partials, one ticket
+    GvdSampleParams* sample_par;       // seed + temperature of the multinomial sampler, copied in before each decode
     // beam search (rows = B * beam)
     BeamBufs bb;
     int* bos_att;
@@ -651,6 +660,8 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     w.ticket = (int*)take(BD * 4);
     w.pk_part = (float*)take((size_t)gvd_cdiv(d.vocab_size, 32) * 128 * 8 * 4);
     w.pk_ticket = (int*)take(256);
+    // the sampler's parameter block shares the ticket's slot: the workspace keeps the size and layout it has without sampling
+    w.sample_par = (GvdSampleParams*)((char*)w.pk_ticket + 128);
     if (beam > 1) {
         const size_t L = d.seq_length, K = beam;
         w.bb.seq = (int*)take((size_t)B * L * K * 4);
@@ -1225,10 +1236,12 @@ extern "C" GVD_API int gvd_decode_step_fwd(gvd_model_t* m, int B, int T, void* w
     return 0;
 }
 
-// S1: the 21-iteration greedy loop (model.py:579-624) enqueued on `st`; every pointer is fixed for a given workspace, so the
-// whole enqueue is capturable as a CUDA graph.
+// S1: the 21-iteration decode loop (model.py:579-624) enqueued on `st`; every pointer is fixed for a given workspace, so the
+// whole enqueue is capturable as a CUDA graph.  sample == nullptr: greedy (top-2 + UNK rule, sample_max = 1); otherwise multinomial
+// sampling (sample_max = 0) with the seed and temperature the kernels read from the parameter block `sample`.
 static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void* workspace, size_t workspace_bytes, const uint8_t* pnt_mask,
-                                 int64_t* seq_out, float* logprobs_out, float* att2_logits_out, cudaStream_t st) {
+                                 int64_t* seq_out, float* logprobs_out, float* att2_logits_out, cudaStream_t st,
+                                 const GvdSampleParams* sample = nullptr) {
     GvdF16Scope f16;
     const gvd_dims_t& d = m->d;
     const int H = d.rnn_size, V = d.vocab_size, L = d.seq_length, R = m->R;
@@ -1240,7 +1253,7 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
     // gvd_op_logit_pick_tc); its merge is a serial chain on one CTA, so the loop only uses it when GVD_FUSED_PICK is set.
     const bool tc = (gvd_backend() & 1) != 0 && H % 8 == 0;
     static const bool fused_pick = getenv("GVD_FUSED_PICK") != nullptr;
-    const bool fused = tc && fused_pick && B <= 128;
+    const bool fused = tc && fused_pick && B <= 128 && !sample;     // the fused head has no multinomial sampler: sampling takes the split-K path
     for (int t = 0; t < L; ++t) {
         GVD_TRY(core_step(m, w, B, T, t, w.it, pnt_mask, pnt_mask, att2_logits_out + (size_t)t * R, (long long)L * R, st, 1, 0, tc && t > 0));
         const float* h = w.h_lang + (size_t)((t + 1) & 1) * B * H;
@@ -1262,16 +1275,66 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
                     GVD_REQUIRE(!sk16, "decode: packed vocabulary-head weights missing");
                     GVD_STAGE("decode.logit", gvd_skinny_splitk(m->P("logit.weight"), V, H, h, H, B, S, w.sk_part, m->Vp, st));
                 }
-                GVD_STAGE("decode.pick", gvd_reduce_pick(w.sk_part, S, m->Vp, m->P("logit.bias"), B, V, d.unk_idx, w.it, (long long*)seq_out + t,
-                                                         logprobs_out ? logprobs_out + t : nullptr, L, m->P("embed.0.weight"), sk_core ? w.xcat_att : w.xt,
-                                                         sk_core ? E + H : E, E, nullptr, 0, st, sk16 ? w.xp_att : nullptr, E + H));
+                if (sample) {
+                    GVD_STAGE("decode.sample", gvd_reduce_sample(w.sk_part, S, m->Vp, m->P("logit.bias"), B, V, sample, t, w.it, (long long*)seq_out + t,
+                                                                 logprobs_out ? logprobs_out + t : nullptr, L, m->P("embed.0.weight"),
+                                                                 sk_core ? w.xcat_att : w.xt, sk_core ? E + H : E, E, st, sk16 ? w.xp_att : nullptr, E + H));
+                } else {
+                    GVD_STAGE("decode.pick", gvd_reduce_pick(w.sk_part, S, m->Vp, m->P("logit.bias"), B, V, d.unk_idx, w.it, (long long*)seq_out + t,
+                                                             logprobs_out ? logprobs_out + t : nullptr, L, m->P("embed.0.weight"), sk_core ? w.xcat_att : w.xt,
+                                                             sk_core ? E + H : E, E, nullptr, 0, st, sk16 ? w.xp_att : nullptr, E + H));
+                }
             } else {
                 GVD_STAGE("decode.logit", gvd_linear(h, H, m->P("logit.weight"), H, m->P("logit.bias"), w.logits, m->Vp, B, V, H, GVD_ACT_NONE, st));
-                GVD_STAGE("decode.pick", gvd_greedy_pick(w.logits, m->Vp, B, V, d.unk_idx, w.it, (long long*)seq_out + t, logprobs_out ? logprobs_out + t : nullptr,
-                                                         L, tc ? m->P("embed.0.weight") : nullptr, tc ? (sk_core ? w.xcat_att : w.xt) : nullptr, E, st, sk_core ? E + H : E));
+                if (sample) {   // the logits already hold the bias: one plane, no bias
+                    GVD_STAGE("decode.sample", gvd_reduce_sample(w.logits, 1, m->Vp, nullptr, B, V, sample, t, w.it, (long long*)seq_out + t,
+                                                                 logprobs_out ? logprobs_out + t : nullptr, L, tc ? m->P("embed.0.weight") : nullptr,
+                                                                 tc ? (sk_core ? w.xcat_att : w.xt) : nullptr, sk_core ? E + H : E, E, st));
+                } else {
+                    GVD_STAGE("decode.pick", gvd_greedy_pick(w.logits, m->Vp, B, V, d.unk_idx, w.it, (long long*)seq_out + t, logprobs_out ? logprobs_out + t : nullptr,
+                                                             L, tc ? m->P("embed.0.weight") : nullptr, tc ? (sk_core ? w.xcat_att : w.xt) : nullptr, E, st, sk_core ? E + H : E));
+                }
             }
         }
     }
+    return 0;
+}
+
+// The decode loop through its captured graph: built on the first call for (B, T, backend, workspace) and replayed afterwards.
+static int decode_loop_run(gvd_model_t* m, const WS& w, int B, int T, void* workspace, size_t workspace_bytes, const uint8_t* pnt_mask,
+                           int64_t* seq_out, float* logprobs_out, float* att2_logits_out, cudaStream_t st, const GvdSampleParams* sample,
+                           cudaGraphExec_t& exec, LoopKey& key, long long& nodes) {
+    const int L = m->d.seq_length, R = m->R;
+    // Direct enqueue when the stage profiler is on (its events cannot be captured) or when asked (GVD_NO_GRAPH: per-kernel profiling)
+    static const bool no_graph = getenv("GVD_NO_GRAPH") != nullptr;
+    if (no_graph || g_prof_on.load(std::memory_order_relaxed) != 0)
+        return decode_greedy_enqueue(m, w, B, T, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_logits_out, st, sample);
+    // Graph path: the loop reads the mask from / writes its results to workspace-resident buffers (fixed addresses), the caller's
+    // tensors are copied in / out around the replay.
+    if (!exec || key.B != B || key.T != T || key.backend != gvd_backend() || key.ws != workspace || key.ws_bytes != workspace_bytes) {
+        if (exec) { cudaGraphExecDestroy(exec); exec = nullptr; }
+        if (!m->capture_stream) GVD_CHECK_CUDA(cudaStreamCreateWithFlags(&m->capture_stream, cudaStreamNonBlocking));
+        cudaGraph_t graph = nullptr;
+        GVD_CHECK_CUDA(cudaStreamBeginCapture(m->capture_stream, cudaStreamCaptureModeThreadLocal));
+        const long long l0 = g_launches.load();
+        const int rc = decode_greedy_enqueue(m, w, B, T, workspace, workspace_bytes, w.in_mask, (int64_t*)w.out_seq, w.out_logp, w.out_att2,
+                                             m->capture_stream, sample);
+        const cudaError_t ce = cudaStreamEndCapture(m->capture_stream, &graph);
+        nodes = g_launches.load() - l0;
+        g_launches.store(l0);                              // capturing launches nothing
+        if (rc != 0) { if (graph) cudaGraphDestroy(graph); return rc; }
+        GVD_CHECK_CUDA(ce);
+        const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
+        cudaGraphDestroy(graph);
+        GVD_CHECK_CUDA(ie);
+        key = {B, T, gvd_backend(), workspace, workspace_bytes};
+    }
+    if (pnt_mask != w.in_mask) GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_mask, pnt_mask, (size_t)B * (R + 1), cudaMemcpyDeviceToDevice, st));
+    GVD_CHECK_CUDA(cudaGraphLaunch(exec, st));
+    g_launches.fetch_add(nodes, std::memory_order_relaxed);
+    if (seq_out != (int64_t*)w.out_seq) GVD_CHECK_CUDA(cudaMemcpyAsync(seq_out, w.out_seq, (size_t)B * L * 8, cudaMemcpyDeviceToDevice, st));
+    if (logprobs_out && logprobs_out != w.out_logp) GVD_CHECK_CUDA(cudaMemcpyAsync(logprobs_out, w.out_logp, (size_t)B * L * 4, cudaMemcpyDeviceToDevice, st));
+    if (att2_logits_out != w.out_att2) GVD_CHECK_CUDA(cudaMemcpyAsync(att2_logits_out, w.out_att2, (size_t)B * L * R * 4, cudaMemcpyDeviceToDevice, st));
     return 0;
 }
 
@@ -1280,39 +1343,23 @@ extern "C" GVD_API int gvd_decode_greedy(gvd_model_t* m, int B, int T, void* wor
     WS w;
     GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
     GVD_REQUIRE(pnt_mask && seq_out && att2_logits_out, "decode_greedy: null argument");
+    return decode_loop_run(m, w, B, T, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_logits_out, (cudaStream_t)stream, nullptr,
+                           m->greedy_exec, m->greedy_key, m->greedy_nodes);
+}
+
+extern "C" GVD_API int gvd_decode_sample(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes, const uint8_t* pnt_mask,
+                                 uint64_t seed, float temperature, int64_t* seq_out, float* logprobs_out, float* att2_logits_out, void* stream) {
+    WS w;
+    GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
+    GVD_REQUIRE(pnt_mask && seq_out && att2_logits_out, "decode_sample: null argument");
+    GVD_REQUIRE(std::isfinite(temperature) && temperature > 0.f, "decode_sample: temperature must be finite and > 0 (got %g)", (double)temperature);
+    GVD_REQUIRE(m->d.vocab_size <= 6144, "decode_sample: the sampler holds a vocabulary of at most 6144 words (got %d)", m->d.vocab_size);
     cudaStream_t st = (cudaStream_t)stream;
-    const int L = m->d.seq_length, R = m->R;
-    // Direct enqueue when the stage profiler is on (its events cannot be captured) or when asked (GVD_NO_GRAPH: per-kernel profiling)
-    static const bool no_graph = getenv("GVD_NO_GRAPH") != nullptr;
-    if (no_graph || g_prof_on.load(std::memory_order_relaxed) != 0)
-        return decode_greedy_enqueue(m, w, B, T, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_logits_out, st);
-    // Graph path: the loop reads the mask from / writes its results to workspace-resident buffers (fixed addresses), the caller's
-    // tensors are copied in / out around the replay.
-    if (!m->greedy_exec || m->greedy_key.B != B || m->greedy_key.T != T || m->greedy_key.backend != gvd_backend() || m->greedy_key.ws != workspace ||
-        m->greedy_key.ws_bytes != workspace_bytes) {
-        if (m->greedy_exec) { cudaGraphExecDestroy(m->greedy_exec); m->greedy_exec = nullptr; }
-        if (!m->capture_stream) GVD_CHECK_CUDA(cudaStreamCreateWithFlags(&m->capture_stream, cudaStreamNonBlocking));
-        cudaGraph_t graph = nullptr;
-        GVD_CHECK_CUDA(cudaStreamBeginCapture(m->capture_stream, cudaStreamCaptureModeThreadLocal));
-        const long long l0 = g_launches.load();
-        const int rc = decode_greedy_enqueue(m, w, B, T, workspace, workspace_bytes, w.in_mask, (int64_t*)w.out_seq, w.out_logp, w.out_att2, m->capture_stream);
-        const cudaError_t ce = cudaStreamEndCapture(m->capture_stream, &graph);
-        m->greedy_nodes = g_launches.load() - l0;
-        g_launches.store(l0);                              // capturing launches nothing
-        if (rc != 0) { if (graph) cudaGraphDestroy(graph); return rc; }
-        GVD_CHECK_CUDA(ce);
-        const cudaError_t ie = cudaGraphInstantiate(&m->greedy_exec, graph, 0);
-        cudaGraphDestroy(graph);
-        GVD_CHECK_CUDA(ie);
-        m->greedy_key = {B, T, gvd_backend(), workspace, workspace_bytes};
-    }
-    if (pnt_mask != w.in_mask) GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_mask, pnt_mask, (size_t)B * (R + 1), cudaMemcpyDeviceToDevice, st));
-    GVD_CHECK_CUDA(cudaGraphLaunch(m->greedy_exec, st));
-    g_launches.fetch_add(m->greedy_nodes, std::memory_order_relaxed);
-    if (seq_out != (int64_t*)w.out_seq) GVD_CHECK_CUDA(cudaMemcpyAsync(seq_out, w.out_seq, (size_t)B * L * 8, cudaMemcpyDeviceToDevice, st));
-    if (logprobs_out && logprobs_out != w.out_logp) GVD_CHECK_CUDA(cudaMemcpyAsync(logprobs_out, w.out_logp, (size_t)B * L * 4, cudaMemcpyDeviceToDevice, st));
-    if (att2_logits_out != w.out_att2) GVD_CHECK_CUDA(cudaMemcpyAsync(att2_logits_out, w.out_att2, (size_t)B * L * R * 4, cudaMemcpyDeviceToDevice, st));
-    return 0;
+    // the parameter block is copied in on the caller's stream ahead of the loop (pageable source: staged before this call returns)
+    const GvdSampleParams par{(uint32_t)(seed & 0xffffffffull), (uint32_t)(seed >> 32), temperature, 0u};
+    GVD_CHECK_CUDA(cudaMemcpyAsync(w.sample_par, &par, sizeof(par), cudaMemcpyHostToDevice, st));
+    return decode_loop_run(m, w, B, T, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_logits_out, st, w.sample_par,
+                           m->sample_exec, m->sample_key, m->sample_nodes);
 }
 
 namespace {
@@ -1696,6 +1743,22 @@ extern "C" GVD_API int gvd_op_reduce_pick(const float* part, int S, int ldp, con
     GVD_REQUIRE(part && S >= 1 && B >= 1 && (!xt || embed), "op_reduce_pick: bad arguments");
     return gvd_reduce_pick(part, S, ldp, bias, B, V, unk_idx, (long long*)it_out, (long long*)seq_out, logp_out, out_stride, embed, xt, ld_xt, E,
                            logits_out, ld_logits, (cudaStream_t)stream, xt_pk, ld_xt_pk);
+}
+extern "C" GVD_API int gvd_op_reduce_sample(const float* part, int S, int ldp, const float* bias, int B, int V, float temperature, uint64_t seed,
+                                            int step, int64_t* it_out, int64_t* seq_out, float* logp_out, int64_t out_stride, const float* embed,
+                                            float* xt, int64_t ld_xt, int E, float* xt_pk, int64_t ld_xt_pk, void* stream) {
+    GVD_REQUIRE(part && S >= 1 && B >= 1 && (!xt || embed), "op_reduce_sample: bad arguments");
+    GVD_REQUIRE(std::isfinite(temperature) && temperature > 0.f, "op_reduce_sample: temperature must be finite and > 0 (got %g)", (double)temperature);
+    cudaStream_t st = (cudaStream_t)stream;
+    const GvdSampleParams par{(uint32_t)(seed & 0xffffffffull), (uint32_t)(seed >> 32), temperature, 0u};
+    GvdSampleParams* dpar = nullptr;
+    GVD_CHECK_CUDA(cudaMallocAsync((void**)&dpar, sizeof(par), st));
+    int rc = 0;
+    if (cudaMemcpyAsync(dpar, &par, sizeof(par), cudaMemcpyHostToDevice, st) != cudaSuccess) { gvd_set_error("op_reduce_sample: copy failed"); rc = 2; }
+    if (!rc) rc = gvd_reduce_sample(part, S, ldp, bias, B, V, dpar, step, (long long*)it_out, (long long*)seq_out, logp_out, out_stride, embed, xt, ld_xt,
+                                    E, st, xt_pk, ld_xt_pk);
+    cudaFreeAsync(dpar, st);
+    return rc;
 }
 extern "C" GVD_API int gvd_op_greedy_pick(const float* logits, int64_t ld, int B, int V, int unk_idx, int64_t* it_out, int64_t* seq_out,
                                           float* logp_out, int64_t out_stride, const float* embed, float* xt, int64_t ld_xt, int E, void* stream) {

@@ -91,6 +91,19 @@ __device__ __forceinline__ float ex2_approx(float x) {
 }
 __device__ __forceinline__ float sigmoid_acc(float x) { return 1.f / (1.f + expf(-x)); }
 
+// ---------------------------------------------------------------- counter-based random numbers (train-mode dropout, multinomial sampler)
+// Philox4x32-10 (Salmon et al., SC'11): four 32-bit words from a 128-bit counter and a 64-bit key, no state.
+__device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1, uint32_t out[4]) {
+#pragma unroll
+    for (int r = 0; r < 10; ++r) {
+        const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
+        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
+        c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
+        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
+    }
+    out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
+}
+
 // ---------------------------------------------------------------- fp16x3 operand image (gvd_wgmma.cu: skinny_f16_kernel, pre-split weights)
 // A row of K fp32 values is stored as K 32-bit words: per 32-wide K slice 16 words of hi pairs (k = 2p, 2p + 1 in word p, low half = even k)
 // followed by 16 words of lo pairs; hi = the value rounded to 11 significant bits (exact in fp16), lo = fp16(value - hi); values are

@@ -98,6 +98,11 @@ int gvd_reduce_bias(const float* part, int S, int Nw, int ldp, const float* bias
 int gvd_reduce_pick(const float* part, int S, int ldp, const float* bias, int B, int V, int unk_idx, long long* it_out, long long* seq_out,
                     float* logp_out, long long out_stride, const float* embed, float* xt, long long ld_xt, int E, float* logits_out,
                     long long ld_logits, cudaStream_t st, float* xt_pk = nullptr, long long ld_xt_pk = 0);
+// parameter block of the multinomial sampler, device-resident (a captured decode loop replays with a new seed / temperature)
+struct GvdSampleParams { uint32_t seed_lo, seed_hi; float temperature; uint32_t pad; };
+int gvd_reduce_sample(const float* part, int S, int ldp, const float* bias, int B, int V, const GvdSampleParams* params, int step,
+                      long long* it_out, long long* seq_out, float* logp_out, long long out_stride, const float* embed, float* xt,
+                      long long ld_xt, int E, cudaStream_t st, float* xt_pk = nullptr, long long ld_xt_pk = 0);
 int gvd_gemm_nt_tc(const GemmArgs& g, int batch, cudaStream_t stream);
 int gvd_gemm_nt_astat(const GemmArgs& g, int batch, cudaStream_t stream);   // short-K (<= 192), one K pass
 // self-attention pair (W operands pre-split into tf32 hi / lo planes): softmax-numerator scores + group factors F, then (F (.) E) V

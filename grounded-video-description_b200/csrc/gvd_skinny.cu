@@ -12,6 +12,8 @@
 //                    slots of the concatenated inputs of the next products), c                                (AttModel.py:139,160)
 //   reduce_bias      out[b][n] = sum_s part[s][b][n] + bias[n]                                                 (attention queries)
 //   reduce_pick      vocabulary head: sum_s + bias -> log-softmax, top-2, UNK rule, next token + its embedding  (model.py:590-615)
+//   reduce_sample    vocabulary head: sum_s + bias -> multinomial draw at a temperature (Gumbel-max), next token + its embedding
+//                                                                                                              (model.py:595-605)
 #include "gvd_common.cuh"
 #include "gvd_kernels.cuh"
 
@@ -164,6 +166,107 @@ __global__ void __launch_bounds__(PICK_NT) reduce_pick_kernel(const float* __res
     }
 }
 
+// Multinomial sampling (sample_max = 0, model.py:595-603): it ~ softmax(logit / temperature), drawn with the Gumbel-max trick
+//   it = argmax_i (logit_i / temperature + g_i),  g_i = -log(-log(u_i)),  ties -> lower index,
+//   logp = logit_it - logsumexp(logit)                    (untempered, model.py:602; no UNK rule in this branch)
+// u_i for batch row b, decode step t: word (i & 3) of Philox4x32-10(counter = (i >> 2, b, t, 0), key = seed), u = ((word >> 9) + 0.5) 2^-23:
+// 23-bit uniforms strictly inside (0, 1), exact in fp32, so g lies in [-2.82, 16.64] and a word whose key is more than ~19.5 below the
+// best is never drawn (its probability is < 1e-8).  b is the row's index in THIS launch: splitting a batch changes the draws.
+// A row whose keys are all -inf or all NaN yields token 0.
+__device__ __forceinline__ float gumbel_from_word(uint32_t w) {
+    const float u = ((float)(w >> 9) + 0.5f) * (1.f / 8388608.f);
+    return -logf(-logf(u));
+}
+struct ArgKey { float key, logit; int i; };
+__device__ __forceinline__ void argkey_merge(ArgKey& a, float key, float logit, int i) {
+    if (key > a.key || (key == a.key && i < a.i)) { a.key = key; a.logit = logit; a.i = i; }
+}
+template <int NPT>
+__global__ void __launch_bounds__(PICK_NT) reduce_sample_kernel(const float* __restrict__ part, int S, long long plane, int ldp, const float* __restrict__ bias,
+                                                            int V, const GvdSampleParams* __restrict__ par, int step, long long* __restrict__ it_out,
+                                                            long long* __restrict__ seq_out, float* __restrict__ logp_out, long long out_stride,
+                                                            const float* __restrict__ embed, float* __restrict__ xt, long long ld_xt, int E,
+                                                            float* __restrict__ xt_pk, long long ld_xt_pk, float pk_scale) {
+    __shared__ __align__(16) float gum[PICK_NT * NPT];
+    __shared__ float red[32];
+    __shared__ ArgKey wbest[32];
+    __shared__ float wmax[32];
+    __shared__ int tok_s;
+    const int b = blockIdx.x, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    pdl_trigger();
+    // the noise depends on nothing the decode loop writes: drawn before waiting for the previous kernel
+    const uint32_t seed_lo = par->seed_lo, seed_hi = par->seed_hi;
+    const float temperature = par->temperature;
+    for (int q = threadIdx.x; 4 * q < V; q += PICK_NT) {
+        uint32_t r[4];
+        philox4x32_10((uint32_t)q, (uint32_t)b, (uint32_t)step, 0u, seed_lo, seed_hi, r);
+        reinterpret_cast<float4*>(gum)[q] = make_float4(gumbel_from_word(r[0]), gumbel_from_word(r[1]), gumbel_from_word(r[2]), gumbel_from_word(r[3]));
+    }
+    pdl_wait();
+    __syncthreads();
+    const float* p = part + (long long)b * ldp;
+    float x[NPT];
+    ArgKey a{-INFINITY, -INFINITY, 0x7fffffff};
+    float m = -INFINITY;
+#pragma unroll
+    for (int k = 0; k < NPT; ++k) {
+        const int i = threadIdx.x + k * PICK_NT;
+        float v = -INFINITY;
+        if (i < V) {
+            v = p[i];
+            for (int s = 1; s < S; ++s) v += p[i + s * plane];
+            if (bias) v += __ldg(bias + i);
+            m = fmaxf(m, v);
+            argkey_merge(a, v / temperature + gum[i], v, i);
+        }
+        x[k] = v;
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ok = __shfl_xor_sync(0xffffffffu, a.key, o), ol = __shfl_xor_sync(0xffffffffu, a.logit, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, a.i, o);
+        argkey_merge(a, ok, ol, oi);
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    }
+    if (lane == 0) { wbest[warp] = a; wmax[warp] = m; }
+    __syncthreads();
+    a = wbest[lane];                                             // every warp merges the 32 warp results the same way (fixed order)
+    m = wmax[lane];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ok = __shfl_xor_sync(0xffffffffu, a.key, o), ol = __shfl_xor_sync(0xffffffffu, a.logit, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, a.i, o);
+        argkey_merge(a, ok, ol, oi);
+        m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    }
+    float s = 0.f;
+#pragma unroll
+    for (int k = 0; k < NPT; ++k) s += (threadIdx.x + k * PICK_NT < V) ? expf(x[k] - m) : 0.f;
+    s = block_sum(s, red);
+    if (threadIdx.x == 0) {
+        int it = a.i;
+        if ((unsigned)it >= (unsigned)V) it = 0;                 // every key NaN: stay inside the embedding table
+        it_out[b] = it;
+        if (seq_out) seq_out[(long long)b * out_stride] = it;
+        if (logp_out) logp_out[(long long)b * out_stride] = a.logit - (m + logf(s));
+        tok_s = it;
+    }
+    if (xt) {                                                    // next step's input xt = ReLU(embed[token]) (model.py:79-82,605)
+        __syncthreads();
+        const float* row = embed + (long long)tok_s * E;
+        for (int e = threadIdx.x; e < E; e += blockDim.x) xt[(long long)b * ld_xt + e] = fmaxf(row[e], 0.f);
+        if (xt_pk) {                                             // and its fp16x3 operand image (E is even)
+            uint32_t* d = reinterpret_cast<uint32_t*>(xt_pk) + (long long)b * ld_xt_pk;
+            for (int e2 = threadIdx.x; 2 * e2 < E; e2 += blockDim.x) {
+                uint32_t hi, lo;
+                f16x3_split_pair(fmaxf(row[2 * e2], 0.f), fmaxf(row[2 * e2 + 1], 0.f), pk_scale, hi, lo);
+                const long long w = f16x3_word(2 * e2);
+                d[w] = hi; d[w + 16] = lo;
+            }
+        }
+    }
+}
+
 }  // namespace
 
 // Number of K splits for a skinny product with Nw weight rows and Ktot columns (0 = shape not supported by this path):
@@ -222,6 +325,20 @@ int gvd_reduce_pick(const float* part, int S, int ldp, const float* bias, int B,
     if (V <= PICK_NT * 2) GVD_CHECK_CUDA(gvd_launch(reduce_pick_kernel<2>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, unk_idx, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, logits_out, ld_logits, xt_pk, ld_xt_pk, GVD_F16_SA));
     else if (V <= PICK_NT * 5) GVD_CHECK_CUDA(gvd_launch(reduce_pick_kernel<5>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, unk_idx, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, logits_out, ld_logits, xt_pk, ld_xt_pk, GVD_F16_SA));
     else GVD_CHECK_CUDA(gvd_launch(reduce_pick_kernel<6>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, unk_idx, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, logits_out, ld_logits, xt_pk, ld_xt_pk, GVD_F16_SA));
+    GVD_CHECK_LAUNCH();
+    return 0;
+}
+
+int gvd_reduce_sample(const float* part, int S, int ldp, const float* bias, int B, int V, const GvdSampleParams* params, int step,
+                      long long* it_out, long long* seq_out, float* logp_out, long long out_stride, const float* embed, float* xt,
+                      long long ld_xt, int E, cudaStream_t st, float* xt_pk, long long ld_xt_pk) {
+    GVD_REQUIRE(V >= 2 && V <= PICK_NT * 6 && params && it_out && step >= 0, "reduce_sample: vocabulary of 2..6144 entries");
+    GVD_REQUIRE(!xt_pk || (xt && E % 2 == 0 && ld_xt_pk % 32 == 0 && ld_xt_pk >= (E + 31) / 32 * 32),
+                "reduce_sample: the packed xt needs an even E and a 32-multiple pitch covering E");
+    const long long plane = (long long)B * ldp;
+    if (V <= PICK_NT * 2) GVD_CHECK_CUDA(gvd_launch(reduce_sample_kernel<2>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, params, step, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, xt_pk, ld_xt_pk, GVD_F16_SA));
+    else if (V <= PICK_NT * 5) GVD_CHECK_CUDA(gvd_launch(reduce_sample_kernel<5>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, params, step, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, xt_pk, ld_xt_pk, GVD_F16_SA));
+    else GVD_CHECK_CUDA(gvd_launch(reduce_sample_kernel<6>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, params, step, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, xt_pk, ld_xt_pk, GVD_F16_SA));
     GVD_CHECK_LAUNCH();
     return 0;
 }

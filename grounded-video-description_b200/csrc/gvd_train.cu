@@ -459,16 +459,6 @@ __global__ void __launch_bounds__(256) adam_flat_kernel(float* __restrict__ w, f
 // ---------------------------------------------------------------- dropout: counter-based masks (Philox4x32-10), nothing stored
 // Element i of a tensor at dropout site `site` in optimisation step `step` draws word (i & 3) of Philox(counter = (i >> 2, site, step_lo,
 // step_hi), key = seed): the backward regenerates the same mask from the same (seed, site, step) — no mask tensor, no RNG state.
-__device__ __forceinline__ void philox4x32_10(uint32_t c0, uint32_t c1, uint32_t c2, uint32_t c3, uint32_t k0, uint32_t k1, uint32_t out[4]) {
-#pragma unroll
-    for (int r = 0; r < 10; ++r) {
-        const uint32_t hi0 = __umulhi(0xD2511F53u, c0), lo0 = 0xD2511F53u * c0;
-        const uint32_t hi1 = __umulhi(0xCD9E8D57u, c2), lo1 = 0xCD9E8D57u * c2;
-        c0 = hi1 ^ c1 ^ k0; c1 = lo1; c2 = hi0 ^ c3 ^ k1; c3 = lo0;
-        k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-    }
-    out[0] = c0; out[1] = c1; out[2] = c2; out[3] = c3;
-}
 // y = keep ? x / (1 - p) : 0 with keep = uniform >= p, uniform = (word >> 8) * 2^-24   (nn.Dropout / F.dropout train-mode arithmetic)
 __global__ void dropout_kernel(const float* __restrict__ x, float* __restrict__ y, long long n, float p, float inv_keep, uint32_t seed_lo,
                                uint32_t seed_hi, uint32_t site, uint32_t step_lo, uint32_t step_hi) {

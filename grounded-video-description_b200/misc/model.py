@@ -8,6 +8,7 @@ and the return tuples.  What is new: all arithmetic runs in hand-written sm_90a 
 the C-ABI (include/gvd_b200.h); the three copies of the prologue (model.py:302-409, 504-568,
 634-698) are one native call; nothing executes on the CPU and there is no torch fallback.
 """
+import math
 import os
 import pickle
 import warnings
@@ -179,10 +180,16 @@ class AttModel(CaptionModel):
         return nm, sim
 
     def _sample(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, opt={}):
-        """Greedy (beam_size=1) or beam decode (model.py:492-624, 627-742)."""
-        if not opt.get("sample_max", 1):
-            raise NotImplementedError("multinomial sampling (sample_max=0) is not on the accelerated path")
+        """Beam search, greedy or multinomial decode (model.py:492-624, 627-742), dispatched in the reference's order: beam_size > 1 ->
+        beam search whatever sample_max is (model.py:501); the transformer captioner decodes greedily whatever sample_max is
+        (model.py:570-578); sample_max = 1 -> greedy; sample_max = 0 -> multinomial sampling at eval_opt['temperature'] (model.py:595-603).
+
+        Sampling draws from softmax(logits / temperature) like the reference's torch.multinomial, but through counter-based noise keyed by
+        a per-call seed (gvd_decode_sample): the seed is one draw from torch's default CPU generator, so torch.manual_seed(s) reproduces a
+        call and successive calls differ.  The draws of a row depend on its index in the batch: splitting a batch changes them."""
+        sample_max = opt.get("sample_max", 1)
         beam_size = opt.get("beam_size", 1)
+        temperature = opt.get("temperature", 1.0)
         if beam_size > 1:
             if self.att_model == "transformer":
                 raise NotImplementedError("the transformer captioner decodes greedily (Decoder.greedy, transformer.py:214); the reference has no "
@@ -196,8 +203,17 @@ class AttModel(CaptionModel):
             seq = self._tfm.decode_greedy(*self._tfm_encodings(nm, B, T))
             zero = seq.new_zeros(B, 1)
             return seq, zero, zero.clone()                # model.py:578
+        if not sample_max:
+            temperature = float(temperature)
+            if not (math.isfinite(temperature) and temperature > 0):
+                raise ValueError("temperature must be finite and > 0 (got %r)" % (temperature,))
+            seed = int(torch.randint(0, 2 ** 62, (1,)))
         nm, sim = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask)
-        seq, logp, att2 = nm.decode_greedy(B, T, self._u8(pnt_mask).contiguous())
+        mask = self._u8(pnt_mask).contiguous()
+        if sample_max:
+            seq, logp, att2 = nm.decode_greedy(B, T, mask)
+        else:
+            seq, logp, att2 = nm.decode_sample(B, T, mask, seed, temperature)
         return seq, logp, att2, sim
 
     def _tfm_encodings(self, nm, B, T):

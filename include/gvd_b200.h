@@ -89,6 +89,22 @@ GVD_API int gvd_decode_greedy(gvd_model_t* m, int B, int T, void* workspace, siz
                       float* att2_logits_out,       /* [B,L,R] masked logits (Q8)  */
                       void* stream);
 
+/* ---- the same loop with multinomial sampling (sample_max = 0, misc/model.py:595-603): same shapes and outputs as gvd_decode_greedy.
+ * Word i of batch row b at step t (0 .. L-1) is drawn with the Gumbel-max trick: it = argmax_i (logit_i / temperature + g_i), ties to the
+ * lower index, g_i = -log(-log(u_i)), u_i = ((w >> 9) + 0.5) * 2^-23 with w = word (i & 3) of Philox4x32-10(counter = (i >> 2, b, t, 0),
+ * key = seed) — the token follows softmax(logit / temperature), the distribution torch.multinomial draws from.  logprobs_out holds the
+ * UNTEMPERED log-softmax of the drawn word (model.py:602); there is no UNK rule.  The 23-bit uniforms bound g to [-2.82, 16.64]: a word
+ * whose key is more than ~19.5 below the best is never drawn (probability < 1e-8).  b is the row's index in this call, so splitting a batch
+ * changes the draws.  A row whose keys are all -inf or all NaN yields token 0.  temperature: finite and > 0; vocab_size <= 6144.
+ * The seed and temperature travel in a workspace-resident parameter block, so the captured loop is replayed, not re-captured, for new ones. */
+GVD_API int gvd_decode_sample(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes,
+                      const uint8_t* pnt_mask,      /* [B,R+1]                     */
+                      uint64_t seed, float temperature,
+                      int64_t* seq_out,             /* [B,L]                       */
+                      float* logprobs_out,          /* [B,L] or NULL               */
+                      float* att2_logits_out,       /* [B,L,R] masked logits (Q8)  */
+                      void* stream);
+
 /* ---- S2-S4 one teacher-forced / externally driven step (misc/AttModel.py:134-164).
  * state layout in the workspace; `step` selects the ping-pong parity and must count from 0. */
 GVD_API int gvd_decode_step_fwd(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes, int step,
@@ -197,6 +213,10 @@ GVD_API int gvd_op_reduce_pick(const float* part, int S, int ldp, const float* b
                   float* logits_out, int64_t ld_logits, float* xt_pk, int64_t ld_xt_pk, void* stream);
 GVD_API int gvd_op_greedy_pick(const float* logits, int64_t ld, int B, int V, int unk_idx, int64_t* it_out, int64_t* seq_out, float* logp_out,
                   int64_t out_stride, const float* embed, float* xt, int64_t ld_xt, int E, void* stream);
+/* the multinomial sampler of gvd_decode_sample on S partial planes (+ bias or NULL) at decode step `step`, same destinations as reduce_pick */
+GVD_API int gvd_op_reduce_sample(const float* part, int S, int ldp, const float* bias, int B, int V, float temperature, uint64_t seed, int step,
+                  int64_t* it_out, int64_t* seq_out, float* logp_out, int64_t out_stride, const float* embed, float* xt, int64_t ld_xt, int E,
+                  float* xt_pk, int64_t ld_xt_pk, void* stream);
 /* vocabulary head h [B,K] . W [V,K]^T + bias with the sampler in the GEMM epilogue; B <= 128, E % 4 == 0, xt [B,E] */
 GVD_API int gvd_op_logit_pick_tc(const float* h, int64_t ldh, const float* W, int64_t ldw, const float* bias, int B, int V, int K, int unk_idx,
                   const float* embed, int E, int64_t* it_out, int64_t* seq_out, float* logp_out, int64_t out_stride, float* xt, void* stream);
