@@ -20,7 +20,8 @@ EXPORTS = [
     "gvd_decode_reset_state", "gvd_sample_greedy_host", "gvd_op_linear", "gvd_op_tanh", "gvd_op_kernel_launches",
     "gvd_profile_enable", "gvd_profile_reset", "gvd_profile_count", "gvd_profile_entry",
     "gvd_op_linear_tc", "gvd_op_linear_f16ss", "gvd_op_skinny_partials", "gvd_op_reduce_lstm", "gvd_op_reduce_bias", "gvd_op_reduce_pick",
-    "gvd_op_reduce_sample", "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
+    "gvd_op_reduce_sample", "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_attention", "gvd_op_beam_topk",
+    "gvd_op_row_argmax", "gvd_op_beam_search_scripted", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
     "gvd_tfm_workspace_bytes", "gvd_tfm_decode_greedy", "gvd_tfm_teacher_fwd",
     "gvd_grounding_extract", "gvd_grounding_eval", "gvd_plan_skinny_splits", "gvd_plan_h2d_chunks", "gvd_workspace_bytes_beam", "gvd_beam_decode", "gvd_workspace_bytes_teacher", "gvd_teacher_fwd",
     # training-step primitives (csrc/gvd_train.cu; bound in train_ops.py)
@@ -96,6 +97,11 @@ def lib():
     L.gvd_op_reduce_sample.argtypes = [vp, ci, ci, vp, ci, ci, ctypes.c_float, ctypes.c_uint64, ci, vp, vp, vp, i64, vp, vp, i64, ci, vp, i64, vp]
     L.gvd_op_logit_pick_tc.argtypes = [vp, i64, vp, i64, vp, ci, ci, ci, ci, vp, ci, vp, vp, vp, i64, vp, vp]
     L.gvd_op_gru_layer.argtypes = [ci, vp, vp, vp, vp, ci, ci, ci, vp, vp]
+    L.gvd_op_attention.argtypes = [vp, vp, vp, vp, vp, vp, ci, vp, vp, vp, vp, vp, vp, vp, i64, vp, i64, vp, vp, vp, i64, vp, i64,
+                                   ci, ci, ci, ci, ci, ci, ci, ci, vp]
+    L.gvd_op_beam_topk.argtypes = [vp, i64, ci, ci, ci, vp, vp, vp]
+    L.gvd_op_row_argmax.argtypes = [vp, i64, ci, ci, vp, vp]
+    L.gvd_op_beam_search_scripted.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
     L.gvd_set_backend.argtypes = [ci]
     L.gvd_tfm_workspace_bytes.argtypes = [vp, ci, ci, ci, ci]
     L.gvd_tfm_workspace_bytes.restype = sz
@@ -616,6 +622,57 @@ def op_gru_layer(path, gi, Whh, bhh, sample_idx=None):
     check(lib().gvd_op_gru_layer(int(path), _dev(gi, torch.float32, "gi"), _dev(Whh, torch.float32, "Whh"), _dev(bhh, torch.float32, "bhh"),
                                  _dev(sample_idx, torch.int64, "sample_idx") if sample_idx is not None else None, B, T, G, _ptr(out), _stream()))
     return out
+
+
+def op_attention(p_pool, pool, p_conv, conv, w1, b1, w2, b2, att_mask, out_mask, z_out, partial, x_out, RC, TC, q=None, q_part=None,
+                 q_bias=None, ticket=None, x_pk=None, feat_div=1):
+    """The decode attention of B query rows through gvd_op_attention.  Features [B / feat_div, N, A | H]; q [B, 2A] or its split-K planes
+    q_part [q_S, B, 2A] + q_bias [2A]; att_mask [B / feat_div, R+1]; out_mask [B / feat_div, R+1] or a [B / feat_div, R+1] column window
+    of a wider mask (its row pitch is passed); z_out [B, R] and x_out [B, H] (x_pk [B, rup32(H)] int32 words) may be column windows of
+    wider buffers; partial [B, nch, H+4]; ticket [B] int32 (None: the separate combine kernel)."""
+    Bf, R, A = p_pool.shape
+    T, H = conv.shape[1], conv.shape[2]
+    B = (q if q is not None else q_part[0]).shape[0]
+    q_S = q_part.shape[0] if q_part is not None else 0
+    if out_mask.stride(1) != 1 or att_mask.stride(1) != 1 or att_mask.stride(0) != R + 1:
+        raise GvdError("masks must have dense rows, att_mask a pitch of R+1")
+    check(lib().gvd_op_attention(
+        _dev(p_pool, torch.float32, "p_pool"), _dev(pool, torch.float32, "pool"), _dev(p_conv, torch.float32, "p_conv"),
+        _dev(conv, torch.float32, "conv"), _ptr(q), _ptr(q_part), q_S, _ptr(q_bias), _ptr(w1), _ptr(b1), _ptr(w2), _ptr(b2), _ptr(att_mask),
+        _ptr(out_mask), out_mask.stride(0), _ptr(z_out), _pitch(z_out), _ptr(partial), _ptr(ticket), _ptr(x_out), _pitch(x_out), _ptr(x_pk),
+        _pitch(x_pk), B, R, T, A, H, int(RC), int(TC), int(feat_div), _stream()))
+
+
+def op_beam_topk(logits, K):
+    """(topv [rows, K] float32, topi [rows, K] int32) of logits [rows, V] (dense rows, any pitch), outputs pre-filled with NaN / -1."""
+    rows, V = logits.shape
+    topv = torch.full((rows, K), float("nan"), dtype=torch.float32, device="cuda")
+    topi = torch.full((rows, K), -1, dtype=torch.int32, device="cuda")
+    check(lib().gvd_op_beam_topk(_ptr(logits), _pitch(logits), rows, V, int(K), _ptr(topv), _ptr(topi), _stream()))
+    return topv, topi
+
+
+def op_row_argmax(z):
+    """idx [rows] int32 (pre-filled with -1) = first index of each row maximum of z [rows, R]."""
+    rows, R = z.shape
+    idx = torch.full((rows,), -1, dtype=torch.int32, device="cuda")
+    check(lib().gvd_op_row_argmax(_ptr(z), _pitch(z), rows, R, _ptr(idx), _stream()))
+    return idx
+
+
+def op_beam_search_scripted(logits, z, probe, K):
+    """The beam bookkeeping of gvd_beam_decode on scripted logits [L, B*K, V] and region scores [L+1, B*K, R]; probe [B*K, H] is reordered
+    in place.  Returns seq [B, L] int64, logp [B, L], att2_idx [B, L] int64 and parents [L, B*K] int32, pre-filled with sentinels."""
+    L, BK, V = logits.shape
+    R, H = z.shape[2], probe.shape[1]
+    B = BK // K
+    seq = torch.full((B, L), -7, dtype=torch.int64, device="cuda")
+    logp = torch.full((B, L), float("nan"), dtype=torch.float32, device="cuda")
+    att = torch.full((B, L), -7, dtype=torch.int64, device="cuda")
+    parents = torch.full((L, BK), -7, dtype=torch.int32, device="cuda")
+    check(lib().gvd_op_beam_search_scripted(_dev(logits, torch.float32, "logits"), _dev(z, torch.float32, "z"), _dev(probe, torch.float32, "probe"),
+                                            B, int(K), L, V, R, H, _ptr(seq), _ptr(logp), _ptr(att), _ptr(parents), _stream()))
+    return seq, logp, att, parents
 
 
 def op_linear(A, W, bias=None, act=0, tc=False):

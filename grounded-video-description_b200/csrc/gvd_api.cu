@@ -1435,6 +1435,48 @@ extern "C" GVD_API int gvd_teacher_fwd(gvd_model_t* m, int B, int T, int nbox, i
     return 0;
 }
 
+// The bookkeeping of the beam search around the model, shared by gvd_beam_decode and its scripted test hook (gvd_op_beam_search_scripted):
+//   bookkeeping init (<bos> tokens 0, beam_seq 0, att2 indices -1, sums 0); scores(0) = the <bos> step's region scores, row_argmax;
+//   then for t = 0 .. L-1: logits(t), beam_topk, beam_update and, but at the last step (the reference runs one more, unused, core step),
+//   the recurrent rows of state(t) reordered to the surviving beams (CaptionModelBU.py:85-89), scores(t + 1), row_argmax; finally beam_finish.
+// scores(t) runs model step t on bb.tokens and returns its region scores [B*K, R]; logits(t, &ld) returns step t's logits [B*K, V] (pitch
+// ld); state(t, bufs) fills at most 4 recurrent [B*K, H] buffers and returns their number.  parents_out: optional [L][B*K] copy of every
+// step's bb.parent.
+template <class Scores, class Logits, class State>
+static int beam_search_run(const BeamBufs& bb, int* bos_att, float* gather_tmp, int B, int K, int L, int V, int R, int H, int64_t* seq_out,
+                           float* lp_out, int64_t* att_out, int* parents_out, cudaStream_t st, Scores scores, Logits logits, State state) {
+    const int BK = B * K;
+    GVD_CHECK_CUDA(cudaMemsetAsync(bb.tokens, 0, (size_t)BK * 8, st));
+    GVD_CHECK_CUDA(cudaMemsetAsync(bb.seq, 0, (size_t)B * L * K * 4, st));
+    GVD_CHECK_CUDA(cudaMemsetAsync(bb.lp, 0, (size_t)B * L * K * 4, st));
+    GVD_CHECK_CUDA(cudaMemsetAsync(bb.att, 0xFF, (size_t)B * L * K * 4, st));
+    GVD_CHECK_CUDA(cudaMemsetAsync(bb.att_ind, 0xFF, (size_t)BK * 4, st));
+    GVD_CHECK_CUDA(cudaMemsetAsync(bb.sums, 0, (size_t)B * K * 4, st));
+    GVD_CHECK_CUDA(cudaMemsetAsync(bb.done_flag, 0, (size_t)B * 4, st));
+    const float* z = nullptr;
+    GVD_TRY(scores(0, &z));
+    GVD_STAGE("beam.argmax", gvd_row_argmax(z, R, BK, R, bos_att, st));
+    for (int t = 0; t < L; ++t) {
+        const float* lg = nullptr;
+        long long ld = 0;
+        GVD_TRY(logits(t, &lg, &ld));
+        GVD_STAGE("beam.topk", gvd_beam_topk(lg, ld, BK, V, K, bb.topv, bb.topi, st));
+        GVD_STAGE("beam.update", gvd_beam_update(bb, B, K, L, t, st));
+        if (parents_out) GVD_CHECK_CUDA(cudaMemcpyAsync(parents_out + (size_t)t * BK, bb.parent, (size_t)BK * 4, cudaMemcpyDeviceToDevice, st));
+        if (t == L - 1) break;
+        float* bufs[4];
+        const int n = state(t, bufs);
+        for (int i = 0; i < n; ++i) {
+            GVD_STAGE("beam.gather", gvd_beam_gather_rows(bufs[i], gather_tmp, bb.parent, B, K, H, st));
+            GVD_CHECK_CUDA(cudaMemcpyAsync(bufs[i], gather_tmp, (size_t)BK * H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        }
+        GVD_TRY(scores(t + 1, &z));
+        GVD_STAGE("beam.argmax", gvd_row_argmax(z, R, BK, R, bb.att_ind, st));
+    }
+    GVD_STAGE("beam.finish", gvd_beam_finish(bb, bos_att, B, K, L, (long long*)seq_out, lp_out, (long long*)att_out, st));
+    return 0;
+}
+
 // B1/B2: beam search for every clip at once (misc/model.py:700-742 + misc/CaptionModelBU.py:104-185, repaired semantics)
 extern "C" GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_size, void* workspace, size_t workspace_bytes,
                                        const uint8_t* pnt_mask, int64_t* seq_out, float* logprobs_out, int64_t* att2_idx_out, void* stream) {
@@ -1446,42 +1488,32 @@ extern "C" GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_si
     const gvd_dims_t& d = m->d;
     const int H = d.rnn_size, V = d.vocab_size, L = d.seq_length, R = m->R, K = beam_size, BK = B * K;
     const size_t BKH = (size_t)BK * H;
-    {   // zero state, <bos> tokens, bookkeeping init (beam_seq 0, att2 indices -1, sums 0)
+    {   // zero state and attention tickets (the bookkeeping is initialised by beam_search_run)
         const size_t n = BKH * sizeof(float);
         GVD_CHECK_CUDA(cudaMemsetAsync(w.h_att, 0, 2 * n, st));
         GVD_CHECK_CUDA(cudaMemsetAsync(w.c_att, 0, n, st));
         GVD_CHECK_CUDA(cudaMemsetAsync(w.h_lang, 0, 2 * n, st));
         GVD_CHECK_CUDA(cudaMemsetAsync(w.c_lang, 0, n, st));
-        GVD_CHECK_CUDA(cudaMemsetAsync(w.bb.tokens, 0, (size_t)BK * 8, st));
-        GVD_CHECK_CUDA(cudaMemsetAsync(w.bb.seq, 0, (size_t)B * L * K * 4, st));
-        GVD_CHECK_CUDA(cudaMemsetAsync(w.bb.lp, 0, (size_t)B * L * K * 4, st));
-        GVD_CHECK_CUDA(cudaMemsetAsync(w.bb.att, 0xFF, (size_t)B * L * K * 4, st));
-        GVD_CHECK_CUDA(cudaMemsetAsync(w.bb.att_ind, 0xFF, (size_t)BK * 4, st));
-        GVD_CHECK_CUDA(cudaMemsetAsync(w.bb.sums, 0, (size_t)B * K * 4, st));
-        GVD_CHECK_CUDA(cudaMemsetAsync(w.bb.done_flag, 0, (size_t)B * 4, st));
         GVD_CHECK_CUDA(cudaMemsetAsync(w.ticket, 0, (size_t)BK * sizeof(int), st));
     }
-    // first core step on <bos> (model.py:723-733): all K rows of a clip are identical
-    GVD_TRY(core_step(m, w, BK, T, 0, w.bb.tokens, pnt_mask, pnt_mask, w.z_rows, R, st, K));
-    GVD_STAGE("beam.argmax", gvd_row_argmax(w.z_rows, R, BK, R, w.bos_att, st));
-    for (int t = 0; t < L; ++t) {
-        const int par = (t + 1) & 1;                      // state parity written by the previous core step
-        float* h_att = w.h_att + (size_t)par * BKH;
-        float* h_lang = w.h_lang + (size_t)par * BKH;
+    // core step t on the beam tokens; step 0 is the <bos> step (model.py:723-733), whose K rows of a clip are identical
+    auto scores = [&](int t, const float** z) {
+        *z = w.z_rows;
+        return core_step(m, w, BK, T, t, w.bb.tokens, pnt_mask, pnt_mask, w.z_rows, R, st, K);
+    };
+    auto logits = [&](int t, const float** lg, long long* ld) {
+        const float* h_lang = w.h_lang + (size_t)((t + 1) & 1) * BKH;   // state parity written by the previous core step
+        *lg = w.logits;
+        *ld = m->Vp;
         GVD_STAGE("decode.logit", gvd_linear(h_lang, H, m->P("logit.weight"), H, m->P("logit.bias"), w.logits, m->Vp, BK, V, H, GVD_ACT_NONE, st));
-        GVD_STAGE("beam.topk", gvd_beam_topk(w.logits, m->Vp, BK, V, K, w.bb.topv, w.bb.topi, st));
-        GVD_STAGE("beam.update", gvd_beam_update(w.bb, B, K, L, t, st));
-        if (t == L - 1) break;                            // the reference runs one more (unused) core step
-        float* bufs[4] = {h_att, w.c_att, h_lang, w.c_lang};
-        for (float* buf : bufs) {                         // rearrange recurrent state to the surviving beams (CaptionModelBU.py:85-89)
-            GVD_STAGE("beam.gather", gvd_beam_gather_rows(buf, w.gather_tmp, w.bb.parent, B, K, H, st));
-            GVD_CHECK_CUDA(cudaMemcpyAsync(buf, w.gather_tmp, BKH * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        }
-        GVD_TRY(core_step(m, w, BK, T, t + 1, w.bb.tokens, pnt_mask, pnt_mask, w.z_rows, R, st, K));
-        GVD_STAGE("beam.argmax", gvd_row_argmax(w.z_rows, R, BK, R, w.bb.att_ind, st));
-    }
-    GVD_STAGE("beam.finish", gvd_beam_finish(w.bb, w.bos_att, B, K, L, (long long*)seq_out, logprobs_out, (long long*)att2_idx_out, st));
-    return 0;
+        return 0;
+    };
+    auto state = [&](int t, float** bufs) {
+        const int par = (t + 1) & 1;
+        bufs[0] = w.h_att + (size_t)par * BKH; bufs[1] = w.c_att; bufs[2] = w.h_lang + (size_t)par * BKH; bufs[3] = w.c_lang;
+        return 4;
+    };
+    return beam_search_run(w.bb, w.bos_att, w.gather_tmp, B, K, L, V, R, H, seq_out, logprobs_out, att2_idx_out, nullptr, st, scores, logits, state);
 }
 
 // Clip chunks of the host-buffer entry point.  The pipeline starts with one attention sub-batch (`unit` clips: the first kernel waits for the
@@ -1804,6 +1836,74 @@ extern "C" GVD_API int gvd_op_gru_layer(int path, const float* gi, const float* 
         if (cudaMemsetAsync(hstate, 0, state * sizeof(float), st) != cudaSuccess) { gvd_set_error("op_gru_layer: memset failed"); rc = 2; }
         if (!rc) rc = gru_layer_steps(gi, Whh, bhh, hstate, tail, out, (const long long*)sample_idx, B, T, G, st);
     }
+    cudaFreeAsync(buf, st);
+    return rc;
+}
+// The decode attention (attn_partial_kernel) with every AttnArgs field the decode step sets.  ticket != NULL: the last chunk CTA of each row
+// merges the partials (the decode step's fused path; the caller zeroes the tickets once); ticket == NULL: attn_combine_kernel merges them
+// after the partial launch, into x_out at pitch H.  Test hook.
+extern "C" GVD_API int gvd_op_attention(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                                        const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
+                                        const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
+                                        int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
+                                        int B, int R, int T, int A, int H, int RC, int TC, int feat_div, void* stream) {
+    GVD_REQUIRE(p_pool && pool && p_conv && conv && w1 && b1 && w2 && b2 && att_mask && out_mask && z_out && partial && x_out && B >= 1 &&
+                R >= 1 && T >= 1 && feat_div >= 1 && B % feat_div == 0, "op_attention: bad arguments");
+    GVD_REQUIRE(q ? !q_part : (q_part && q_bias && q_S >= 1), "op_attention: give either q or (q_part, q_S >= 1, q_bias)");
+    GVD_REQUIRE(z_stride_b >= R && (out_mask_stride == 0 || out_mask_stride >= R + 1), "op_attention: bad z / out_mask pitch");
+    GVD_REQUIRE(x_ld == 0 || (x_ld >= H && x_ld % 4 == 0), "op_attention: x_ld must be 0 or a multiple of 4 covering H");
+    GVD_REQUIRE(!x_pk || (x_pk_ld % 32 == 0 && x_pk_ld >= (H + 31) / 32 * 32), "op_attention: x_pk_ld must be a 32-multiple covering H");
+    GVD_REQUIRE(ticket || ((x_ld == 0 || x_ld == H) && !x_pk), "op_attention: the separate combine writes x_out at pitch H and no image");
+    AttnArgs a{};
+    a.p_pool = p_pool; a.pool = pool; a.p_conv = p_conv; a.conv = conv; a.q = q;
+    if (!q) { a.q_part = q_part; a.q_S = q_S; a.q_plane = (long long)B * 2 * A; a.q_bias = q_bias; }
+    a.w1 = w1; a.b1 = b1; a.w2 = w2; a.b2 = b2;
+    a.att_mask = att_mask; a.out_mask = out_mask; a.out_mask_stride = out_mask_stride; a.z_out = z_out; a.z_stride_b = z_stride_b;
+    a.partial = partial; a.ticket = ticket; a.x_out = x_out; a.x_ld = x_ld; a.x_pk = x_pk; a.x_pk_ld = x_pk_ld;
+    a.B = B; a.R = R; a.T = T; a.A = A; a.H = H; a.RC = RC; a.TC = TC; a.feat_div = feat_div;
+    cudaStream_t st = (cudaStream_t)stream;
+    GVD_TRY(gvd_attn_partial(a, st));
+    if (ticket) return 0;
+    int nch_r, nch_t;
+    gvd_attn_chunks(R, T, RC, TC, &nch_r, &nch_t);
+    return gvd_attn_combine(partial, x_out, B, H, nch_r, nch_t, st);
+}
+// beam_topk / row_argmax on their own.  Test hooks.
+extern "C" GVD_API int gvd_op_beam_topk(const float* logits, int64_t ld, int rows, int V, int K, float* topv, int* topi, void* stream) {
+    GVD_REQUIRE(logits && topv && topi && rows >= 1 && ld >= V, "op_beam_topk: bad arguments");
+    return gvd_beam_topk(logits, ld, rows, V, K, topv, topi, (cudaStream_t)stream);
+}
+extern "C" GVD_API int gvd_op_row_argmax(const float* z, int64_t ld, int rows, int R, int* idx, void* stream) {
+    GVD_REQUIRE(z && idx && rows >= 1 && R >= 1 && ld >= R, "op_row_argmax: bad arguments");
+    return gvd_row_argmax(z, ld, rows, R, idx, (cudaStream_t)stream);
+}
+// gvd_beam_decode's bookkeeping (beam_search_run) with the model replaced by a script: step t's logits are logits[t] [B*K, V], the region
+// scores of core step t are z[t] [B*K, R] (t = 0: <bos>), and the recurrent state is one probe buffer [B*K, H] that is reordered like the
+// model's state.  The bookkeeping buffers are allocated here.  Test hook.
+extern "C" GVD_API int gvd_op_beam_search_scripted(const float* logits, const float* z, float* probe, int B, int K, int L, int V, int R, int H,
+                                                   int64_t* seq_out, float* logp_out, int64_t* att2_idx_out, int* parents_out, void* stream) {
+    GVD_REQUIRE(logits && z && probe && seq_out && logp_out && att2_idx_out && parents_out && B >= 1 && V >= 1 && R >= 1 && H >= 4 && H % 4 == 0,
+                "op_beam_search_scripted: bad arguments");
+    GVD_REQUIRE(K >= 1 && L >= 1, "op_beam_search_scripted: beam_size and seq_length must be >= 1");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t BK = (size_t)B * K, BLK = (size_t)B * L * K;
+    const size_t n4 = 3 * BLK + 2 * BK * K + 4 * BK + 2 * (size_t)B + 2 * (size_t)B * L;   // 4-byte words after the gather rows and tokens
+    char* buf = nullptr;
+    GVD_CHECK_CUDA(cudaMallocAsync((void**)&buf, BK * H * 4 + BK * 8 + n4 * 4, st));
+    float* gather_tmp = (float*)buf;                                 // [B*K, H], 16-byte rows
+    BeamBufs bb{};
+    bb.tokens = (long long*)(buf + BK * H * 4);
+    int* p = (int*)(bb.tokens + BK);
+    auto take = [&](size_t n) { int* r = p; p += n; return r; };
+    bb.seq = take(BLK); bb.att = take(BLK); bb.lp = (float*)take(BLK); bb.topv = (float*)take(BK * K); bb.topi = take(BK * K);
+    bb.sums = (float*)take(BK); bb.parent = take(BK); bb.att_ind = take(BK);
+    int* bos_att = take(BK);
+    bb.done_flag = take(B); bb.done_slot = take(B); bb.done_seq = take((size_t)B * L); bb.done_lp = (float*)take((size_t)B * L);
+    auto scores = [&](int t, const float** zt) { *zt = z + (size_t)t * BK * R; return 0; };
+    auto step_logits = [&](int t, const float** lg, long long* ld) { *lg = logits + (size_t)t * BK * V; *ld = V; return 0; };
+    auto state = [&](int, float** bufs) { bufs[0] = probe; return 1; };
+    const int rc = beam_search_run(bb, bos_att, gather_tmp, B, K, L, V, R, H, seq_out, logp_out, att2_idx_out, parents_out, st, scores, step_logits,
+                                   state);
     cudaFreeAsync(buf, st);
     return rc;
 }

@@ -15,7 +15,9 @@ namespace {
 constexpr int BEAM_MAXK = 8;
 constexpr int BEAM_MAXL = 64;
 
-// per row: log_softmax and the K best (value desc, index asc on ties) — ys/ix of CaptionModelBU.py:45
+// per row: log_softmax and the K best (value desc, index asc on ties) — ys/ix of CaptionModelBU.py:45.  NaN words are skipped (no
+// comparison with a NaN succeeds); a pick that finds only NaN left takes the lowest untaken index, so an all-NaN row gives 0 .. K-1 like a
+// stable torch.sort(descending=True), and the token never leaves the vocabulary.  (torch ranks NaN first: rows only partly NaN differ.)
 __global__ void __launch_bounds__(256) beam_topk_kernel(const float* __restrict__ logits, long long ld, int V, int K,
                                                         float* __restrict__ topv, int* __restrict__ topi) {
     __shared__ float red[32];
@@ -52,6 +54,14 @@ __global__ void __launch_bounds__(256) beam_topk_kernel(const float* __restrict_
         if (threadIdx.x == 0) {
             for (int w = 1; w < 8; ++w)
                 if (wv[w] > bv || (wv[w] == bv && wi[w] < bi)) { bv = wv[w]; bi = wi[w]; }
+            if (bi == 0x7fffffff) {                   // every untaken word is NaN
+                bool taken = true;                    // the lowest untaken index: at most k < K <= V
+                for (bi = 0; taken; bi += taken) {
+                    taken = false;
+                    for (int j = 0; j < k; ++j) taken |= (chosen[j] == bi);
+                }
+                bv = x[bi];
+            }
             chosen[k] = bi;
             chosen_v[k] = bv;
         }
@@ -136,7 +146,8 @@ __global__ void beam_gather_rows_kernel(const float* __restrict__ src, float* __
         *reinterpret_cast<float4*>(dst + (long long)row * H + h) = *reinterpret_cast<const float4*>(src + (long long)srow * H + h);
 }
 
-// first index of the row maximum (torch.max(att2_weight, 1)[1], CaptionModelBU.py:182)
+// first index of the row maximum (torch.max(att2_weight, 1)[1], CaptionModelBU.py:182); NaN entries are skipped, an all-NaN row gives 0
+// like torch.argmax
 __global__ void __launch_bounds__(256) row_argmax_kernel(const float* __restrict__ z, long long ld, int R, int* __restrict__ out) {
     __shared__ float wv[8];
     __shared__ int wi[8];
@@ -159,7 +170,7 @@ __global__ void __launch_bounds__(256) row_argmax_kernel(const float* __restrict
     if (threadIdx.x == 0) {
         for (int w = 1; w < 8; ++w)
             if (wv[w] > bv || (wv[w] == bv && wi[w] < bi)) { bv = wv[w]; bi = wi[w]; }
-        out[row] = bi;
+        out[row] = bi == 0x7fffffff ? 0 : bi;      // no comparison succeeded: every entry NaN
     }
 }
 

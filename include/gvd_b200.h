@@ -118,7 +118,9 @@ GVD_API int gvd_decode_reset_state(gvd_model_t* m, int B, int T, void* workspace
 
 /* ---- B1/B2: beam search of all clips at once, bookkeeping on the device (misc/model.py:627-742,
  * misc/CaptionModelBU.py:24-185 with the documented minimal repair; as-run aliasing reproduced).
- * Needs a workspace of gvd_workspace_bytes_beam() bytes that gvd_prologue_fwd filled for the same (B,T). */
+ * Needs a workspace of gvd_workspace_bytes_beam() bytes that gvd_prologue_fwd filled for the same (B,T).
+ * NaN rules of the bookkeeping: a row of logits that is all NaN ranks words 0 .. beam_size-1 (as a stable torch.sort(descending=True) does),
+ * an all-NaN row of region scores gives region 0 (torch.argmax); see gvd_op_beam_topk / gvd_op_row_argmax. */
 GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_size, void* workspace, size_t workspace_bytes,
                     const uint8_t* pnt_mask,      /* [B,R+1]                              */
                     int64_t* seq_out,             /* [B,L]                                */
@@ -225,6 +227,34 @@ GVD_API int gvd_op_logit_pick_tc(const float* h, int64_t ldh, const float* W, in
  * follows the backend switch); path 1: tensor-core layer kernel (B <= 128, G % 32 == 0). */
 GVD_API int gvd_op_gru_layer(int path, const float* gi, const float* Whh, const float* bhh, const int64_t* sample_idx, int B, int T, int G,
                   float* out, void* stream);
+/* ---- the decode attention and the beam-search bookkeeping op by op (tests/test_gpu_attn_beam_ops.py).
+ * gvd_op_attention: Attention + Attention2 (AttModel.py:33-53, :71-108) of B query rows; row b attends over clip b / feat_div.
+ *   p_pool [B/feat_div,R,A], pool [.,R,H], p_conv [.,T,A], conv [.,T,H]; the query [B,2A] (temporal | region) is either q or the sum
+ *   q_bias + q_part[0..q_S) over split-K planes [q_S][B][2A] (then q == NULL).  w1,b1 / w2,b2: the two alpha_net layers ([A], [1]).
+ *   Masks [B/feat_div, R+1] uint8 with the legacy leading column (ignored); out_mask rows at pitch out_mask_stride (0 = R+1).
+ *   z_out[b * z_stride_b + r] = region logit, MIN_VALUE where att_mask or out_mask is set.  x_out[b * x_ld + h] (x_ld 0 = H) = att + att2;
+ *   x_pk: optional fp16x3 image of it (scale 4, pitch x_pk_ld words).  RC / TC rows per region / temporal chunk (1 .. 128); partial
+ *   [B, ceil(R/RC) + ceil(T/TC), H+4] chunk records (max, sum of exp, 2 unused words, unnormalised weighted sum), region chunks first.
+ *   ticket [B] zeroed ints: the last chunk CTA of a row merges (and resets its ticket to 0); NULL: a separate combine kernel merges
+ *   (x_ld must then be 0 or H, no x_pk).  A, H multiples of 4, A and H <= 1024. */
+GVD_API int gvd_op_attention(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q, const float* q_part,
+                  int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2, const float* b2, const uint8_t* att_mask,
+                  const uint8_t* out_mask, int64_t out_mask_stride, float* z_out, int64_t z_stride_b, float* partial, int* ticket, float* x_out,
+                  int64_t x_ld, float* x_pk, int64_t x_pk_ld, int B, int R, int T, int A, int H, int RC, int TC, int feat_div, void* stream);
+/* beam_topk: per row of logits [rows, V] (pitch ld) the K <= 8 (K <= V) best words, value descending, ties to the lower index:
+ *   topv [rows, K] = their log_softmax, topi [rows, K].  NaN words are skipped; a pick that finds only NaN left takes the lowest untaken
+ *   index, so an all-NaN row gives 0 .. K-1 (as a stable torch.sort(descending=True) does).  Rows only partly NaN differ from torch,
+ *   which ranks NaN first.
+ * row_argmax: idx [rows] int32 = first index of the row maximum of z [rows, R] (pitch ld); an all -inf or all-NaN row gives 0 like
+ *   torch.argmax (NaN entries are skipped: a row only partly NaN differs, torch returns its first NaN). */
+GVD_API int gvd_op_beam_topk(const float* logits, int64_t ld, int rows, int V, int K, float* topv, int* topi, void* stream);
+GVD_API int gvd_op_row_argmax(const float* z, int64_t ld, int rows, int R, int* idx, void* stream);
+/* gvd_beam_decode's bookkeeping with the model replaced by a script (K <= 8, L <= 64): logits [L][B*K][V] (step t's vocabulary logits),
+ * z [L+1][B*K][R] (region scores of core step t; t = 0 is the <bos> step), probe [B*K][H] (H % 4 == 0): a stand-in for the recurrent
+ * state, reordered to the surviving beams after every step but the last, in place.  seq_out / logp_out / att2_idx_out [B, L] as
+ * gvd_beam_decode returns them; parents_out [L][B*K] int32: every step's parent beam of each new beam (index within the clip). */
+GVD_API int gvd_op_beam_search_scripted(const float* logits, const float* z, float* probe, int B, int K, int L, int V, int R, int H,
+                  int64_t* seq_out, float* logp_out, int64_t* att2_idx_out, int* parents_out, void* stream);
 /* arithmetic backend switches: bit 0 wgmma tensor cores for every GEMM-shaped stage (0 = fp32 CUDA cores); bit 1 fused self-attention pair;
    bit 2 (4) inert; bit 3 (8) operand-swapped split-K decode products with fused
    reduce + sampler; bit 4 (16) fp16x3 instead of 3xTF32 in the forward GEMMs, pre-split weights, conversion-free decode step, tensor-core GRU;
