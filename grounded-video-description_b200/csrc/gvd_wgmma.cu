@@ -11,13 +11,18 @@
 //            already split, as the fp16x3 operand image of gvd_common.cuh: per row and 32-wide K slice 64 B
 //            of hi halves | 64 B of lo halves = one SWIZZLE_128B row of a K-major wgmma operand.
 //
-// One kernel serves the whole family.  Per CTA (one 128 x 64 output tile, K streamed in 32-element =
-// 128-byte slices through a ring of WG_STAGES stages):
+// One kernel serves the whole family.  Per CTA (one 128 x BN output tile, K streamed in 32-element =
+// 128-byte slices through a ring of stages).  The mode picks the tile width: BN = 128 for MODE_SS (both operands arrive as operand
+// images; the prologue's dense GEMMs, where wider tiles cut the L2 -> SM operand traffic per MAC by a third), BN = 64 for every other
+// mode (their epilogues are built around 64 columns or 16-unit gate boxes, and their N is small):
 //   warp 8    : TMA producer  - cp.async.bulk.tensor (SWIZZLE_128B) of the A / W slices, one mbarrier per stage
 //   warps 0-7 : two consumer warpgroups.  All 256 threads split the raw fp32 slices of the stage in shared
 //               memory (skipped for pre-split operands), fence.proxy.async, then each warpgroup issues the
 //               wgmma products of ITS 64 rows and folds the slice's result into fp32 register accumulators
-//               (round-to-nearest adds; the tensor core's own accumulation is only trusted for one slice).
+//               (round-to-nearest adds; the tensor core's own accumulation is only trusted for one slice).  At BN = 128
+//               each warpgroup issues m64n128k16 products; per output element the products and the fold are those of
+//               the 64-wide tile, so the result is bit-identical.  (9 warps: 3 share a 16K-register SM quarter, so
+//               ptxas caps the kernel at 168 registers; a second in-flight result set, 64 more, does not fit.)
 //   epilogue  : the accumulator fragments are exchanged through shared memory so that every thread owns one
 //               output row (thread <-> row, lane <-> row within the warp); the epilogues are written for
 //               that layout: bias / activation store, transposed split-K partial, fused LSTM cell, fused
@@ -35,10 +40,11 @@ namespace {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BN = 64;
+constexpr int TC_BN_SS = 128;             // tile width of MODE_SS
 constexpr int TC_BK = 32;                 // fp32 elements per K slice = 128 bytes = one swizzle row
 constexpr int WG_CONSUMERS = 256;         // two warpgroups
 constexpr int WG_THREADS = WG_CONSUMERS + 32;
-constexpr int WG_STAGES = 4;
+constexpr int WG_STAGES = 4;              // also at 128-wide tiles (32 KB stages): 6 stages measured no faster on the H100
 constexpr int WG_UJ = 16;                 // hidden units per CTA of the gate-interleaved tiles (LSTM: 4 x 16, GRU: 3 x 16 columns)
 
 enum { MODE_STORE = 0, MODE_LSTM = 1, MODE_PICK = 2, MODE_TRANS = 3, MODE_SS = 4, MODE_GRU = 5, MODE_PV_IMG = 6 };
@@ -171,19 +177,40 @@ __device__ __forceinline__ void wgmma_f16(float (&d)[32], uint64_t da, uint64_t 
         : WG_D32(d)
         : "l"(da), "l"(db), "r"(accumulate));
 }
+// D[64 x 128]: the same fragment layout with j = 0..15
+#define WG_D64(d) WG_D32(d), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), \
+    "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]),     \
+    "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),     \
+    "+f"(d[63])
+#define WG_D64_LIST "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31," \
+    "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}"
+__device__ __forceinline__ void wgmma_f16(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " WG_D64_LIST ", %64, %65, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : WG_D64(d)
+        : "l"(da), "l"(db), "r"(accumulate));
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0(float (&d)[32]) {
     asm volatile("wgmma.wait_group.sync.aligned 0;" : WG_D32(d) : : "memory");
 }
+__device__ __forceinline__ void wgmma_wait0(float (&d)[64]) {
+    asm volatile("wgmma.wait_group.sync.aligned 0;" : WG_D64(d) : : "memory");
+}
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(WG_CONSUMERS) : "memory"); }
 
-template <bool F16> struct WgCfg {
+template <bool F16, int BN> struct WgCfg {
+    static_assert(BN == 64 || (F16 && BN == 128), "tile widths: 64 (every mode), 128 (MODE_SS: fp16x3 operand images)");
     static constexpr int A_BYTES = TC_BM * 128;            // one plane of the A slice (fp16x3: the whole slice, hi | lo halves per row)
-    static constexpr int B_BYTES = TC_BN * 128;
+    static constexpr int B_BYTES = BN * 128;
     static constexpr int STAGE = F16 ? (A_BYTES + B_BYTES) : 2 * (A_BYTES + B_BYTES);
     static constexpr int B_OFF = F16 ? A_BYTES : 2 * A_BYTES;
-    static constexpr int LDS = TC_BN + 4;                  // pitch of the fp32 exchange tile of the epilogue
+    static constexpr int LDS = BN + 4;                     // pitch of the fp32 exchange tile of the epilogue
     static constexpr size_t SMEM = (size_t)WG_STAGES * STAGE + 1024 /*align*/ + 8 * 2 * WG_STAGES + 64;
     static_assert((size_t)WG_STAGES * STAGE >= (size_t)TC_BM * LDS * 4, "the epilogue exchanges the C tile through the pipeline buffers");
     static_assert(SMEM <= 232448, "shared-memory budget (227 KB per CTA)");
@@ -283,13 +310,14 @@ __device__ __forceinline__ void ss_store_row(const SsParams& p, const float (&ac
     }
 }
 
-template <bool F16>
+template <bool F16, int BN>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
                const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapW0,
                const __grid_constant__ CUtensorMap mapW1, const __grid_constant__ CUtensorMap mapW2, const TcParams p) {
-    using Cfg = WgCfg<F16>;
+    using Cfg = WgCfg<F16, BN>;
     constexpr int ST = WG_STAGES;
+    constexpr bool WIDE = BN == 128;            // MODE_SS only: both operands arrive as operand images, nothing to convert
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)ST * Cfg::STAGE);
@@ -299,7 +327,7 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
     const int zb = p.ksplit ? 0 : blockIdx.z / p.nh, zh = p.ksplit ? 0 : blockIdx.z % p.nh;
     const int kz = p.ksplit * (int)blockIdx.z;
     const int m0 = blockIdx.y * TC_BM;
-    const int n0 = blockIdx.x * (p.nbox > 1 ? WG_UJ : TC_BN);     // first output column / first hidden unit (gate-interleaved tiles)
+    const int n0 = blockIdx.x * (p.nbox > 1 ? WG_UJ : BN);        // first output column / first hidden unit (gate-interleaved tiles)
 
     if (tid == 0) {
         for (int s = 0; s < ST; ++s) {
@@ -343,9 +371,9 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
 
     // ---------------------------------------------------------------------- consumer warpgroups (warps 0..7)
     const int wg = warp >> 2;
-    float acc[32];
+    float acc[BN / 2];
 #pragma unroll
-    for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
     const float* Fz = p.Fc ? p.Fc + (long long)blockIdx.z * p.ngrp * p.M : nullptr;
     {
         int i = 0;
@@ -355,7 +383,9 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                 const int s = i % ST;
                 mbar_wait(&full[s], (uint32_t)(i / ST) & 1u);
                 const uint32_t st_addr = smem_u32(smem + (size_t)s * Cfg::STAGE);
-                if constexpr (F16) {
+                if constexpr (WIDE) {
+                    // both operands arrived as operand images: nothing to convert
+                } else if constexpr (F16) {
                     // ---- raw fp32 slice -> operand image, in place: a 128-byte row of 32 floats becomes 64 B of hi halves | 64 B of lo halves.
                     // Chunk pair c2 (2 x 16 B = 8 floats) of a row -> hi chunk c2, lo chunk 4 + c2; the threads that share a row are
                     // neighbouring lanes of one warp: read, __syncwarp, write.
@@ -429,7 +459,7 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                     consumer_sync();
                 }
                 // ---- products of this warpgroup's 64 rows, small terms first: lo.hi, hi.lo, hi.hi per K step (+32 bytes inside the swizzled row)
-                float d[32];
+                float d[BN / 2];
                 const uint64_t da = make_smem_desc_sw128(st_addr + (uint32_t)wg * 64u * 128u);
                 const uint64_t db = make_smem_desc_sw128(st_addr + Cfg::B_OFF);
                 wgmma_fence();
@@ -456,7 +486,7 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty[s]);          // stage free once this warp's MMAs have read it
 #pragma unroll
-                for (int e = 0; e < 32; ++e) {
+                for (int e = 0; e < BN / 2; ++e) {
                     if constexpr (F16) acc[e] = fmaf(d[e], p.oscale, acc[e]);      // undo the power-of-two operand scales (exact)
                     else acc[e] += d[e];
                 }
@@ -471,16 +501,26 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
     {
         const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) {
+        for (int j = 0; j < BN / 8; ++j) {
             *reinterpret_cast<float2*>(Cs + r0 * LDS_ + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
             *reinterpret_cast<float2*>(Cs + (r0 + 8) * LDS_ + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
     }
     consumer_sync();
     const int q = warp & 3, row = q * 32 + lane, m = m0 + row;
-    const int cbeg = (warp >> 2) * 32;          // thread = (row, column half) in the modes that use all eight warps
+    const int cbeg = (warp >> 2) * (BN / 2);    // thread = (row, column half) in the modes that use all eight warps
 
-    if (p.mode == MODE_STORE) {
+    if constexpr (WIDE) {
+        // MODE_SS: this thread's 64 columns of row m
+        float a64[64];
+#pragma unroll
+        for (int j = 0; j < 64; j += 4) {
+            const float4 t = *reinterpret_cast<const float4*>(Cs + row * LDS_ + cbeg + j);
+            a64[j] = t.x; a64[j + 1] = t.y; a64[j + 2] = t.z; a64[j + 3] = t.w;
+        }
+        const bool vec_ok = (p.ss.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.ss.C) & 15) == 0);
+        ss_store_row<64>(p.ss, a64, m, n0 + cbeg, lane, vec_ok);
+    } else if (p.mode == MODE_STORE) {
         // bias / activation, whole contiguous row segments per store instruction (128-bit, coalesced)
         const float* bias = p.bias ? p.bias + zb * p.sBb : nullptr;
         float* C = p.C + zb * p.sCb + zh * p.sCh;
@@ -520,15 +560,6 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                 if (n < p.N) C[(long long)n * p.ldc + m] = Cs[row * LDS_ + cbeg + j] * p.alpha;
             }
         }
-    } else if (p.mode == MODE_SS) {
-        float a32[32];
-#pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-            const float4 t = *reinterpret_cast<const float4*>(Cs + row * LDS_ + cbeg + j);
-            a32[j] = t.x; a32[j + 1] = t.y; a32[j + 2] = t.z; a32[j + 3] = t.w;
-        }
-        const bool vec_ok = (p.ss.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.ss.C) & 15) == 0);
-        ss_store_row<32>(p.ss, a32, m, n0 + cbeg, lane, vec_ok);
     } else if (p.mode == MODE_PV_IMG) {
         // 4 columns = 2 hi words + 2 lo words: a 4-column group never straddles a 32-wide K slice of the Wo operand (the head stride sCh and
         // the column offsets are multiples of 4), 8-byte stores
@@ -768,16 +799,33 @@ __global__ void pack_f16x3_kernel(const float* __restrict__ W, long long ldw, in
     out[n * Kp + kb * 32 + 16 + pr] = f16x3_pack_pair(x0 - a0, x1 - a1);
 }
 
+// every mode but MODE_SS: 128 x 64 tiles
 int launch_wg(const CUtensorMap* mA, const CUtensorMap* mW, const TcParams& p, dim3 grid, cudaStream_t st) {
     static bool attr_set = false;
     if (!attr_set) {
-        GVD_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<false>::SMEM));
-        GVD_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<true>::SMEM));
+        GVD_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<false, TC_BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<false, TC_BN>::SMEM));
+        GVD_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<true, TC_BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<true, TC_BN>::SMEM));
         attr_set = true;
     }
+    GVD_REQUIRE(p.mode != MODE_SS, "tcgemm: MODE_SS runs on the 128-wide tiles (launch_wg_ss)");
     GVD_REQUIRE(p.f16 || (!p.apre && !p.wpre), "tcgemm: operand images belong to the fp16x3 products");
-    if (p.f16) GVD_CHECK_CUDA(gvd_launch(wg_gemm_kernel<true>, grid, dim3(WG_THREADS), WgCfg<true>::SMEM, st, mA[0], mA[1], mA[2], mW[0], mW[1], mW[2], p));
-    else GVD_CHECK_CUDA(gvd_launch(wg_gemm_kernel<false>, grid, dim3(WG_THREADS), WgCfg<false>::SMEM, st, mA[0], mA[1], mA[2], mW[0], mW[1], mW[2], p));
+    if (p.f16)
+        GVD_CHECK_CUDA(gvd_launch(wg_gemm_kernel<true, TC_BN>, grid, dim3(WG_THREADS), WgCfg<true, TC_BN>::SMEM, st, mA[0], mA[1], mA[2], mW[0], mW[1], mW[2], p));
+    else
+        GVD_CHECK_CUDA(gvd_launch(wg_gemm_kernel<false, TC_BN>, grid, dim3(WG_THREADS), WgCfg<false, TC_BN>::SMEM, st, mA[0], mA[1], mA[2], mW[0], mW[1], mW[2], p));
+    GVD_CHECK_LAUNCH();
+    return 0;
+}
+// MODE_SS: 128 x 128 tiles, both operands fp16x3 images (the W tensor map's box has TC_BN_SS rows)
+int launch_wg_ss(const CUtensorMap* mA, const CUtensorMap* mW, const TcParams& p, dim3 grid, cudaStream_t st) {
+    using Cfg = WgCfg<true, TC_BN_SS>;
+    static bool attr_set = false;
+    if (!attr_set) {
+        GVD_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<true, TC_BN_SS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
+        attr_set = true;
+    }
+    GVD_REQUIRE(p.mode == MODE_SS && p.f16 && p.apre && p.wpre && p.nbox <= 1 && !p.ksplit, "tcgemm: the 128-wide tiles serve MODE_SS only");
+    GVD_CHECK_CUDA(gvd_launch(wg_gemm_kernel<true, TC_BN_SS>, grid, dim3(WG_THREADS), Cfg::SMEM, st, mA[0], mA[1], mA[2], mW[0], mW[1], mW[2], p));
     GVD_CHECK_LAUNCH();
     return 0;
 }
@@ -970,7 +1018,7 @@ int gvd_gemm_f16ss(const float* Ap, long long lda, const float* Wp, long long ld
     CUtensorMap mA[3], mW[3];
     TcParams p{};
     GVD_TRY(make_map(&mA[0], Ap, Kp, M, lda, 1, 0, 1, 0, TC_BM, &p.a_mul_h, &p.a_mul_b));
-    GVD_TRY(make_map(&mW[0], Wp, Kp, N, ldw, 1, 0, 1, 0, TC_BN, &p.w_mul_h, &p.w_mul_b));
+    GVD_TRY(make_map(&mW[0], Wp, Kp, N, ldw, 1, 0, 1, 0, TC_BN_SS, &p.w_mul_h, &p.w_mul_b));
     mA[1] = mA[2] = mA[0];
     mW[1] = mW[2] = mW[0];
     p.nseg = 1;
@@ -987,7 +1035,7 @@ int gvd_gemm_f16ss(const float* Ap, long long lda, const float* Wp, long long ld
         s.k_img = reinterpret_cast<uint32_t*>(qkv->k_img); s.vt_img = reinterpret_cast<uint32_t*>(qkv->vt_img);
         s.qkv_sk = qkv->sk; s.qkv_sv = qkv->sv;
     }
-    return launch_wg(mA, mW, p, dim3(gvd_cdiv(N, TC_BN), gvd_cdiv(M, TC_BM), 1), st);
+    return launch_wg_ss(mA, mW, p, dim3(gvd_cdiv(N, TC_BN_SS), gvd_cdiv(M, TC_BM), 1), st);
 }
 
 // C = act(alpha * A W^T + bias) with the GemmArgs contract of gvd_gemm.cuh (batched over (b,h))
