@@ -295,11 +295,11 @@ class AttModel(CaptionModel):
 
     def _forward_tfm(self, segs_feat, gt_seq, ppls, num, ppls_feat, sample_idx, pnt_mask):
         """att_model='transformer' branch of _forward (model.py:411-419): the teacher-forced language loss and five zeros ("Masked Transformer
-        does not support box supervision yet"); 'GRD' takes the same branch in the reference.  Eval-mode arithmetic (no dropout); the backward
-        of the captioner is not built, so train mode is refused rather than faked."""
+        does not support box supervision yet"); 'GRD' takes the same branch in the reference.  Eval-mode arithmetic (no dropout).  The training
+        step of this captioner is gvd_b200.train.Trainer (TrainStep's transformer branch); train mode through this module is refused."""
         if self.training:
-            raise NotImplementedError("the transformer captioner's training step (dropout + backward) is not on the accelerated path; "
-                                      "call model.eval() for the teacher-forced loss")
+            raise NotImplementedError("the transformer captioner trains through gvd_b200.train.Trainer (adopt_module(model) shares the weights "
+                                      "with this module), not through model.train() + 'MLE'; call model.eval() for the teacher-forced loss")
         B, T = segs_feat.size(0), segs_feat.size(1)
         seq = torch.cat((gt_seq.new_zeros(B, 1), gt_seq[:, 0, :]), dim=1).long().contiguous()          # model.py:285-286
         if seq.numel() and (int(seq.min()) < 0 or int(seq.max()) >= self.vocab_size):

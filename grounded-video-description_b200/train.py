@@ -23,8 +23,14 @@ The primitive set `ops` (all tensors fp32, contiguous, on the device of `ops`):
     add, mul, scale, masked_fill, zeros_like / zeros, cat, clip_adam
 """
 import math
+import weakref
 
 import torch
+
+try:
+    from . import capi
+except ImportError:                        # drop-in layout: the package directory itself is on sys.path
+    import capi
 
 MIN_VALUE = -1e8
 
@@ -46,13 +52,18 @@ def head_chunks(H, n_heads=6):
 #   embed (:79-82, sub = decode step) lang_out (AttModel.py:161, sub = decode step) vis_word (model.py:470, second vis_embed call)
 DROP_SITES = {n: i for i, n in enumerate(("seg_info", "fc7", "vis_cls", "loc", "pool_embed", "fc_embed", "att_rgb", "att_mot", "attn", "res_attn",
                                           "res_ffn", "gru_l0", "embed", "lang_out", "vis_word"))}
+# The transformer captioner's decoder (att_model = 'transformer'; p = 0.2, model.py:137-142), numbered after the sites above so their masks do
+# not change:  tfm_embed (embedding + positional encoding, transformer.py:209)  tfm_attn (attention probabilities, :105,
+# sub = (layer * 2 + {0 self, 1 cross}) * 8 + head)  tfm_res (ResidualBlock, :88, sub = layer * 3 + {0 self, 1 cross, 2 feed-forward})
+TFM_DROP_SITES = {n: len(DROP_SITES) + i for i, n in enumerate(("tfm_embed", "tfm_attn", "tfm_res"))}
+_SITE_IDS = dict(DROP_SITES, **TFM_DROP_SITES)
 
 
 class TrainStep:
     """forward_backward(W, opt, inp) -> (losses[4], loss, grads{key});  step(...) adds clip + Adam (first step, main.py:660-677).
 
     dropout: None (every Dropout at p = 0: the deterministic parity mode the oracle pin uses) or dict(seed=int, p_lm=drop_prob_lm (opts.py: 0.5),
-    p_interact=0.2, p_gru=0.2, p_loc=0.5): train-mode masks at the reference's sites, drawn from counter-based Philox keyed by
+    p_interact=0.2, p_gru=0.2, p_loc=0.5, p_tfm=0.2): train-mode masks at the reference's sites, drawn from counter-based Philox keyed by
     (seed, site, optimisation step) so that the backward regenerates them."""
 
     def __init__(self, ops, dropout=None):
@@ -64,10 +75,17 @@ class TrainStep:
         d = self.dropout
         if not d:
             return x
-        p = {"lm": d.get("p_lm", 0.5), "interact": d.get("p_interact", 0.2), "gru": d.get("p_gru", 0.2), "loc": d.get("p_loc", 0.5)}[kind]
+        p = self._p(kind)
         if p <= 0.0:
             return x
-        return self.ops.dropout(x, p, d["seed"], DROP_SITES[site] * 4096 + sub, it)
+        return self.ops.dropout(x, p, d["seed"], _SITE_IDS[site] * 4096 + sub, it)
+
+    def _p(self, kind):
+        d = self.dropout
+        if not d:
+            return 0.0
+        return {"lm": d.get("p_lm", 0.5), "interact": d.get("p_interact", 0.2), "gru": d.get("p_gru", 0.2), "loc": d.get("p_loc", 0.5),
+                "tfm": d.get("p_tfm", 0.2)}[kind]
 
     # ------------------------------------------------------------------ helpers
     def _acc(self, grads, key, g):
@@ -162,11 +180,183 @@ class TrainStep:
         self._acc(grads, "context_enc.bias_ih" + sfx, ops.colsum(dgi2))
         return ops.mm_nn(dgi2, W["context_enc.weight_ih" + sfx]).reshape(B, T, -1)
 
+    # ------------------------------------------------------------------ prologue (model.py:504-568), shared by both captioners
+    def _prologue_fwd(self, W, opt, inp, pmask, keep_d, D_, frames=True, regions=True):
+        """Train-mode prologue; returns its tape.  frames / regions = False skips the frame branch / the region branch (the captioner does not
+        read it: att_input_mode 'region' / 'featmap' of the transformer, model.py:393)."""
+        ops = self.ops
+        H = opt.rnn_size
+        segs, ppls, num = inp["segs_feat"], inp["ppls"], inp["num"]
+        pt = dict(pmask=pmask, segs=segs, fc_feats=None, g_pool=None, simT=None, pool_feats=None, p_pool=None, conv=None, p_conv=None)
+        self.last_bn = None
+        fc = ops.mean_dim1(segs)
+        seg_in = num[:, 3:7].float().contiguous()
+        seg_h = D_(ops.lin(seg_in, W["seg_info_embed.0.weight"], W["seg_info_embed.0.bias"], True), "lm", "seg_info")
+        ln_fc, ln_seg = ops.ln(fc), ops.ln(seg_h)
+        xcat = ops.cat((ln_fc, ln_seg), -1)
+        fc_feats = D_(ops.lin(xcat, W["fc_embed.0.weight"], W["fc_embed.0.bias"], True), "lm", "fc_embed")
+        pt.update(fc=fc, seg_in=seg_in, seg_h=seg_h, ln_seg=ln_seg, xcat=xcat, fc_feats=fc_feats)
+
+        if regions:
+            ppls_feat = inp["ppls_feat"]
+            g_pool = D_(ops.lin(ppls_feat, W["ctx2pool_grd.0.weight"], W["ctx2pool_grd.0.bias"], True), "lm", "fc7")
+            Wc = D_(ops.relu(W["vis_embed.0.weight"]), "lm", "vis_cls")                     # ONE mask for the class table (model.py:320-321)
+            simT_raw = ops.lin(g_pool, Wc, W["vis_classifiers_bias"], False)                 # B, R, C (region-major)
+            simT_raw = ops.masked_fill(simT_raw, pmask.unsqueeze(-1).expand_as(simT_raw), MIN_VALUE)
+            simT = ops.softmax(simT_raw, 1.0)                                                # softmax over the classes
+
+            loc_in = ops.cat((ops.scale(ppls[:, :, :4].contiguous(), 1.0 / 720.0), ops.scale(ppls[:, :, 4:5].contiguous(), 1.0 / float(opt.num_sampled_frm))), -1)
+            loc = D_(ops.lin(loc_in, W["loc_fc.0.weight"], W["loc_fc.0.bias"], True), "loc", "loc")
+            ln_g, ln_loc, ln_sim = ops.ln(g_pool), ops.ln(loc), ops.ln(simT)
+            pool_in = ops.cat((ln_g, ln_loc, ln_sim), -1)
+            pool_embed = D_(ops.lin(pool_in, W["pool_embed.0.weight"], W["pool_embed.0.bias"], True), "lm", "pool_embed")
+            pool = pool_embed
+
+            it_tape = []
+            if opt.obj_interact:
+                sizes = head_chunks(H)
+                scale = 1.0 / math.sqrt(H)
+                x = pool
+                for l in range(2):
+                    p = "obj_interact.encoder.layers.%d." % l
+                    q = ops.lin(x, W[p + "selfattn.layer.wq.weight"], None, False)
+                    k = ops.lin(x, W[p + "selfattn.layer.wk.weight"], None, False)
+                    v = ops.lin(x, W[p + "selfattn.layer.wv.weight"], None, False)
+                    heads, outs, o = [], [], 0
+                    for hi, s in enumerate(sizes):
+                        qh, kh, vh = (t[..., o:o + s].contiguous() for t in (q, k, v))
+                        att = ops.softmax(ops.bmm_nt(qh, kh), scale)
+                        att_d = D_(att, "interact", "attn", l * 8 + hi)                     # transformer.py:100
+                        outs.append(ops.bmm_nn(att_d, vh))
+                        heads.append((att, qh, kh, vh, att_d))
+                        o += s
+                    cat = ops.cat(outs, -1)
+                    a = D_(ops.lin(cat, W[p + "selfattn.layer.wo.weight"], None, False), "interact", "res_attn", l)     # transformer.py:88
+                    x1_in = ops.add(x, a)
+                    x1 = ops.ln_star(x1_in, W[p + "selfattn.layernorm.gamma"], W[p + "selfattn.layernorm.beta"])
+                    f1 = ops.lin(x1, W[p + "feedforward.layer.linear1.weight"], W[p + "feedforward.layer.linear1.bias"], True)
+                    f2 = D_(ops.lin(f1, W[p + "feedforward.layer.linear2.weight"], W[p + "feedforward.layer.linear2.bias"], False), "interact", "res_ffn", l)
+                    x2_in = ops.add(x1, f2)
+                    x2 = ops.ln_star(x2_in, W[p + "feedforward.layernorm.gamma"], W[p + "feedforward.layernorm.beta"])
+                    it_tape.append(dict(l=l, p=p, x=x, heads=heads, cat=cat, x1_in=x1_in, x1=x1, f1=f1, x2_in=x2_in))
+                    x = x2
+                pool = x
+            pool_feats = pool
+            p_pool = ops.lin(pool_feats, W["ctx2pool.weight"], W["ctx2pool.bias"], False)
+            pt.update(ppls_feat=ppls_feat, g_pool=g_pool, Wc=Wc, simT=simT, loc_in=loc_in, loc=loc, ln_g=ln_g, ln_loc=ln_loc, ln_sim=ln_sim,
+                      pool_in=pool_in, pool_embed=pool_embed, it_tape=it_tape, pool_feats=pool_feats, p_pool=p_pool)
+
+        if frames:
+            e_rgb = D_(ops.lin(segs[..., :2048].contiguous(), W["att_embed.0.0.weight"], W["att_embed.0.0.bias"], True), "lm", "att_rgb")
+            e_mot = D_(ops.lin(segs[..., 2048:].contiguous(), W["att_embed.1.0.weight"], W["att_embed.1.0.bias"], True), "lm", "att_mot")
+            e = ops.cat((e_rgb, e_mot), -1)
+            bn = "att_embed_aux.0."
+            Bt, T = e.shape[0], e.shape[1]
+            e2 = e.reshape(Bt * T, -1)
+            e_hat, bn_var = ops.bn_train(e2)                                                # statistics of this batch (train mode)
+            self.last_bn = (ops.scale(ops.colsum(e2), 1.0 / (Bt * T)), bn_var, Bt * T)       # batch mean / biased variance / count: running-stat update
+            e_bn = ops.add(ops.mul(e_hat, W[bn + "weight"].unsqueeze(0).expand_as(e_hat).contiguous()), W[bn + "bias"].unsqueeze(0).expand_as(e_hat).contiguous())
+            gx = ops.relu(e_bn).reshape(Bt, T, -1)
+            gru_tapes, gin = [], gx
+            for layer in range(2):
+                of, tf = self._gru_dir_fwd(gin, W, layer, False)
+                ob, tb = self._gru_dir_fwd(gin, W, layer, True)
+                gru_tapes.append((tf, tb))
+                gin = ops.cat((of, ob), -1)
+                if layer == 0:
+                    gin = D_(gin, "gru", "gru_l0")                                            # nn.GRU(dropout=0.2): between the layers only
+            keep = keep_d.expand(Bt, T, gin.shape[-1]).contiguous()
+            conv = ops.mul(gin, keep)
+            p_conv = ops.lin(conv, W["ctx2att.weight"], W["ctx2att.bias"], False)
+            pt.update(e_rgb=e_rgb, e_mot=e_mot, e_hat=e_hat, bn_var=bn_var, e_bn=e_bn, gru_tapes=gru_tapes, keep=keep, conv=conv, p_conv=p_conv)
+        return pt
+
+    def _prologue_bwd(self, pt, W, opt, grads, D_, dconv=None, dp_conv=None, dfc_feats=None, dpool_feats=None, dp_pool=None, dg_pool=None, dsimT=None):
+        """Backward of _prologue_fwd for the gradients of its outputs (None = the captioner did not read that output: its parameters get no
+        gradient).  Accumulates into `grads`."""
+        ops = self.ops
+        H = opt.rnn_size
+        if dp_conv is not None:
+            dconv = ops.add(dconv, self._lin_bwd(dp_conv, pt["conv"], W, "ctx2att", grads))
+        if dconv is not None:
+            e_bn, e_hat, e_rgb, e_mot, segs, bn = pt["e_bn"], pt["e_hat"], pt["e_rgb"], pt["e_mot"], pt["segs"], "att_embed_aux.0."
+            Bt, T = e_rgb.shape[0], e_rgb.shape[1]
+            dgin = ops.mul(dconv, pt["keep"])
+            G = dgin.shape[-1] // 2
+            for layer in (1, 0):
+                tf, tb = pt["gru_tapes"][layer]
+                if layer == 0:
+                    dgin = D_(dgin, "gru", "gru_l0")
+                dgin = ops.add(self._gru_dir_bwd(dgin[..., :G].contiguous(), tf, W, grads), self._gru_dir_bwd(dgin[..., G:].contiguous(), tb, W, grads))
+            de_bn = ops.relu_bwd(dgin.reshape(Bt * T, -1), e_bn)
+            self._acc(grads, bn + "weight", ops.colsum(ops.mul(de_bn, e_hat)))
+            self._acc(grads, bn + "bias", ops.colsum(de_bn))
+            dxh = ops.mul(de_bn, W[bn + "weight"].unsqueeze(0).expand_as(de_bn).contiguous())
+            de = ops.bn_train_bwd(dxh, e_hat, pt["bn_var"]).reshape(Bt, T, -1)
+            Hh = e_rgb.shape[-1]
+            de_rgb = ops.relu_bwd(D_(de[..., :Hh].contiguous(), "lm", "att_rgb"), e_rgb)
+            de_mot = ops.relu_bwd(D_(de[..., Hh:].contiguous(), "lm", "att_mot"), e_mot)
+            self._lin_bwd(de_rgb, segs[..., :2048].contiguous(), W, "att_embed.0.0", grads, need_dx=False)
+            self._lin_bwd(de_mot, segs[..., 2048:].contiguous(), W, "att_embed.1.0", grads, need_dx=False)
+
+        if dfc_feats is not None:
+            fc_feats, seg_h = pt["fc_feats"], pt["seg_h"]
+            dxcat = self._lin_bwd(ops.relu_bwd(D_(dfc_feats, "lm", "fc_embed"), fc_feats), pt["xcat"], W, "fc_embed.0", grads)
+            dseg_h = ops.relu_bwd(D_(ops.ln_bwd(dxcat[:, pt["fc"].shape[1]:].contiguous(), pt["ln_seg"], seg_h), "lm", "seg_info"), seg_h)
+            self._lin_bwd(dseg_h, pt["seg_in"], W, "seg_info_embed.0", grads, need_dx=False)
+
+        if dpool_feats is None:
+            return
+        pool_feats, g_pool, simT, loc, pmask = pt["pool_feats"], pt["g_pool"], pt["simT"], pt["loc"], pt["pmask"]
+        dpool = ops.add(dpool_feats, self._lin_bwd(dp_pool, pool_feats, W, "ctx2pool", grads)) if dp_pool is not None else dpool_feats
+        if opt.obj_interact:
+            sizes = head_chunks(H)
+            scale = 1.0 / math.sqrt(H)
+            for tp in reversed(pt["it_tape"]):
+                p = tp["p"]
+                dx2_in, dg_, db_ = ops.ln_star_bwd(dpool, tp["x2_in"], W[p + "feedforward.layernorm.gamma"])
+                self._acc(grads, p + "feedforward.layernorm.gamma", dg_)
+                self._acc(grads, p + "feedforward.layernorm.beta", db_)
+                df1 = ops.relu_bwd(self._lin_bwd(D_(dx2_in, "interact", "res_ffn", tp["l"]), tp["f1"], W, p + "feedforward.layer.linear2", grads), tp["f1"])
+                dx1 = ops.add(dx2_in, self._lin_bwd(df1, tp["x1"], W, p + "feedforward.layer.linear1", grads))
+                dx1_in, dg_, db_ = ops.ln_star_bwd(dx1, tp["x1_in"], W[p + "selfattn.layernorm.gamma"])
+                self._acc(grads, p + "selfattn.layernorm.gamma", dg_)
+                self._acc(grads, p + "selfattn.layernorm.beta", db_)
+                dcat = self._lin_bwd(D_(dx1_in, "interact", "res_attn", tp["l"]), tp["cat"], W, p + "selfattn.layer.wo", grads)
+                dqs, dks, dvs, o = [], [], [], 0
+                for hi, (s, (att, qh, kh, vh, att_d)) in enumerate(zip(sizes, tp["heads"])):
+                    do = dcat[..., o:o + s].contiguous()
+                    dvs.append(ops.bmm_tn(att_d, do))                                    # (dropped att)^T do
+                    dsc = ops.softmax_bwd(D_(ops.bmm_nt(do, vh), "interact", "attn", tp["l"] * 8 + hi), att, scale)
+                    dqs.append(ops.bmm_nn(dsc, kh))
+                    dks.append(ops.bmm_tn(dsc, qh))
+                    o += s
+                dx = dx1_in
+                for nm, parts in (("wq", dqs), ("wk", dks), ("wv", dvs)):
+                    dx = ops.add(dx, self._lin_bwd(ops.cat(parts, -1), tp["x"], W, p + "selfattn.layer.%s" % nm, grads))
+                dpool = dx
+        dpool_in = self._lin_bwd(ops.relu_bwd(D_(dpool, "lm", "pool_embed"), pt["pool_embed"]), pt["pool_in"], W, "pool_embed.0", grads)
+        n_g, n_l = g_pool.shape[-1], loc.shape[-1]
+        dg_ln = ops.ln_bwd(dpool_in[..., :n_g].contiguous(), pt["ln_g"], g_pool)
+        dg_pool = dg_ln if dg_pool is None else ops.add(dg_pool, dg_ln)
+        dloc = ops.relu_bwd(D_(ops.ln_bwd(dpool_in[..., n_g:n_g + n_l].contiguous(), pt["ln_loc"], loc), "loc", "loc"), loc)
+        self._lin_bwd(dloc, pt["loc_in"], W, "loc_fc.0", grads, need_dx=False)
+        dsim_ln = ops.ln_bwd(dpool_in[..., n_g + n_l:].contiguous(), pt["ln_sim"], simT)
+        dsimT = dsim_ln if dsimT is None else ops.add(dsimT, dsim_ln)
+        dsim_raw = ops.masked_fill(ops.softmax_bwd(dsimT, simT, 1.0), pmask.unsqueeze(-1).expand_as(simT), 0.0)      # B, R, C
+        dsr2, gp2 = dsim_raw.reshape(-1, dsim_raw.shape[-1]), g_pool.reshape(-1, n_g)
+        dg_pool = ops.add(dg_pool, ops.mm_nn(dsr2, pt["Wc"]).reshape(tuple(g_pool.shape)))
+        self._acc(grads, "vis_embed.0.weight", ops.relu_bwd(D_(ops.mm_tn(dsr2, gp2), "lm", "vis_cls"), W["vis_embed.0.weight"]))
+        self._acc(grads, "vis_classifiers_bias", ops.colsum(dsr2))
+        self._lin_bwd(ops.relu_bwd(D_(dg_pool, "lm", "fc7"), g_pool), pt["ppls_feat"], W, "ctx2pool_grd.0", grads, need_dx=False)
+
     # ------------------------------------------------------------------ the step
     def forward(self, W, opt, inp, host=None):
         """Teacher-forced forward in train mode; returns (the four losses, backward) where backward(w_lm, w_att2, w_grd, w_cls)
         runs the explicit backward for the given loss weights.  `inp` tensors on the device of `ops`; `host` = the CPU copies of the integer / mask inputs that drive control flow
         (targets of the teacher forcing, the early exit `seq[:, i].sum() == 0`, model.py:425) — defaults to `inp`."""
+        if getattr(opt, "att_model", "topdown") == "transformer":
+            return self._tfm_forward(W, opt, inp, host)
         ops = self.ops
         host = host or inp
         it = self.iter                                                                  # keys this step's dropout masks (forward AND backward)
@@ -193,82 +383,9 @@ class TrainStep:
         txt_mask_d = ops.to_device(txt_mask_h)
         cls_idx = ops.to_device(cls_idx_h.reshape(-1).contiguous())
 
-        # ========================================================== forward, prologue
-        segs, ppls, num = inp["segs_feat"], inp["ppls"], inp["num"]
-        fc = ops.mean_dim1(segs)
-        seg_in = num[:, 3:7].float().contiguous()
-        seg_h = D_(ops.lin(seg_in, W["seg_info_embed.0.weight"], W["seg_info_embed.0.bias"], True), "lm", "seg_info")
-        ln_fc, ln_seg = ops.ln(fc), ops.ln(seg_h)
-        xcat = ops.cat((ln_fc, ln_seg), -1)
-        fc_feats = D_(ops.lin(xcat, W["fc_embed.0.weight"], W["fc_embed.0.bias"], True), "lm", "fc_embed")
-
-        ppls_feat = inp["ppls_feat"]
-        g_pool = D_(ops.lin(ppls_feat, W["ctx2pool_grd.0.weight"], W["ctx2pool_grd.0.bias"], True), "lm", "fc7")
-        Wc = D_(ops.relu(W["vis_embed.0.weight"]), "lm", "vis_cls")                     # ONE mask for the class table (model.py:320-321)
-        simT_raw = ops.lin(g_pool, Wc, W["vis_classifiers_bias"], False)                 # B, R, C (region-major)
-        simT_raw = ops.masked_fill(simT_raw, pmask.unsqueeze(-1).expand_as(simT_raw), MIN_VALUE)
-        simT = ops.softmax(simT_raw, 1.0)                                                # softmax over the classes
-
-        loc_in = ops.cat((ops.scale(ppls[:, :, :4].contiguous(), 1.0 / 720.0), ops.scale(ppls[:, :, 4:5].contiguous(), 1.0 / float(opt.num_sampled_frm))), -1)
-        loc = D_(ops.lin(loc_in, W["loc_fc.0.weight"], W["loc_fc.0.bias"], True), "loc", "loc")
-        ln_g, ln_loc, ln_sim = ops.ln(g_pool), ops.ln(loc), ops.ln(simT)
-        pool_in = ops.cat((ln_g, ln_loc, ln_sim), -1)
-        pool_embed = D_(ops.lin(pool_in, W["pool_embed.0.weight"], W["pool_embed.0.bias"], True), "lm", "pool_embed")
-        pool = pool_embed
-
-        it_tape = []
-        if opt.obj_interact:
-            sizes = head_chunks(H)
-            scale = 1.0 / math.sqrt(H)
-            x = pool
-            for l in range(2):
-                p = "obj_interact.encoder.layers.%d." % l
-                q = ops.lin(x, W[p + "selfattn.layer.wq.weight"], None, False)
-                k = ops.lin(x, W[p + "selfattn.layer.wk.weight"], None, False)
-                v = ops.lin(x, W[p + "selfattn.layer.wv.weight"], None, False)
-                heads, outs, o = [], [], 0
-                for hi, s in enumerate(sizes):
-                    qh, kh, vh = (t[..., o:o + s].contiguous() for t in (q, k, v))
-                    att = ops.softmax(ops.bmm_nt(qh, kh), scale)
-                    att_d = D_(att, "interact", "attn", l * 8 + hi)                     # transformer.py:100
-                    outs.append(ops.bmm_nn(att_d, vh))
-                    heads.append((att, qh, kh, vh, att_d))
-                    o += s
-                cat = ops.cat(outs, -1)
-                a = D_(ops.lin(cat, W[p + "selfattn.layer.wo.weight"], None, False), "interact", "res_attn", l)     # transformer.py:88
-                x1_in = ops.add(x, a)
-                x1 = ops.ln_star(x1_in, W[p + "selfattn.layernorm.gamma"], W[p + "selfattn.layernorm.beta"])
-                f1 = ops.lin(x1, W[p + "feedforward.layer.linear1.weight"], W[p + "feedforward.layer.linear1.bias"], True)
-                f2 = D_(ops.lin(f1, W[p + "feedforward.layer.linear2.weight"], W[p + "feedforward.layer.linear2.bias"], False), "interact", "res_ffn", l)
-                x2_in = ops.add(x1, f2)
-                x2 = ops.ln_star(x2_in, W[p + "feedforward.layernorm.gamma"], W[p + "feedforward.layernorm.beta"])
-                it_tape.append(dict(l=l, p=p, x=x, heads=heads, cat=cat, x1_in=x1_in, x1=x1, f1=f1, x2_in=x2_in))
-                x = x2
-            pool = x
-        pool_feats = pool
-        p_pool = ops.lin(pool_feats, W["ctx2pool.weight"], W["ctx2pool.bias"], False)
-
-        e_rgb = D_(ops.lin(segs[..., :2048].contiguous(), W["att_embed.0.0.weight"], W["att_embed.0.0.bias"], True), "lm", "att_rgb")
-        e_mot = D_(ops.lin(segs[..., 2048:].contiguous(), W["att_embed.1.0.weight"], W["att_embed.1.0.bias"], True), "lm", "att_mot")
-        e = ops.cat((e_rgb, e_mot), -1)
-        bn = "att_embed_aux.0."
-        Bt, T = e.shape[0], e.shape[1]
-        e2 = e.reshape(Bt * T, -1)
-        e_hat, bn_var = ops.bn_train(e2)                                                # statistics of this batch (train mode)
-        self.last_bn = (ops.scale(ops.colsum(e2), 1.0 / (Bt * T)), bn_var, Bt * T)       # batch mean / biased variance / count: running-stat update
-        e_bn = ops.add(ops.mul(e_hat, W[bn + "weight"].unsqueeze(0).expand_as(e_hat).contiguous()), W[bn + "bias"].unsqueeze(0).expand_as(e_hat).contiguous())
-        gx = ops.relu(e_bn).reshape(Bt, T, -1)
-        gru_tapes, gin = [], gx
-        for layer in range(2):
-            of, tf = self._gru_dir_fwd(gin, W, layer, False)
-            ob, tb = self._gru_dir_fwd(gin, W, layer, True)
-            gru_tapes.append((tf, tb))
-            gin = ops.cat((of, ob), -1)
-            if layer == 0:
-                gin = D_(gin, "gru", "gru_l0")                                            # nn.GRU(dropout=0.2): between the layers only
-        keep = keep_d.expand(Bt, T, gin.shape[-1]).contiguous()
-        conv = ops.mul(gin, keep)
-        p_conv = ops.lin(conv, W["ctx2att.weight"], W["ctx2att.bias"], False)
+        pt = self._prologue_fwd(W, opt, inp, pmask, keep_d, D_)
+        fc_feats, g_pool, simT, pool_feats, p_pool, conv, p_conv = (pt[k] for k in ("fc_feats", "g_pool", "simT", "pool_feats", "p_pool", "conv",
+                                                                                      "p_conv"))
 
         # ========================================================== forward, teacher-forced loop
         tgt = ops.host_targets(self, opt, inp, host)                                     # overlaps, class targets, per-step labels / masks
@@ -357,72 +474,116 @@ class TrainStep:
                 dembed = ops.add(dembed, ops.index_add_rows(dembed.shape[0], st["tok"], ops.relu_bwd(D_(dx_att[:, H:H + E].contiguous(), "lm", "embed", i), st["emb_raw"])))
             self._acc(grads, "embed.0.weight", dembed)
 
-            # ========================================================== backward, prologue
-            dconv = ops.add(dconv, self._lin_bwd(dp_conv, conv, W, "ctx2att", grads))
-            dgin = ops.mul(dconv, keep)
-            G = dgin.shape[-1] // 2
-            for layer in (1, 0):
-                tf, tb = gru_tapes[layer]
-                if layer == 0:
-                    dgin = D_(dgin, "gru", "gru_l0")
-                dgin = ops.add(self._gru_dir_bwd(dgin[..., :G].contiguous(), tf, W, grads), self._gru_dir_bwd(dgin[..., G:].contiguous(), tb, W, grads))
-            de_bn = ops.relu_bwd(dgin.reshape(Bt * T, -1), e_bn)
-            self._acc(grads, bn + "weight", ops.colsum(ops.mul(de_bn, e_hat)))
-            self._acc(grads, bn + "bias", ops.colsum(de_bn))
-            dxh = ops.mul(de_bn, W[bn + "weight"].unsqueeze(0).expand_as(de_bn).contiguous())
-            de = ops.bn_train_bwd(dxh, e_hat, bn_var).reshape(Bt, T, -1)
-            Hh = e_rgb.shape[-1]
-            de_rgb = ops.relu_bwd(D_(de[..., :Hh].contiguous(), "lm", "att_rgb"), e_rgb)
-            de_mot = ops.relu_bwd(D_(de[..., Hh:].contiguous(), "lm", "att_mot"), e_mot)
-            self._lin_bwd(de_rgb, segs[..., :2048].contiguous(), W, "att_embed.0.0", grads, need_dx=False)
-            self._lin_bwd(de_mot, segs[..., 2048:].contiguous(), W, "att_embed.1.0", grads, need_dx=False)
-
-            dxcat = self._lin_bwd(ops.relu_bwd(D_(dfc_feats, "lm", "fc_embed"), fc_feats), xcat, W, "fc_embed.0", grads)
-            dseg_h = ops.relu_bwd(D_(ops.ln_bwd(dxcat[:, fc.shape[1]:].contiguous(), ln_seg, seg_h), "lm", "seg_info"), seg_h)
-            self._lin_bwd(dseg_h, seg_in, W, "seg_info_embed.0", grads, need_dx=False)
-
-            dpool = ops.add(dpool_feats, self._lin_bwd(dp_pool, pool_feats, W, "ctx2pool", grads))
-            if opt.obj_interact:
-                sizes = head_chunks(H)
-                scale = 1.0 / math.sqrt(H)
-                for tp in reversed(it_tape):
-                    p = tp["p"]
-                    dx2_in, dg_, db_ = ops.ln_star_bwd(dpool, tp["x2_in"], W[p + "feedforward.layernorm.gamma"])
-                    self._acc(grads, p + "feedforward.layernorm.gamma", dg_)
-                    self._acc(grads, p + "feedforward.layernorm.beta", db_)
-                    df1 = ops.relu_bwd(self._lin_bwd(D_(dx2_in, "interact", "res_ffn", tp["l"]), tp["f1"], W, p + "feedforward.layer.linear2", grads), tp["f1"])
-                    dx1 = ops.add(dx2_in, self._lin_bwd(df1, tp["x1"], W, p + "feedforward.layer.linear1", grads))
-                    dx1_in, dg_, db_ = ops.ln_star_bwd(dx1, tp["x1_in"], W[p + "selfattn.layernorm.gamma"])
-                    self._acc(grads, p + "selfattn.layernorm.gamma", dg_)
-                    self._acc(grads, p + "selfattn.layernorm.beta", db_)
-                    dcat = self._lin_bwd(D_(dx1_in, "interact", "res_attn", tp["l"]), tp["cat"], W, p + "selfattn.layer.wo", grads)
-                    dqs, dks, dvs, o = [], [], [], 0
-                    for hi, (s, (att, qh, kh, vh, att_d)) in enumerate(zip(sizes, tp["heads"])):
-                        do = dcat[..., o:o + s].contiguous()
-                        dvs.append(ops.bmm_tn(att_d, do))                                    # (dropped att)^T do
-                        dsc = ops.softmax_bwd(D_(ops.bmm_nt(do, vh), "interact", "attn", tp["l"] * 8 + hi), att, scale)
-                        dqs.append(ops.bmm_nn(dsc, kh))
-                        dks.append(ops.bmm_tn(dsc, qh))
-                        o += s
-                    dx = dx1_in
-                    for nm, parts in (("wq", dqs), ("wk", dks), ("wv", dvs)):
-                        dx = ops.add(dx, self._lin_bwd(ops.cat(parts, -1), tp["x"], W, p + "selfattn.layer.%s" % nm, grads))
-                    dpool = dx
-            dpool_in = self._lin_bwd(ops.relu_bwd(D_(dpool, "lm", "pool_embed"), pool_embed), pool_in, W, "pool_embed.0", grads)
-            n_g, n_l = g_pool.shape[-1], loc.shape[-1]
-            dg_pool = ops.add(dg_pool, ops.ln_bwd(dpool_in[..., :n_g].contiguous(), ln_g, g_pool))
-            dloc = ops.relu_bwd(D_(ops.ln_bwd(dpool_in[..., n_g:n_g + n_l].contiguous(), ln_loc, loc), "loc", "loc"), loc)
-            self._lin_bwd(dloc, loc_in, W, "loc_fc.0", grads, need_dx=False)
-            dsimT = ops.add(dsimT, ops.ln_bwd(dpool_in[..., n_g + n_l:].contiguous(), ln_sim, simT))
-            dsim_raw = ops.masked_fill(ops.softmax_bwd(dsimT, simT, 1.0), pmask.unsqueeze(-1).expand_as(simT), 0.0)      # B, R, C
-            dsr2, gp2 = dsim_raw.reshape(-1, dsim_raw.shape[-1]), g_pool.reshape(-1, n_g)
-            dg_pool = ops.add(dg_pool, ops.mm_nn(dsr2, Wc).reshape(tuple(g_pool.shape)))
-            self._acc(grads, "vis_embed.0.weight", ops.relu_bwd(D_(ops.mm_tn(dsr2, gp2), "lm", "vis_cls"), W["vis_embed.0.weight"]))
-            self._acc(grads, "vis_classifiers_bias", ops.colsum(dsr2))
-            self._lin_bwd(ops.relu_bwd(D_(dg_pool, "lm", "fc7"), g_pool), ppls_feat, W, "ctx2pool_grd.0", grads, need_dx=False)
+            self._prologue_bwd(pt, W, opt, grads, D_, dconv=dconv, dp_conv=dp_conv, dfc_feats=dfc_feats, dpool_feats=dpool_feats, dp_pool=dp_pool,
+                               dg_pool=dg_pool, dsimT=dsimT)
             return grads
 
         return [lm, att2_loss, grd_loss, cls_loss], backward
+
+    def _tfm_forward(self, W, opt, inp, host=None):
+        """att_model = 'transformer' (model.py:404-419): the train-mode prologue, then the teacher-forced decoder of TransformerDecoder.forward
+        (transformer.py:207-212,276-283) over seq = [0, gt_seq][:, :-1] and F.cross_entropy over the positions whose target is non-zero.  Returns
+        ([lm, 0, 0, 0], backward) like forward(): the captioner has no box supervision, so only w_lm is read."""
+        ops = self.ops
+        host = host or inp
+        it = self.iter
+        self.iter += 1
+        D_ = lambda x, kind, site, sub=0: self._drop(x, kind, site, sub, it)
+        B = inp["ppls"].shape[0]
+        H, L, V = opt.rnn_size, opt.seq_length, opt.vocab_size
+        mode = opt.att_input_mode
+        if mode not in ("both", "featmap", "region"):
+            raise NotImplementedError(mode)
+        seq_h = torch.cat((torch.zeros(B, 1, dtype=torch.long), host["gt_seq"][:, 0, :].cpu().long()), dim=1)       # model.py:285-286
+        if int(seq_h.min()) < 0 or int(seq_h.max()) >= V:
+            raise IndexError("caption token id outside [0, %d)" % V)
+        s_in_h, tgt_h = seq_h[:, :-1].contiguous(), seq_h[:, 1:].contiguous()
+        keep_tok_h = tgt_h != 0
+        if not bool(keep_tok_h.any()):
+            # the reference's cross_entropy over no position is NaN and Adam would write NaN into every weight
+            raise capi.GvdError("no caption position has a non-zero target: the language loss is a mean over nothing")
+        T_ = inp["segs_feat"].shape[1]
+        sidx = host["sample_idx"].cpu()
+        tt = torch.arange(T_).view(1, T_)
+        keep_h = ((tt >= sidx[:, 0:1]) & (tt < sidx[:, 1:2])).unsqueeze(-1).float()
+        pe_h = capi.positional_encodings(L, H).unsqueeze(0).expand(B, L, H).contiguous()
+        s_in = ops.to_device(s_in_h.reshape(-1))                                           # one upload burst before any kernel of the step
+        tgt = ops.to_device(tgt_h)
+        keep_tok = ops.to_device(keep_tok_h)
+        keep_d = ops.to_device(keep_h.contiguous())
+        pe = ops.to_device(pe_h)
+
+        frames, regions = mode != "region", mode != "featmap"
+        pt = self._prologue_fwd(W, opt, inp, inp["pnt_mask"][:, 1:].bool(), keep_d, D_, frames=frames, regions=regions)
+        enc = {"both": ("conv", "pool_feats"), "featmap": ("conv", "conv"), "region": ("pool_feats", "pool_feats")}[mode]
+
+        scale = 1.0 / math.sqrt(H)
+        p_att = self._p("tfm")
+        seed = self.dropout["seed"] if self.dropout else 0
+        site = lambda l, cross: _SITE_IDS["tfm_attn"] * 4096 + (l * 2 + cross) * 8
+        dec = "cap_model.decoder."
+        emb_raw = ops.gather_rows(W[dec + "out.weight"], s_in).reshape(B, L, H)
+        x = D_(ops.add(ops.scale(emb_raw, math.sqrt(H)), pe), "tfm", "tfm_embed")              # F.embedding(x, out.weight * sqrt(d)) + pe
+        tape = []
+        for l in range(2):
+            p = dec + "layers.%d." % l
+            e = pt[enc[l]]
+            q = ops.lin(x, W[p + "selfattn.layer.wq.weight"], None, False)
+            k = ops.lin(x, W[p + "selfattn.layer.wk.weight"], None, False)
+            v = ops.lin(x, W[p + "selfattn.layer.wv.weight"], None, False)
+            a, lse = ops.mha_fwd(q, k, v, True, scale, p_att, seed, site(l, 0), it)
+            x1_in = ops.add(x, D_(ops.lin(a, W[p + "selfattn.layer.wo.weight"], None, False), "tfm", "tfm_res", l * 3))
+            x1 = ops.ln_star(x1_in, W[p + "selfattn.layernorm.gamma"], W[p + "selfattn.layernorm.beta"])
+            q2 = ops.lin(x1, W[p + "attention.layer.wq.weight"], None, False)
+            k2 = ops.lin(e, W[p + "attention.layer.wk.weight"], None, False)
+            v2 = ops.lin(e, W[p + "attention.layer.wv.weight"], None, False)
+            c, lse2 = ops.mha_fwd(q2, k2, v2, False, scale, p_att, seed, site(l, 1), it)
+            x2_in = ops.add(x1, D_(ops.lin(c, W[p + "attention.layer.wo.weight"], None, False), "tfm", "tfm_res", l * 3 + 1))
+            x2 = ops.ln_star(x2_in, W[p + "attention.layernorm.gamma"], W[p + "attention.layernorm.beta"])
+            f1 = ops.lin(x2, W[p + "feedforward.layer.linear1.weight"], W[p + "feedforward.layer.linear1.bias"], True)
+            f2 = D_(ops.lin(f1, W[p + "feedforward.layer.linear2.weight"], W[p + "feedforward.layer.linear2.bias"], False), "tfm", "tfm_res", l * 3 + 2)
+            x3_in = ops.add(x2, f2)
+            tape.append(dict(p=p, e=e, x=x, q=q, k=k, v=v, a=a, lse=lse, x1_in=x1_in, x1=x1, q2=q2, k2=k2, v2=v2, c=c, lse2=lse2, x2_in=x2_in,
+                             x2=x2, f1=f1, x3_in=x3_in))
+            x = ops.ln_star(x3_in, W[p + "feedforward.layernorm.gamma"], W[p + "feedforward.layernorm.beta"])
+        logits = ops.lin(x, W[dec + "out.weight"], W[dec + "out.bias"], False)                 # every position; the loss keeps the non-zero targets
+        lm, dlogits = ops.lm_nll(logits, tgt, keep_tok)
+        zero = ops.zeros((1,))
+
+        def backward(w_lm, w_att2=0.0, w_grd=0.0, w_cls=0.0):
+            grads = {}
+            dx = self._lin_bwd(ops.scale(dlogits, w_lm), x, W, dec + "out", grads)
+            denc = {}
+            for l in (1, 0):
+                t = tape[l]
+                p = t["p"]
+                dx3_in, dg_, db_ = ops.ln_star_bwd(dx, t["x3_in"], W[p + "feedforward.layernorm.gamma"])
+                self._acc(grads, p + "feedforward.layernorm.gamma", dg_)
+                self._acc(grads, p + "feedforward.layernorm.beta", db_)
+                df1 = ops.relu_bwd(self._lin_bwd(D_(dx3_in, "tfm", "tfm_res", l * 3 + 2), t["f1"], W, p + "feedforward.layer.linear2", grads), t["f1"])
+                dx2 = ops.add(dx3_in, self._lin_bwd(df1, t["x2"], W, p + "feedforward.layer.linear1", grads))
+                dx2_in, dg_, db_ = ops.ln_star_bwd(dx2, t["x2_in"], W[p + "attention.layernorm.gamma"])
+                self._acc(grads, p + "attention.layernorm.gamma", dg_)
+                self._acc(grads, p + "attention.layernorm.beta", db_)
+                dc = self._lin_bwd(D_(dx2_in, "tfm", "tfm_res", l * 3 + 1), t["c"], W, p + "attention.layer.wo", grads)
+                dq2, dk2, dv2 = ops.mha_bwd(dc, t["q2"], t["k2"], t["v2"], t["c"], t["lse2"], False, scale, p_att, seed, site(l, 1), it)
+                dx1 = ops.add(dx2_in, self._lin_bwd(dq2, t["x1"], W, p + "attention.layer.wq", grads))
+                de = ops.add(self._lin_bwd(dk2, t["e"], W, p + "attention.layer.wk", grads), self._lin_bwd(dv2, t["e"], W, p + "attention.layer.wv", grads))
+                denc[enc[l]] = de if enc[l] not in denc else ops.add(denc[enc[l]], de)      # d enc = dK Wk + dV Wv, summed over the layers
+                dx1_in, dg_, db_ = ops.ln_star_bwd(dx1, t["x1_in"], W[p + "selfattn.layernorm.gamma"])
+                self._acc(grads, p + "selfattn.layernorm.gamma", dg_)
+                self._acc(grads, p + "selfattn.layernorm.beta", db_)
+                da = self._lin_bwd(D_(dx1_in, "tfm", "tfm_res", l * 3), t["a"], W, p + "selfattn.layer.wo", grads)
+                dq, dk, dv = ops.mha_bwd(da, t["q"], t["k"], t["v"], t["a"], t["lse"], True, scale, p_att, seed, site(l, 0), it)
+                dx = dx1_in
+                for nm, g in (("wq", dq), ("wk", dk), ("wv", dv)):
+                    dx = ops.add(dx, self._lin_bwd(g, t["x"], W, p + "selfattn.layer.%s" % nm, grads))
+            demb = D_(dx, "tfm", "tfm_embed").reshape(B * L, H)
+            self._acc(grads, dec + "out.weight", ops.scale(ops.index_add_rows(V, s_in, demb), math.sqrt(H)))     # the tied embedding
+            self._prologue_bwd(pt, W, opt, grads, D_, dconv=denc.get("conv"), dpool_feats=denc.get("pool_feats"))
+            return grads
+
+        return [lm, zero, zero, zero], backward
 
     def forward_backward(self, W, opt, inp, n_replicas=1, host=None):
         """loss = (lm + w_att2 att2 + w_grd grd + w_cls cls) / n_replicas with the zero-weight terms dropped (main.py:238-255)."""
@@ -483,8 +644,9 @@ class Trainer:
         BatchNorm running statistics (train-mode side effect of model.py:114; rank-local like DataParallel's replica 0)
 
     `W` (the dict handed out by `.weights`) holds VIEWS into `flat_w`, so a module whose parameters are re-pointed at them
-    (`adopt_module`) trains in place.  Tensors that never receive a gradient (core.i2h_2 / h2h_2, quirk Q10) keep lr 0 in the table:
-    torch.optim.Adam skips them as well."""
+    (`adopt_module`) trains in place.  Tensors that receive no gradient keep lr 0 in the table and come out of a step unchanged, as
+    torch.optim.Adam skips them: core.i2h_2 / h2h_2 (quirk Q10) from the start, and whatever else the last backward left out (with
+    att_model = 'transformer': the top-down core, its embedding and heads, and the branch att_input_mode does not read)."""
 
     def __init__(self, ops, state_dict, opt, lr=5e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, grad_clip=0.1, all_reduce=None,
                  n_replicas=1):
@@ -495,6 +657,8 @@ class Trainer:
         self.t = 0
         self.keys = [k for k, v in state_dict.items() if torch.is_tensor(v) and v.is_floating_point() and "running_" not in k]
         self.never = ("core.i2h_2", "core.h2h_2")
+        self.idle = frozenset()                                    # keys the last backward gave no gradient
+        self._adopted = weakref.WeakSet()
         offs, o = {}, 0
         for k in self.keys:
             offs[k] = o
@@ -520,7 +684,7 @@ class Trainer:
     def set_lr(self, lr):
         """One param group per tensor; 'ctx2pool_grd' / 'vis_embed' fine-tune at lr x 0.1 (main.py:663-669); utils.set_lr decay = call again."""
         self.lr = lr
-        lrs = [0.0 if k.startswith(self.never) else (lr * 0.1 if ("ctx2pool_grd" in k or "vis_embed" in k) else lr) for k in self.keys]
+        lrs = [0.0 if (k in self.idle or k.startswith(self.never)) else (lr * 0.1 if ("ctx2pool_grd" in k or "vis_embed" in k) else lr) for k in self.keys]
         self.seg_lr = torch.tensor(lrs, dtype=torch.float32, device=self.ops.device)
 
     def grad_view(self, k):
@@ -528,12 +692,16 @@ class Trainer:
         return self.flat_g[self.offsets[k]:self.offsets[k] + n].view(self.weights[k].shape)
 
     def adopt_module(self, module):
-        """Re-point an nn.Module's parameters (and their .grad) at the flat buffers: `loss.backward(); optimizer.step()` drivers and
-        this Trainer then share storage."""
+        """Re-point an nn.Module's parameters (and their .grad) at the flat buffers, and its buffers (BatchNorm running statistics) at this
+        Trainer's: `loss.backward(); optimizer.step()` drivers and this Trainer then share storage, and the module decodes with the trained state."""
         for k, p in module.named_parameters():
             if k in self.weights:
                 p.data = self.weights[k]
                 p.grad = self.grad_view(k)
+        for k, b in module.named_buffers():
+            if k in self.buffers and self.buffers[k].shape == b.shape:
+                b.data = self.buffers[k]
+        self._adopted.add(module)
 
     def state_dict(self):
         sd = {k: v.detach().clone() for k, v in self.weights.items()}
@@ -548,6 +716,10 @@ class Trainer:
         self.flat_g.zero_()
         for k, g in grads.items():
             self.grad_view(k).copy_(g.reshape(self.weights[k].shape))
+        idle = frozenset(k for k in self.keys if k not in grads)
+        if idle != self.idle:
+            self.idle = idle
+            self.set_lr(self.lr)
         return losses, loss
 
     def step(self, inp, host=None):
@@ -565,6 +737,12 @@ class Trainer:
         ops.grad_norm_(self.flat_g, self.grad_clip, self.norm)
         ops.adam_flat_(self.flat_w, self.flat_g, self.flat_m, self.flat_v, self.seg_end, self.seg_lr, self.norm, self.betas[0], self.betas[1],
                        self.eps, self.weight_decay, self.t)
+        # the Adam kernel writes the weights behind torch's back: bump the version counters of adopted modules' parameters, so that
+        # code keyed on them (the module's cached native weights, AttModel._native_model) sees the new values
+        for m in self._adopted:
+            for k, p in m.named_parameters():
+                if k in self.weights:
+                    torch.autograd.graph.increment_version(p)
         if getattr(self.step_fn, "last_bn", None) is not None:
             mu, var, n = self.step_fn.last_bn
             rm, rv = self.buffers["att_embed_aux.0.running_mean"], self.buffers["att_embed_aux.0.running_var"]

@@ -51,6 +51,8 @@ _SIGS = {
     "gvd_tr_adam_flat": [_vp, _vp, _vp, _vp, _ll, _vp, _vp, _ci, _vp, _cf, _cf, _cf, _cf, _ci, _vp],
     "gvd_tr_gemm_nt_batched": [_vp, _ll, _ll, _vp, _ll, _ll, _vp, _ll, _ll, _ci, _ci, _ci, _ci, _vp],
     "gvd_tr_transpose": [_vp, _vp, _ci, _ci, _ci, _vp],
+    "gvd_tr_mha_fwd": [_vp, _vp, _vp, _vp, _vp, _ci, _ci, _ci, _ci, _ci, _cf, _cf, _ll, _ci, _ll, _vp],
+    "gvd_tr_mha_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ci, _ci, _ci, _ci, _ci, _cf, _cf, _ll, _ci, _ll, _vp],
 }
 _bound = False
 
@@ -326,6 +328,32 @@ class NativeOps:
         out = self._new(n_rows, rows.shape[1])
         capi.check(self.L.gvd_tr_index_add_rows(_p(idx), _p(rows), _p(out), n_rows, rows.shape[0], rows.shape[1], self._st()))
         return out
+
+    # ---- multi-head attention of the transformer captioner's decoder (csrc/gvd_tfm_train.cu)
+    def mha_fwd(self, q, k, v, causal, scale, p=0.0, seed=0, site_base=0, step=0):
+        """q [B, Lq, H], k / v [B, N, H] -> (o [B, Lq, H], lse [B, heads, Lq]); p > 0: per-head probability dropout at site site_base + head."""
+        q, k, v = _f(q), _f(k), _f(v)
+        B, Lq, H = q.shape
+        N = k.shape[1]
+        if k.shape != (B, N, H) or v.shape != (B, N, H):
+            raise capi.GvdError("mha_fwd: q %s, k %s, v %s" % (tuple(q.shape), tuple(k.shape), tuple(v.shape)))
+        c = -(-H // 6)                                                                      # torch.chunk(6, -1) column ranges
+        o, lse = torch.empty_like(q), self._new(B, -(-H // c), Lq)
+        capi.check(self.L.gvd_tr_mha_fwd(_p(q), _p(k), _p(v), _p(o), _p(lse), B, Lq, N, H, 1 if causal else 0, float(scale), float(p), int(seed),
+                                         int(site_base), int(step), self._st()))
+        return o, lse
+
+    def mha_bwd(self, do, q, k, v, o, lse, causal, scale, p=0.0, seed=0, site_base=0, step=0):
+        """-> (dq, dk, dv) for the upstream gradient do of mha_fwd's o (same dropout arguments: the masks are regenerated)."""
+        q, k, v, o, do, lse = _f(q), _f(k), _f(v), _f(o), _f(do), _f(lse)
+        B, Lq, H = q.shape
+        N = k.shape[1]
+        if do.shape != q.shape or o.shape != q.shape or k.shape != (B, N, H) or v.shape != (B, N, H):
+            raise capi.GvdError("mha_bwd: shapes differ from the forward's")
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        capi.check(self.L.gvd_tr_mha_bwd(_p(q), _p(k), _p(v), _p(o), _p(do), _p(lse), _p(dq), _p(dk), _p(dv), B, Lq, N, H, 1 if causal else 0,
+                                         float(scale), float(p), int(seed), int(site_base), int(step), self._st()))
+        return dq, dk, dv
 
     # ---- loss heads (value + gradient for d(loss) = 1); the 1/n of every masked mean stays on the device: no host round trip
     def _count_inv(self, t):

@@ -329,6 +329,16 @@ GVD_API int gvd_tr_count_inv(const void* data, long long n, int elem_bytes /* 1:
 GVD_API int gvd_tr_scalar_mul(const float* a, const float* b, float* out, void* stream);
 GVD_API int gvd_tr_outer_rows_acc(const float* a, const float* v, float* acc, int B, int N, int H, void* stream);   /* acc[b,n,:] += a[b,n] v[b,:] */
 GVD_API int gvd_tr_transpose(const float* in, float* out, int batch, int R, int C, void* stream);                      /* out[z,c,r] = in[z,r,c] */
+/* multi-head attention of the transformer captioner's decoder in train mode (misc/transformer.py:92-123; csrc/gvd_tfm_train.cu): q [B, Lq, H],
+   k / v [B, N, H] already projected, heads = the torch.chunk(6, -1) column ranges read in place, scores q.k * scale, causal: row t sees keys
+   r <= t.  o [B, Lq, H] (heads concatenated), lse [B, n_heads, Lq] = the softmax's log-sum-exp for the backward.  p > 0: each head's
+   probabilities are dropped with the mask gvd_tr_dropout draws on that head's contiguous [B, Lq, N] tensor at site site_base + head.
+   Lq <= 64, N <= 1000, head width <= 192; anything else is refused with status 1. */
+GVD_API int gvd_tr_mha_fwd(const float* q, const float* k, const float* v, float* o, float* lse, int B, int Lq, int N, int H, int causal, float scale,
+                           float p, long long seed, int site_base, long long step, void* stream);
+GVD_API int gvd_tr_mha_bwd(const float* q, const float* k, const float* v, const float* o, const float* d_o, const float* lse, float* dq, float* dk,
+                           float* dv, int B, int Lq, int N, int H, int causal, float scale, float p, long long seed, int site_base, long long step,
+                           void* stream);
 
 /* ---- transformer captioner (att_model = 'transformer'): Decoder.greedy of misc/transformer.py:214-241 behind
  * TransformerDecoder.forward(infer=True) (:271-274), called by misc/model.py:570-578 after the prologue.  The weights are the
