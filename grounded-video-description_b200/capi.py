@@ -21,7 +21,7 @@ EXPORTS = [
     "gvd_profile_enable", "gvd_profile_reset", "gvd_profile_count", "gvd_profile_entry",
     "gvd_op_linear_tc", "gvd_op_linear_f16ss", "gvd_op_skinny_partials", "gvd_op_reduce_lstm", "gvd_op_reduce_bias", "gvd_op_reduce_pick",
     "gvd_op_reduce_sample", "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_attention", "gvd_op_beam_topk",
-    "gvd_op_row_argmax", "gvd_op_beam_search_scripted", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
+    "gvd_op_row_argmax", "gvd_op_beam_search_scripted", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_self_attention_fused", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
     "gvd_tfm_workspace_bytes", "gvd_tfm_decode_greedy", "gvd_tfm_teacher_fwd",
     "gvd_grounding_extract", "gvd_grounding_eval", "gvd_plan_skinny_splits", "gvd_plan_h2d_chunks", "gvd_workspace_bytes_beam", "gvd_beam_decode", "gvd_workspace_bytes_teacher", "gvd_teacher_fwd",
     # training-step primitives (csrc/gvd_train.cu; bound in train_ops.py)
@@ -84,6 +84,7 @@ def lib():
     L.gvd_op_linear_f16ss.argtypes = [vp, i64, vp, i64, vp, vp, i64, vp, ci, ci, ci, ci, vp]
     L.gvd_op_scores_tc.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, i64, vp]
     L.gvd_op_self_attention_tc.argtypes = [vp, vp, ci, ci, ci, ci, ci, ctypes.c_float, vp, vp, ci, vp]
+    L.gvd_op_self_attention_fused.argtypes = [vp, vp, ci, ci, ci, ci, ci, ctypes.c_float, vp, ctypes.c_int64, vp]
     L.gvd_grounding_extract.argtypes = [vp, vp, ci, ci, ci, ci, vp, vp, vp]
     L.gvd_plan_skinny_splits.argtypes = [ci, ci, ci]
     L.gvd_plan_h2d_chunks.argtypes = [ci, ci, vp, ci]
@@ -722,6 +723,23 @@ def op_self_attention_tc(qkv, nh, hs, scale, debug=False, E=None, F=None, stages
     check(lib().gvd_op_self_attention_tc(_dev(qkv, torch.float32, "qkv"), ctypes.c_void_p(out.data_ptr()), nb, nh, R, hs, HP,
                                          float(scale), _dev(E, torch.float32, "E"), _dev(F, torch.float32, "F"), int(stages), _stream()))
     return (out, E, F) if debug else out
+
+
+def op_self_attention_fused(qkv, nh, hs, scale, img=None):
+    """concat_h softmax(Q_h K_h^T * scale) V_h for qkv [nb, R, 3*HP] through the fused self-attention kernel.  Returns out [nb, R, HP]
+    (fp32); with img (an int32 tensor [nb*R, img_ld]) the kernel stores the fp16x3 operand image of the output there instead and out is
+    left as allocated (zeros)."""
+    nb, R, three_hp = qkv.shape
+    HP = three_hp // 3
+    out = torch.zeros(nb, R, HP, dtype=torch.float32, device="cuda")
+    img_ptr, img_ld = None, 0
+    if img is not None:
+        if img.dtype != torch.int32 or not img.is_cuda or not img.is_contiguous() or img.dim() != 2 or img.shape[0] != nb * R:
+            raise ValueError("img must be a contiguous CUDA int32 tensor [nb*R, img_ld]")
+        img_ptr, img_ld = ctypes.c_void_p(img.data_ptr()), img.shape[1]
+    check(lib().gvd_op_self_attention_fused(_dev(qkv, torch.float32, "qkv"), ctypes.c_void_p(out.data_ptr()), nb, nh, R, hs, HP,
+                                            float(scale), img_ptr, int(img_ld), _stream()))
+    return out
 
 
 def grounding_extract(att2, ppls, num_frames, num_prop, want_boxes=True):

@@ -807,7 +807,7 @@ static int obj_interact_fwd(const gvd_model* m, const WS& w0, int c0, int B, cud
         long long ldwp = 0;
         const bool qkv_img = fuse && att16 && !no_qkv_img && R % 2 == 0 && HS % 4 == 0 && linear_w_f16ss(w, m->wqk[l], H, (int)BR, 3 * HP, H, &Wp, &ldwp);
         if (qkv_img) {
-            GvdQkvImages qi{HP, HS, KH, nh, R, Rp, w.k_img, w.vt_img, GVD_ATT_SK_HOST, GVD_ATT_SV_HOST};
+            GvdQkvImages qi{HP, HS, KH, nh, R, Rp, w.k_img, w.vt_img, GVD_ATT_SK, GVD_ATT_SV};
             ProfScope _pk("kernel.f16ss_gemm", st);
             GVD_STAGE("interact.qkv_proj", gvd_gemm_f16ss(w.img_h, (H + 31) / 32 * 32, Wp, ldwp, nullptr, nullptr, nullptr, GVD_ACT_NONE, w.qk, 3 * HP, (int)BR, 3 * HP, H,
                                                           st, nullptr, 0, &qi));
@@ -816,8 +816,8 @@ static int obj_interact_fwd(const gvd_model* m, const WS& w0, int c0, int B, cud
                                                 fuse ? w.img_h : nullptr));
         if (qkv_img) {
         } else if (att16) {
-            GVD_STAGE("interact.k_split", gvd_pack_heads_f16x3(w.qk + HP, 3 * HP, BR, nh, HS, HS, KH, GVD_ATT_SK_HOST, w.k_img, st));
-            GVD_STAGE("interact.v_transpose", gvd_transpose_pack_f16x3(w.qk + 2 * HP, w.vt_img, B, R, HP, 3 * HP, Rp, GVD_ATT_SV_HOST, st));
+            GVD_STAGE("interact.k_split", gvd_pack_heads_f16x3(w.qk + HP, 3 * HP, BR, nh, HS, HS, KH, GVD_ATT_SK, w.k_img, st));
+            GVD_STAGE("interact.v_transpose", gvd_transpose_pack_f16x3(w.qk + 2 * HP, w.vt_img, B, R, HP, 3 * HP, Rp, GVD_ATT_SV, st));
         } else if (fused) {
             // tf32 hi / lo planes of K and V^T, made once per layer: the two attention kernels then stream them without converting
             GVD_STAGE("interact.k_split", gvd_split_hilo(w.qk + HP, 3 * HP, w.khi, w.klo, HP, BR, HP, st));
@@ -826,11 +826,15 @@ static int obj_interact_fwd(const gvd_model* m, const WS& w0, int c0, int B, cud
             // V^T per clip (the P.V product is then again an NT GEMM with K = R contiguous)
             GVD_STAGE("interact.v_transpose", gvd_transpose(w.qk + 2 * HP, w.vT, B, R, HP, 3 * HP, st));
         }
-        // The P.V epilogue stores the operand image of the output projection's input (no fp32 att_o, no pack pass).
-        // GVD_NO_ATT_O_IMG restores the pack pass.
-        static const bool no_o_img = getenv("GVD_NO_ATT_O_IMG") != nullptr;
+        // With pack fusion the attention stores the operand image of the output projection's input (no fp32 att_o, no pack pass).
         const long long HPi = (HP + 31) / 32 * 32;
-        const bool o_img = fuse && att16 && !no_o_img && HS % 4 == 0 && linear_w_f16ss(w, m->wo[l], HP, (int)BR, H, HP);
+        const bool o_img = fuse && att16 && HS % 4 == 0 && linear_w_f16ss(w, m->wo[l], HP, (int)BR, H, HP);
+        if (att16) {
+            // softmax(Q K^T / sqrt(d_model)) V of every clip and head in one launch, the scores never leave the SM
+            // (the scale is sqrt(1024)=32, not sqrt(d_head): transformer.py:94,111; quirk Q1)
+            GVD_STAGE("interact.attn", gvd_self_attn_fused(w.qk, 3 * HP, w.k_img, w.vt_img, B, R, nh, HS, HP, 1.f / sqrtf((float)H), w.att_o, HP,
+                                                           o_img ? w.a_pk : nullptr, HPi, st));
+        } else
         for (int b0 = 0; b0 < B; b0 += w.clip_chunk) {
             const int cb = std::min(w.clip_chunk, B - b0);
             {   // S[b,h] = Q_h K_h^T  (heads are zero-padded to HS columns)
@@ -843,10 +847,6 @@ static int obj_interact_fwd(const gvd_model* m, const WS& w0, int c0, int B, cud
                     // scores + softmax numerator in one sweep: E = exp((s - mu_group)/sqrt(d_model)), group factors -> smxF
                     // (the scale is sqrt(1024)=32, not sqrt(d_head): transformer.py:94,111; quirk Q1)
                     g.W = w.khi + (long long)b0 * R * HP; g.ldw = HP; g.sWb = (long long)R * HP;
-                    if (att16) {
-                        g.W = w.k_img + (long long)b0 * R * nh * KH; g.ldw = (long long)nh * KH; g.sWb = (long long)R * nh * KH; g.sWh = KH;
-                        GVD_STAGE("interact.scores", gvd_attn_scores_tc(g, nullptr, w.smxF, 1.f / sqrtf((float)H), cb * nh, st, 1));
-                    } else
                     GVD_STAGE("interact.scores", gvd_attn_scores_tc(g, w.klo + (long long)b0 * R * HP, w.smxF, 1.f / sqrtf((float)H), cb * nh, st));
                 } else {
                     GVD_STAGE("interact.scores", gvd_gemm_nt(g, cb * nh, st));
@@ -860,11 +860,7 @@ static int obj_interact_fwd(const gvd_model* m, const WS& w0, int c0, int B, cud
                 g.W = w.vT + (long long)b0 * HP * R; g.ldw = R; g.sWb = (long long)HP * R; g.sWh = (long long)HS * R;
                 g.C = w.att_o + (long long)b0 * R * HP; g.ldc = HP; g.sCb = (long long)R * HP; g.sCh = HS;
                 g.M = R; g.N = HS; g.K = R; g.nh = nh; g.alpha = 1.f;
-                if (att16) {
-                    g.W = w.vt_img + (long long)b0 * HP * Rp; g.ldw = Rp; g.sWb = (long long)HP * Rp; g.sWh = (long long)HS * Rp;
-                    // pack fusion: the epilogue stores the operand image of the output projection's input (a_pk, free here) instead of fp32 att_o
-                    GVD_STAGE("interact.pv", gvd_attn_pv_tc(g, nullptr, w.smxF, cb * nh, st, 1, o_img ? w.a_pk + (long long)b0 * R * HPi : nullptr, HPi));
-                } else if (fused) GVD_STAGE("interact.pv", gvd_attn_pv_tc(g, w.vTl + (long long)b0 * HP * R, w.smxF, cb * nh, st));
+                if (fused) GVD_STAGE("interact.pv", gvd_attn_pv_tc(g, w.vTl + (long long)b0 * HP * R, w.smxF, cb * nh, st));
                 else GVD_STAGE("interact.pv", gvd_gemm_nt(g, cb * nh, st));
             }
         }
@@ -1932,7 +1928,7 @@ extern "C" GVD_API int gvd_op_self_attention_tc(const float* qkv, float* out, in
     auto body16 = [&]() -> int {
         GVD_CHECK_CUDA(cudaMalloc(&khi, BR * nh * KH * 4)); GVD_CHECK_CUDA(cudaMalloc(&vh, (size_t)nb * HP * Rp * 4));
         if (stages & 1) {
-            GVD_TRY(gvd_pack_heads_f16x3(qkv + HP, 3 * HP, (long long)BR, nh, hs, hs, KH, GVD_ATT_SK_HOST, khi, st));
+            GVD_TRY(gvd_pack_heads_f16x3(qkv + HP, 3 * HP, (long long)BR, nh, hs, hs, KH, GVD_ATT_SK, khi, st));
             GemmArgs g{};
             g.A = qkv; g.lda = 3 * HP; g.sAb = (long long)R * 3 * HP; g.sAh = hs;
             g.W = khi; g.ldw = (long long)nh * KH; g.sWb = (long long)R * nh * KH; g.sWh = KH;
@@ -1941,7 +1937,7 @@ extern "C" GVD_API int gvd_op_self_attention_tc(const float* qkv, float* out, in
             GVD_TRY(gvd_attn_scores_tc(g, nullptr, F, scale, nb * nh, st, 1));
         }
         if (stages & 2) {
-            GVD_TRY(gvd_transpose_pack_f16x3(qkv + 2 * HP, vh, nb, R, HP, 3 * HP, Rp, GVD_ATT_SV_HOST, st));
+            GVD_TRY(gvd_transpose_pack_f16x3(qkv + 2 * HP, vh, nb, R, HP, 3 * HP, Rp, GVD_ATT_SV, st));
             GemmArgs v{};
             v.A = E; v.lda = R; v.sAb = (long long)nh * R * R; v.sAh = (long long)R * R;
             v.W = vh; v.ldw = Rp; v.sWb = (long long)HP * Rp; v.sWh = (long long)hs * Rp;
@@ -1978,6 +1974,27 @@ extern "C" GVD_API int gvd_op_self_attention_tc(const float* qkv, float* out, in
     };
     const int rc = att16 ? body16() : body();
     cudaFree(khi); cudaFree(klo); cudaFree(vh); cudaFree(vl);
+    return rc;
+}
+// Self-attention core through the fused kernel (gvd_attn.cu): key / V^T images built here, O as fp32 (out) or as its operand image (img).
+extern "C" GVD_API int gvd_op_self_attention_fused(const float* qkv, float* out, int nb, int nh, int R, int hs, int HP, float scale, float* img,
+                                                   int64_t img_ld, void* stream) {
+    GVD_REQUIRE(qkv && (out || img) && nb > 0 && nh > 0 && R > 0 && HP % 4 == 0 && nh * hs <= HP, "op_self_attention_fused: bad arguments");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t BR = (size_t)nb * R;
+    const int KH = (hs + 31) / 32 * 32, Rp = (R + 31) / 32 * 32;
+    float *kimg = nullptr, *vimg = nullptr;
+    auto body = [&]() -> int {
+        GVD_CHECK_CUDA(cudaMalloc(&kimg, BR * nh * KH * 4));
+        GVD_CHECK_CUDA(cudaMalloc(&vimg, (size_t)nb * HP * Rp * 4));
+        GVD_TRY(gvd_pack_heads_f16x3(qkv + HP, 3 * HP, (long long)BR, nh, hs, hs, KH, GVD_ATT_SK, kimg, st));
+        GVD_TRY(gvd_transpose_pack_f16x3(qkv + 2 * HP, vimg, nb, R, HP, 3 * HP, Rp, GVD_ATT_SV, st));
+        GVD_TRY(gvd_self_attn_fused(qkv, 3 * HP, kimg, vimg, nb, R, nh, hs, HP, scale, out, HP, img, img_ld, st));
+        GVD_CHECK_CUDA(cudaStreamSynchronize(st));
+        return 0;
+    };
+    const int rc = body();
+    cudaFree(kimg); cudaFree(vimg);
     return rc;
 }
 extern "C" GVD_API int gvd_op_tanh(const float* x, float* y, int n, void* stream) { return gvd_tanh_test(x, y, n, (cudaStream_t)stream); }

@@ -107,9 +107,13 @@ int gvd_gemm_nt_tc(const GemmArgs& g, int batch, cudaStream_t stream);
 int gvd_gemm_nt_astat(const GemmArgs& g, int batch, cudaStream_t stream);   // short-K (<= 192), one K pass
 // self-attention pair (W operands pre-split into tf32 hi / lo planes): softmax-numerator scores + group factors F, then (F (.) E) V
 int gvd_attn_scores_tc(const GemmArgs& g, const float* W_lo, float* F, float smx_scale, int batch, cudaStream_t stream, int f16 = 0);
-int gvd_attn_pv_tc(const GemmArgs& g, const float* W_lo, const float* F, int batch, cudaStream_t stream, int f16 = 0, float* img = nullptr,
-                   long long img_ld = 0);       // img: store O as the fp16x3 operand image (rows = clip-major regions, pitch img_ld words) instead of fp32 C
+int gvd_attn_pv_tc(const GemmArgs& g, const float* W_lo, const float* F, int batch, cudaStream_t stream, int f16 = 0);
 int gvd_lstm_step_tc(const LstmArgs& a, cudaStream_t stream);
+// fused self-attention (gvd_attn.cu): O[b, r, h] = softmax(Q_h K_h^T * scale) V_h for every clip and head in one launch.  Q fp32 (row b * R + r,
+// head h at column h * hs), the key image of gvd_pack_heads_f16x3 (KH = hs rounded up to 32), the V^T image of gvd_transpose_pack_f16x3 (HP
+// columns per clip, Rp = R rounded up to 32); O as fp32 (out, pitch ldo) or, when img is given, as the fp16x3 operand image of the next GEMM
+int gvd_self_attn_fused(const float* q, long long ldq, const float* k_img, const float* vt_img, int B, int R, int nh, int hs, int HP, float scale,
+                        float* out, long long ldo, float* img, long long img_ld, cudaStream_t st);
 int gvd_logit_pick_tc(const float* h, long long ldh, const float* W, long long ldw, const float* bias, int B, int V, int K, int unk_idx,
                       float* part, int* ticket, long long* it_out, long long* seq_out, float* logp_out, long long out_stride,
                       const float* embed, float* xt, int E, cudaStream_t stream);
@@ -142,9 +146,12 @@ int gvd_gru_layer(const float* gi, const float* whh, const float* bhh, float* hb
 int gvd_gru_layer_f16(const float* gi, const float* Whh_img, const float* bhh, float* hstate, float* h_img, float* out, const long long* sample_idx, int B,
                       int T, int G, cudaStream_t st);
 
-// fp16x3 operand images for the fused self-attention: per-head key image, transposed value image (scales must match gvd_wgmma.cu)
-#define GVD_ATT_SK_HOST 16.f
-#define GVD_ATT_SV_HOST 16.f
+// power-of-two scales of the fp16x3 operands of the self-attention (queries, keys, probabilities, values)
+#define GVD_ATT_SQ 4.f
+#define GVD_ATT_SK 16.f
+#define GVD_ATT_SP 1024.f
+#define GVD_ATT_SV 16.f
+// fp16x3 operand images for the self-attention: per-head key image (scale GVD_ATT_SK), transposed value image (GVD_ATT_SV)
 int gvd_pack_heads_f16x3(const float* in, long long ld_in, long long rows, int nh, int hs_in, int hs, int KH, float scale, float* out, cudaStream_t st);
 int gvd_transpose_pack_f16x3(const float* in, float* out, int B, int R, int C, int ld_in, int Rp, float scale, cudaStream_t st);
 

@@ -26,7 +26,7 @@
 //   epilogue  : the accumulator fragments are exchanged through shared memory so that every thread owns one
 //               output row (thread <-> row, lane <-> row within the warp); the epilogues are written for
 //               that layout: bias / activation store, transposed split-K partial, fused LSTM cell, fused
-//               greedy pick, operand-image stores (Q|K|V projection, P.V), fused GRU cell.
+//               greedy pick, operand-image stores (Q|K|V projection), fused GRU cell.
 // Up to three K segments (different A / W tensors) feed one accumulator, so the LSTM gate GEMMs never
 // materialise a concatenated input (AttModel.py:138,147-160).
 #include <cuda.h>
@@ -34,20 +34,19 @@
 #include <algorithm>
 #include <cstdlib>
 
-#include "gvd_kernels.cuh"
+#include "gvd_wgmma.cuh"
 
 namespace {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BN = 64;
 constexpr int TC_BN_SS = 128;             // tile width of MODE_SS
-constexpr int TC_BK = 32;                 // fp32 elements per K slice = 128 bytes = one swizzle row
 constexpr int WG_CONSUMERS = 256;         // two warpgroups
 constexpr int WG_THREADS = WG_CONSUMERS + 32;
 constexpr int WG_STAGES = 4;              // also at 128-wide tiles (32 KB stages): 6 stages measured no faster on the H100
 constexpr int WG_UJ = 16;                 // hidden units per CTA of the gate-interleaved tiles (LSTM: 4 x 16, GRU: 3 x 16 columns)
 
-enum { MODE_STORE = 0, MODE_LSTM = 1, MODE_PICK = 2, MODE_TRANS = 3, MODE_SS = 4, MODE_GRU = 5, MODE_PV_IMG = 6 };
+enum { MODE_STORE = 0, MODE_LSTM = 1, MODE_PICK = 2, MODE_TRANS = 3, MODE_SS = 4, MODE_GRU = 5 };
 
 struct TcSeg {
     int k_len;          // K extent of this segment
@@ -108,31 +107,10 @@ struct TcParams {
     long long pk_stride;
     int pk_unk;
     const float* pk_embed; float* pk_xt; int pk_E;          // xt[M, E] = ReLU(embed[token]) for the next step
-    // P.V image mode: store the output as the fp16x3 operand image of the next GEMM (Wo) instead of fp32 C: row (zb * M + m) of img (pitch
-    // img_ld words, zb = clip of the sub-batch), head zh at columns [zh * sCh, zh * sCh + slot) with the pad columns n >= N written as zeros
-    uint32_t* img; long long img_ld; float img_scale; int img_slot;
     SsParams ss;
     GruStepParams gru;
 };
 
-__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-        : "memory");
-}
-__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
-}
-__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
-    // K-major, SWIZZLE_128B canonical layout: rows of 128 B, 8-row groups 1024 B apart (SBO), LBO unused
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);            // start address        bits [0,14)
-    d |= (uint64_t)1 << 16;                                // leading byte offset  bits [16,30) (ignored for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;                      // stride byte offset   bits [32,46)
-    d |= (uint64_t)1 << 62;                                // layout type SWIZZLE_128B
-    return d;
-}
 __device__ __forceinline__ float4 lds128(uint32_t addr) {
     float4 v;
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr));
@@ -150,58 +128,6 @@ __device__ __forceinline__ void split_h4(const float4& v, float s, uint32_t& h01
     f16x3_split_pair(v.z, v.w, s, h23, l23);
 }
 
-// ---- wgmma: D[64 x 64] (+)= A[64 x K] . B[64 x K]^T, both operands K-major in shared memory (SWIZZLE_128B descriptors).
-// Accumulator fragment of thread t of the warpgroup: d[4 j + {0,1}] = row 16 (t / 32) + (t % 32) / 4, columns 8 j + 2 (t % 4) + {0,1};
-// d[4 j + {2,3}] = the same columns of row + 8.
-#define WG_D32(d) "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), \
-    "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]),       \
-    "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-#define WG_D32_LIST "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}"
-__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " WG_D32_LIST ", %32, %33, p, 1, 1;\n\t"
-        "}\n"
-        : WG_D32(d)
-        : "l"(da), "l"(db), "r"(accumulate));
-}
-__device__ __forceinline__ void wgmma_f16(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %34, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " WG_D32_LIST ", %32, %33, p, 1, 1, 0, 0;\n\t"
-        "}\n"
-        : WG_D32(d)
-        : "l"(da), "l"(db), "r"(accumulate));
-}
-// D[64 x 128]: the same fragment layout with j = 0..15
-#define WG_D64(d) WG_D32(d), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), \
-    "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]),     \
-    "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),     \
-    "+f"(d[63])
-#define WG_D64_LIST "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31," \
-    "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}"
-__device__ __forceinline__ void wgmma_f16(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t"
-        ".reg .pred p;\n\t"
-        "setp.ne.b32 p, %66, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " WG_D64_LIST ", %64, %65, p, 1, 1, 0, 0;\n\t"
-        "}\n"
-        : WG_D64(d)
-        : "l"(da), "l"(db), "r"(accumulate));
-}
-__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait0(float (&d)[32]) {
-    asm volatile("wgmma.wait_group.sync.aligned 0;" : WG_D32(d) : : "memory");
-}
-__device__ __forceinline__ void wgmma_wait0(float (&d)[64]) {
-    asm volatile("wgmma.wait_group.sync.aligned 0;" : WG_D64(d) : : "memory");
-}
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(WG_CONSUMERS) : "memory"); }
 
 template <bool F16, int BN> struct WgCfg {
@@ -560,37 +486,6 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                 if (n < p.N) C[(long long)n * p.ldc + m] = Cs[row * LDS_ + cbeg + j] * p.alpha;
             }
         }
-    } else if (p.mode == MODE_PV_IMG) {
-        // 4 columns = 2 hi words + 2 lo words: a 4-column group never straddles a 32-wide K slice of the Wo operand (the head stride sCh and
-        // the column offsets are multiples of 4), 8-byte stores
-        if (m < p.M) {
-            uint32_t* irow = p.img + ((long long)zb * p.M + m) * p.img_ld;
-            if (zh == p.nh - 1 && blockIdx.x == 0 && cbeg == 0) {
-                // the K padding of the Wo operand (columns [nh * sCh, img_ld) of the row) belongs to nobody's head: zeros, like the pack pass wrote
-                for (int gc = p.nh * (int)p.sCh; gc < (int)p.img_ld; gc += 4) {
-                    uint32_t* dz = irow + f16x3_word(gc);
-                    *reinterpret_cast<uint2*>(dz) = make_uint2(0u, 0u);
-                    *reinterpret_cast<uint2*>(dz + 16) = make_uint2(0u, 0u);
-                }
-            }
-#pragma unroll
-            for (int j = 0; j < 32; j += 4) {
-                const int n = n0 + cbeg + j;
-                if (n >= p.img_slot) continue;                              // columns past the head's slot belong to the next head's CTA
-                const float4 t = *reinterpret_cast<const float4*>(Cs + row * LDS_ + cbeg + j);
-                const float tv[4] = {t.x, t.y, t.z, t.w};
-                uint32_t hi[2], lo[2];
-#pragma unroll
-                for (int pr = 0; pr < 2; ++pr) {
-                    const float v0 = (n + 2 * pr < p.N) ? tv[2 * pr] * p.alpha : 0.f;
-                    const float v1 = (n + 2 * pr + 1 < p.N) ? tv[2 * pr + 1] * p.alpha : 0.f;
-                    f16x3_split_pair(v0, v1, p.img_scale, hi[pr], lo[pr]);
-                }
-                uint32_t* dw = irow + f16x3_word(zh * (int)p.sCh + n);
-                *reinterpret_cast<uint2*>(dw) = make_uint2(hi[0], hi[1]);
-                *reinterpret_cast<uint2*>(dw + 16) = make_uint2(lo[0], lo[1]);
-            }
-        }
     } else if (warp < 4) {
         // ---- modes in which one thread finishes a whole row of the tile alone: all 64 columns of row m
         float a64[TC_BN];
@@ -748,42 +643,6 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
     }
 }
 
-// ------------------------------------------------------------------------------------ host side
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn get_encode() {
-    static EncodeTiledFn fn = nullptr;
-    static bool tried = false;
-    if (!tried) {
-        tried = true;
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeTiledFn>(p);
-    }
-    return fn;
-}
-
-// rank-4 fp32 tensor map {K, rows, heads, batch}; box {32, box_rows, 1, 1}; 128B swizzle; OOB -> 0.
-// An axis with stride 0 (operand shared across it) is encoded with extent 1; *mul tells the kernel to pass coordinate 0.
-int make_map(CUtensorMap* map, const float* base, long long K, long long rows, long long ld, long long nh, long long s_h, long long nb,
-             long long s_b, int box_rows, int* mul_h, int* mul_b) {
-    EncodeTiledFn enc = get_encode();
-    GVD_REQUIRE(enc, "tcgemm: cuTensorMapEncodeTiled is unavailable in this driver");
-    GVD_REQUIRE(((uintptr_t)base & 15) == 0 && ld % 4 == 0 && s_h % 4 == 0 && s_b % 4 == 0, "tcgemm: operand not 16-byte aligned");
-    const bool use_h = nh > 1 && s_h != 0, use_b = nb > 1 && s_b != 0;
-    *mul_h = use_h ? 1 : 0;
-    *mul_b = use_b ? 1 : 0;
-    cuuint64_t dims[4] = {(cuuint64_t)K, (cuuint64_t)rows, (cuuint64_t)(use_h ? nh : 1), (cuuint64_t)(use_b ? nb : 1)};
-    cuuint64_t strides[3] = {(cuuint64_t)ld * 4, (cuuint64_t)(use_h ? s_h : ld * rows) * 4, (cuuint64_t)(use_b ? s_b : ld * rows) * 4};
-    cuuint32_t box[4] = {TC_BK, (cuuint32_t)box_rows, 1, 1};
-    cuuint32_t estr[4] = {1, 1, 1, 1};
-    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    GVD_REQUIRE(r == CUDA_SUCCESS, "tcgemm: cuTensorMapEncodeTiled failed (%d) K=%lld rows=%lld ld=%lld", (int)r, K, rows, ld);
-    return 0;
-}
 
 // fp32 [N, K] (row pitch ldw) -> the W-operand image of the fp16x3 kernel: per row and 32-wide K slice 16 words of hi pairs then 16 words
 // of lo pairs (k = 2p, 2p + 1 in word p), values scaled by GVD_F16_SW; K padded with zeros to a multiple of 32 (row pitch Kp words)
@@ -859,12 +718,6 @@ __global__ void attn_softmax_rows_kernel(float* __restrict__ C, long long ldc, l
 
 }  // namespace
 
-// scales of the fp16x3 operands of the self-attention pair (queries, keys, probabilities, values); the key / value images are packed with
-// GVD_ATT_SK_HOST / GVD_ATT_SV_HOST
-#define GVD_ATT_SQ 4.f
-#define GVD_ATT_SK 16.f
-#define GVD_ATT_SP 1024.f
-#define GVD_ATT_SV 16.f
 
 // Batched product without bias / activation for the self-attention scores.
 //   W_lo == nullptr : g.W is plain fp32 (split inside the kernel);  else g.W / W_lo are its tf32 hi / lo planes (same strides): two K segments
@@ -905,7 +758,7 @@ int gvd_attn_scores_tc(const GemmArgs& g, const float* W_lo, float* F, float smx
     return launch_scores(g, W_lo, F, smx_scale, batch, stream, f16);
 }
 // O[z] = (F (.) A[z]) W[z]^T with W given as tf32 hi / lo planes or (f16) as its fp16x3 image, N <= 192, any K;  F [batch][ceil(K/32)][M] or null
-int gvd_attn_pv_tc(const GemmArgs& g, const float* W_lo, const float* F, int batch, cudaStream_t stream, int f16, float* img, long long img_ld) {
+int gvd_attn_pv_tc(const GemmArgs& g, const float* W_lo, const float* F, int batch, cudaStream_t stream, int f16) {
     GVD_REQUIRE(g.M > 0 && g.N > 0 && g.N <= 192 && g.K > 0 && g.nh >= 1 && batch % g.nh == 0 && (W_lo || f16), "attn pv: needs N <= 192 and pre-split W");
     GVD_REQUIRE(!g.bias && g.act == GVD_ACT_NONE, "attn pv: no bias / activation epilogue");
     GVD_REQUIRE(g.K % 4 == 0 && g.lda % 4 == 0 && g.ldw % 4 == 0, "attn pv: K/lda/ldw must be multiples of 4");
@@ -927,13 +780,6 @@ int gvd_attn_pv_tc(const GemmArgs& g, const float* W_lo, const float* F, int bat
     p.mode = MODE_STORE;
     p.sa = p.sw = p.oscale = 1.f;
     if (f16) { p.f16 = 1; p.wpre = 1; p.sa = GVD_ATT_SP; p.oscale = 1.f / (GVD_ATT_SP * GVD_ATT_SV); }
-    if (img) {
-        // every head owns sCh columns of the row (its N real ones + zero pads): together the heads must tile the image row exactly
-        GVD_REQUIRE(g.sCh % 4 == 0 && g.N <= g.sCh && g.sCh <= bn && img_ld % 32 == 0 && img_ld >= (long long)g.nh * g.sCh &&
-                    (reinterpret_cast<uintptr_t>(img) & 15) == 0, "attn pv: output image needs 4-column granularity of the head layout");
-        p.mode = MODE_PV_IMG;
-        p.img = reinterpret_cast<uint32_t*>(img); p.img_ld = img_ld; p.img_scale = GVD_F16_SA; p.img_slot = std::min(bn, (int)g.sCh);
-    }
     return launch_wg(mA, mW, p, dim3(gvd_cdiv(bn, TC_BN), gvd_cdiv(g.M, TC_BM), batch), stream);
 }
 

@@ -1,0 +1,164 @@
+// gvd: Hopper tensor-core plumbing shared by the wgmma kernels (gvd_wgmma.cu, gvd_attn.cu): TMA tensor maps and loads,
+// shared-memory matrix descriptors, wgmma wrappers.
+#pragma once
+#include <cuda.h>
+
+#include "gvd_kernels.cuh"
+
+namespace {
+
+constexpr int TC_BK = 32;                 // fp32 elements per K slice = 128 bytes = one swizzle row
+
+__device__ __forceinline__ void tma_load_4d(void* smem_dst, const CUtensorMap* map, uint64_t* bar, int c0, int c1, int c2, int c3) {
+    asm volatile(
+        "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+        ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
+        : "memory");
+}
+__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* map) {
+    asm volatile("prefetch.tensormap [%0];" ::"l"(map) : "memory");
+}
+__device__ __forceinline__ uint64_t make_smem_desc_sw128(uint32_t smem_addr) {
+    // K-major, SWIZZLE_128B canonical layout: rows of 128 B, 8-row groups 1024 B apart (SBO), LBO unused
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr >> 4) & 0x3FFF);            // start address        bits [0,14)
+    d |= (uint64_t)1 << 16;                                // leading byte offset  bits [16,30) (ignored for swizzled K-major)
+    d |= (uint64_t)(1024 >> 4) << 32;                      // stride byte offset   bits [32,46)
+    d |= (uint64_t)1 << 62;                                // layout type SWIZZLE_128B
+    return d;
+}
+// ---- wgmma: D[64 x 64] (+)= A[64 x K] . B[64 x K]^T, both operands K-major in shared memory (SWIZZLE_128B descriptors).
+// Accumulator fragment of thread t of the warpgroup: d[4 j + {0,1}] = row 16 (t / 32) + (t % 32) / 4, columns 8 j + 2 (t % 4) + {0,1};
+// d[4 j + {2,3}] = the same columns of row + 8.
+#define WG_D32(d) "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), \
+    "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]),       \
+    "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+#define WG_D32_LIST "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}"
+__device__ __forceinline__ void wgmma_tf32(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 " WG_D32_LIST ", %32, %33, p, 1, 1;\n\t"
+        "}\n"
+        : WG_D32(d)
+        : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_f16(float (&d)[32], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 " WG_D32_LIST ", %32, %33, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : WG_D32(d)
+        : "l"(da), "l"(db), "r"(accumulate));
+}
+// D[64 x 128]: the same fragment layout with j = 0..15
+#define WG_D64(d) WG_D32(d), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), \
+    "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]),     \
+    "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]),     \
+    "+f"(d[63])
+#define WG_D64_LIST "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31," \
+    "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}"
+__device__ __forceinline__ void wgmma_f16(float (&d)[64], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 " WG_D64_LIST ", %64, %65, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : WG_D64(d)
+        : "l"(da), "l"(db), "r"(accumulate));
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait0(float (&d)[32]) {
+    asm volatile("wgmma.wait_group.sync.aligned 0;" : WG_D32(d) : : "memory");
+}
+__device__ __forceinline__ void wgmma_wait0(float (&d)[64]) {
+    asm volatile("wgmma.wait_group.sync.aligned 0;" : WG_D64(d) : : "memory");
+}
+// D[64 x 32], both operands in shared memory (the score product of the fused self-attention): fragment layout as above with j = 0..3
+__device__ __forceinline__ void wgmma_f16(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %18, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n32k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+        : "l"(da), "l"(db), "r"(accumulate));
+}
+template <int N> __device__ __forceinline__ void wgmma_wait(float (&d)[16]) {
+    asm volatile("wgmma.wait_group.sync.aligned %16;" : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]) : "n"(N) : "memory");
+}
+// D[64 x N] with the A operand in registers (the P.V product of the fused self-attention): a[0..3] = the m16n8k16 A fragment of the thread's
+// warp (rows 16 (t / 32) + (t % 32) / 4 (+ 8), k = 2 (t % 4) (+ 8) pairs, low half = even k), i.e. the accumulator fragment of a 16-wide
+// column group of a previous product; B K-major in shared memory
+__device__ __forceinline__ void wgmma_f16_rs(float (&d)[44], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %49, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n88k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43}, {%44,%45,%46,%47}, %48, p, 1, 1, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+template <int N> __device__ __forceinline__ void wgmma_wait(float (&d)[44]) {
+    asm volatile("wgmma.wait_group.sync.aligned %44;" : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]) : "n"(N) : "memory");
+}
+__device__ __forceinline__ void wgmma_f16_rs(float (&d)[48], const uint32_t (&a)[4], uint64_t db, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t"
+        ".reg .pred p;\n\t"
+        "setp.ne.b32 p, %53, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n96k16.f32.f16.f16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47}, {%48,%49,%50,%51}, %52, p, 1, 1, 0;\n\t"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(accumulate));
+}
+template <int N> __device__ __forceinline__ void wgmma_wait(float (&d)[48]) {
+    asm volatile("wgmma.wait_group.sync.aligned %48;" : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]) : "n"(N) : "memory");
+}
+
+// ------------------------------------------------------------------------------------ host side
+// ------------------------------------------------------------------------------------ host side
+typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+EncodeTiledFn get_encode() {
+    static EncodeTiledFn fn = nullptr;
+    static bool tried = false;
+    if (!tried) {
+        tried = true;
+        void* p = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess && q == cudaDriverEntryPointSuccess)
+            fn = reinterpret_cast<EncodeTiledFn>(p);
+    }
+    return fn;
+}
+
+// rank-4 fp32 tensor map {K, rows, heads, batch}; box {32, box_rows, 1, 1}; 128B swizzle; OOB -> 0.
+// An axis with stride 0 (operand shared across it) is encoded with extent 1; *mul tells the kernel to pass coordinate 0.
+int make_map(CUtensorMap* map, const float* base, long long K, long long rows, long long ld, long long nh, long long s_h, long long nb,
+             long long s_b, int box_rows, int* mul_h, int* mul_b) {
+    EncodeTiledFn enc = get_encode();
+    GVD_REQUIRE(enc, "tcgemm: cuTensorMapEncodeTiled is unavailable in this driver");
+    GVD_REQUIRE(((uintptr_t)base & 15) == 0 && ld % 4 == 0 && s_h % 4 == 0 && s_b % 4 == 0, "tcgemm: operand not 16-byte aligned");
+    const bool use_h = nh > 1 && s_h != 0, use_b = nb > 1 && s_b != 0;
+    *mul_h = use_h ? 1 : 0;
+    *mul_b = use_b ? 1 : 0;
+    cuuint64_t dims[4] = {(cuuint64_t)K, (cuuint64_t)rows, (cuuint64_t)(use_h ? nh : 1), (cuuint64_t)(use_b ? nb : 1)};
+    cuuint64_t strides[3] = {(cuuint64_t)ld * 4, (cuuint64_t)(use_h ? s_h : ld * rows) * 4, (cuuint64_t)(use_b ? s_b : ld * rows) * 4};
+    cuuint32_t box[4] = {TC_BK, (cuuint32_t)box_rows, 1, 1};
+    cuuint32_t estr[4] = {1, 1, 1, 1};
+    CUresult r = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    GVD_REQUIRE(r == CUDA_SUCCESS, "tcgemm: cuTensorMapEncodeTiled failed (%d) K=%lld rows=%lld ld=%lld", (int)r, K, rows, ld);
+    return 0;
+}
+
+}  // namespace

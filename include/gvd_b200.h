@@ -186,6 +186,11 @@ GVD_API int gvd_op_scores_tc(const float* A, const float* W, float* C, int nb, i
    32-key group) factors factor [nb,nh,ceil(R/32),R] (softmax = numer * factor); bit 1: the row-scaled P.V -> out */
 GVD_API int gvd_op_self_attention_tc(const float* qkv, float* out, int nb, int nh, int R, int hs, int HP, float scale,
                   float* numer, float* factor, int stages, void* stream);
+/* the same self-attention core through the fused kernel (scores, softmax and P.V in one launch, the scores never leave the SM): the key
+   and V^T operand images are built inside the call.  img == NULL: out[nb, R, HP] fp32 (columns [h*hs, (h+1)*hs) of every head);
+   else the fp16x3 operand image of the output, [nb*R, img_ld] 32-bit words (scale 4, columns [nh*hs, img_ld) zeros), and out is unused */
+GVD_API int gvd_op_self_attention_fused(const float* qkv, float* out, int nb, int nh, int R, int hs, int HP, float scale, float* img,
+                  int64_t img_ld, void* stream);
 /* the conversion-free prologue GEMM on its own (operands packed into fp16x3 images inside the call); img_out: optional fp16x3 image of
    the output, [M, rup32(N)] 32-bit words (what the next GEMM would stream), C may then be NULL */
 GVD_API int gvd_op_linear_f16ss(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias, float* C, int64_t ldc,
