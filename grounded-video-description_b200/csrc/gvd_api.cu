@@ -745,7 +745,7 @@ static int check_ws(const gvd_model* m, int B, int T, void* workspace, size_t by
 
 // ------------------------------------------------------------------------------------ prologue
 // C = act(A W^T + bias) for a constant, registered weight W.  Backend bit 7: pack the activation operand into the fp16x3 image (one
-// element-wise pass: 4 B read + 4 B written per element) and run the conversion-free kernel (MODE_SS of wg_gemm_kernel: TMA -> wgmma on two operand images);
+// element-wise pass: 4 B read + 4 B written per element) and run the conversion-free kernel (ss_gemm_kernel: TMA -> wgmma on two operand images);
 // otherwise the conversion kernel (tc2_gemm_kernel) on the fp32 operand.
 // Pack fusion: the producer of an activation can store its operand image directly (A_img: the image of A, pitch rup32(K), already
 // written by whoever produced A; C_img: have THIS GEMM's epilogue store the image of its output, pitch rup32(N)) — the pack pass and
@@ -1700,7 +1700,7 @@ extern "C" GVD_API int gvd_op_linear_tc(const float* A, int64_t lda, const float
     g.M = M; g.N = N; g.K = K; g.nh = 1; g.act = act; g.alpha = 1.f;
     return gvd_gemm_nt_tc(g, 1, (cudaStream_t)stream);
 }
-// The conversion-free prologue GEMM (MODE_SS of wg_gemm_kernel) on its own: both operands are packed into fp16x3 images here (scratch from the
+// The conversion-free prologue GEMM (ss_gemm_kernel) on its own: both operands are packed into fp16x3 images here (scratch from the
 // stream-ordered allocator), optionally with the fp16x3 image of the output (img_out [M, rup32(N)] words) next to / instead of C.  Test hook.
 extern "C" GVD_API int gvd_op_linear_f16ss(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias, float* C, int64_t ldc,
                                            float* img_out, int M, int N, int K, int act, void* stream) {

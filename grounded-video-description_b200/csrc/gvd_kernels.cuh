@@ -164,8 +164,8 @@ void gvd_f16_scope(int delta);
 #define GVD_F16_SW 256.f
 // registry of pre-split constant weights (filled by gvd_model_finalize): fp32 weight pointer -> packed image (gvd_pack_f16x3)
 int gvd_pack_f16x3(const float* W, long long ldw, int N, int K, float* out, long long Kp, cudaStream_t st, float scale = GVD_F16_SW);
-// conversion-free GEMM on two operand images (gvd_wgmma.cu: MODE_SS)
-// Q|K|V projection epilogue of the region encoder (MODE_SS): Q as fp32, K as the per-head fp16x3 image, V as the image of V^T per clip
+// conversion-free GEMM on two operand images (gvd_wgmma.cu: ss_gemm_kernel)
+// Q|K|V projection epilogue of the region encoder (ss_gemm_kernel): Q as fp32, K as the per-head fp16x3 image, V as the image of V^T per clip
 struct GvdQkvImages { int HP, HS, KH, nh, R, Rp; float *k_img, *vt_img; float sk, sv; };
 int gvd_gemm_f16ss(const float* Ap, long long lda, const float* Wp, long long ldw, const float* bias, const float* scale2, const float* shift2, int act,
                    float* C, long long ldc, int M, int N, int K, cudaStream_t st, float* img = nullptr, long long ld_img = 0,

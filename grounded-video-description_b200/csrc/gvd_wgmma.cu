@@ -11,24 +11,27 @@
 //            already split, as the fp16x3 operand image of gvd_common.cuh: per row and 32-wide K slice 64 B
 //            of hi halves | 64 B of lo halves = one SWIZZLE_128B row of a K-major wgmma operand.
 //
-// One kernel serves the whole family.  Per CTA (one 128 x BN output tile, K streamed in 32-element =
-// 128-byte slices through a ring of stages).  The mode picks the tile width: BN = 128 for MODE_SS (both operands arrive as operand
-// images; the prologue's dense GEMMs, where wider tiles cut the L2 -> SM operand traffic per MAC by a third), BN = 64 for every other
-// mode (their epilogues are built around 64 columns or 16-unit gate boxes, and their N is small):
+// wg_gemm_kernel serves the whole family but the prologue's operand-image GEMMs.  Per CTA (one 128 x 64 output tile, K streamed in
+// 32-element = 128-byte slices through a ring of stages):
 //   warp 8    : TMA producer  - cp.async.bulk.tensor (SWIZZLE_128B) of the A / W slices, one mbarrier per stage
 //   warps 0-7 : two consumer warpgroups.  All 256 threads split the raw fp32 slices of the stage in shared
 //               memory (skipped for pre-split operands), fence.proxy.async, then each warpgroup issues the
 //               wgmma products of ITS 64 rows and folds the slice's result into fp32 register accumulators
-//               (round-to-nearest adds; the tensor core's own accumulation is only trusted for one slice).  At BN = 128
-//               each warpgroup issues m64n128k16 products; per output element the products and the fold are those of
-//               the 64-wide tile, so the result is bit-identical.  (9 warps: 3 share a 16K-register SM quarter, so
-//               ptxas caps the kernel at 168 registers; a second in-flight result set, 64 more, does not fit.)
+//               (round-to-nearest adds; the tensor core's own accumulation is only trusted for one slice).
 //   epilogue  : the accumulator fragments are exchanged through shared memory so that every thread owns one
 //               output row (thread <-> row, lane <-> row within the warp); the epilogues are written for
 //               that layout: bias / activation store, transposed split-K partial, fused LSTM cell, fused
-//               greedy pick, operand-image stores (Q|K|V projection), fused GRU cell.
+//               greedy pick, fused GRU cell.
 // Up to three K segments (different A / W tensors) feed one accumulator, so the LSTM gate GEMMs never
 // materialise a concatenated input (AttModel.py:138,147-160).
+//
+// ss_gemm_kernel runs the prologue's dense GEMMs, whose operands both arrive as fp16x3 operand images (nothing to convert), on
+// 128 x 128 tiles (a third less L2 -> SM operand traffic per MAC than 128 x 64) and warp-specialized, 384 threads:
+//   warpgroup 2    : TMA producer (one thread, setmaxnreg 40), the same 4-stage ring of 32 KB stages
+//   warpgroups 0-1 : consumers (setmaxnreg 232), 64 rows each.  The m64n128k16 products of slice i go into one of two result sets and
+//                    are in flight while slice i - 1 is folded from the other one, so the tensor core does not idle during the fold.
+// Per output element the products (lo.hi, hi.lo, hi.hi per k16 step, the first of a slice not accumulating) and the fold order are
+// those of wg_gemm_kernel's fp16x3 products, so both kernels give the same bits.
 #include <cuda.h>
 
 #include <algorithm>
@@ -40,13 +43,14 @@ namespace {
 
 constexpr int TC_BM = 128;
 constexpr int TC_BN = 64;
-constexpr int TC_BN_SS = 128;             // tile width of MODE_SS
 constexpr int WG_CONSUMERS = 256;         // two warpgroups
 constexpr int WG_THREADS = WG_CONSUMERS + 32;
 constexpr int WG_STAGES = 4;              // also at 128-wide tiles (32 KB stages): 6 stages measured no faster on the H100
 constexpr int WG_UJ = 16;                 // hidden units per CTA of the gate-interleaved tiles (LSTM: 4 x 16, GRU: 3 x 16 columns)
+constexpr int SS_BN = 128;                // tile width of ss_gemm_kernel
+constexpr int SS_THREADS = 384;           // two consumer warpgroups + the producer warpgroup
 
-enum { MODE_STORE = 0, MODE_LSTM = 1, MODE_PICK = 2, MODE_TRANS = 3, MODE_SS = 4, MODE_GRU = 5 };
+enum { MODE_STORE = 0, MODE_LSTM = 1, MODE_PICK = 2, MODE_TRANS = 3, MODE_GRU = 5 };
 
 struct TcSeg {
     int k_len;          // K extent of this segment
@@ -55,6 +59,8 @@ struct TcSeg {
 struct SsParams {
     float* C; long long ldc;
     int M, N;
+    int nk;                                             // 32-wide K slices
+    float oscale;                                       // inverse product of the operand images' power-of-two scales
     const float* bias; const float* scale2; const float* shift2; int act;
     uint32_t* img; long long ld_img; float img_scale;   // also store the fp16x3 operand image of the (activated) output: the next GEMM streams
                                                         // it directly; C may then be null (output consumed by that GEMM only)
@@ -107,7 +113,6 @@ struct TcParams {
     long long pk_stride;
     int pk_unk;
     const float* pk_embed; float* pk_xt; int pk_E;          // xt[M, E] = ReLU(embed[token]) for the next step
-    SsParams ss;
     GruStepParams gru;
 };
 
@@ -130,13 +135,21 @@ __device__ __forceinline__ void split_h4(const float4& v, float s, uint32_t& h01
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(WG_CONSUMERS) : "memory"); }
 
-template <bool F16, int BN> struct WgCfg {
-    static_assert(BN == 64 || (F16 && BN == 128), "tile widths: 64 (every mode), 128 (MODE_SS: fp16x3 operand images)");
+template <bool F16> struct WgCfg {
     static constexpr int A_BYTES = TC_BM * 128;            // one plane of the A slice (fp16x3: the whole slice, hi | lo halves per row)
-    static constexpr int B_BYTES = BN * 128;
+    static constexpr int B_BYTES = TC_BN * 128;
     static constexpr int STAGE = F16 ? (A_BYTES + B_BYTES) : 2 * (A_BYTES + B_BYTES);
     static constexpr int B_OFF = F16 ? A_BYTES : 2 * A_BYTES;
-    static constexpr int LDS = BN + 4;                     // pitch of the fp32 exchange tile of the epilogue
+    static constexpr int LDS = TC_BN + 4;                  // pitch of the fp32 exchange tile of the epilogue
+    static constexpr size_t SMEM = (size_t)WG_STAGES * STAGE + 1024 /*align*/ + 8 * 2 * WG_STAGES + 64;
+    static_assert((size_t)WG_STAGES * STAGE >= (size_t)TC_BM * LDS * 4, "the epilogue exchanges the C tile through the pipeline buffers");
+    static_assert(SMEM <= 232448, "shared-memory budget (227 KB per CTA)");
+};
+struct SsCfg {                                             // ss_gemm_kernel: both slices are fp16x3 images, hi | lo halves per 128-byte row
+    static constexpr int A_BYTES = TC_BM * 128;
+    static constexpr int B_BYTES = SS_BN * 128;
+    static constexpr int STAGE = A_BYTES + B_BYTES;
+    static constexpr int LDS = SS_BN + 4;
     static constexpr size_t SMEM = (size_t)WG_STAGES * STAGE + 1024 /*align*/ + 8 * 2 * WG_STAGES + 64;
     static_assert((size_t)WG_STAGES * STAGE >= (size_t)TC_BM * LDS * 4, "the epilogue exchanges the C tile through the pipeline buffers");
     static_assert(SMEM <= 232448, "shared-memory budget (227 KB per CTA)");
@@ -236,14 +249,181 @@ __device__ __forceinline__ void ss_store_row(const SsParams& p, const float (&ac
     }
 }
 
-template <bool F16, int BN>
+// C = A W^T on 128 x 128 tiles, both operands fp16x3 images.  Stage / phase schedule over nk slices: the producer fills slice i into
+// stage i % 4 once slice i - 4 is retired (empty parity ((i / 4) & 1) ^ 1); consumers wait full with parity (i / 4) & 1, issue slice i
+// into d[i & 1], then retire slice i - 1 (wgmma_wait<1>, arrive on empty, fold); the last slice is retired with wgmma_wait<0> and needs
+// no arrival (nothing is loaded after it).  tests/test_ss_pipeline_emulation.py runs this schedule on the CPU.
+__global__ void __launch_bounds__(SS_THREADS, 1)
+ss_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__ CUtensorMap mapW, const SsParams p) {
+    constexpr int ST = WG_STAGES;
+    extern __shared__ unsigned char smem_raw[];
+    unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
+    uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)ST * SsCfg::STAGE);
+    uint64_t* empty = full + ST;
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int m0 = blockIdx.y * TC_BM, n0 = blockIdx.x * SS_BN, nk = p.nk;
+
+    if (tid == 0) {
+        for (int s = 0; s < ST; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], WG_CONSUMERS / 32);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+    pdl_wait();                                 // (no-op unless launched with programmatic stream serialization)
+
+    if (warp >= WG_CONSUMERS / 32) {
+        // ------------------------------------------------------------------ TMA producer (warpgroup 2)
+        setmaxnreg_dec<40>();
+        if (tid == WG_CONSUMERS) {
+            prefetch_tmap(&mapA); prefetch_tmap(&mapW);
+            for (int i = 0; i < nk; ++i) {
+                const int s = i % ST;
+                mbar_wait(&empty[s], ((uint32_t)(i / ST) & 1u) ^ 1u);
+                unsigned char* st = smem + (size_t)s * SsCfg::STAGE;
+                mbar_expect_tx(&full[s], SsCfg::STAGE);
+                tma_load_4d(st, &mapA, &full[s], i * TC_BK, m0, 0, 0);
+                tma_load_4d(st + SsCfg::A_BYTES, &mapW, &full[s], i * TC_BK, n0, 0, 0);
+            }
+        }
+    } else {
+        // ------------------------------------------------------------------ consumer warpgroups (warps 0..7)
+        setmaxnreg_inc<232>();
+        const int wg = warp >> 2;
+        const float osc = p.oscale;
+        float acc[SS_BN / 2], d0[SS_BN / 2], d1[SS_BN / 2];
+#pragma unroll
+        for (int e = 0; e < SS_BN / 2; ++e) acc[e] = 0.f;
+        // products of this warpgroup's 64 rows for slice i, small terms first: lo.hi, hi.lo, hi.hi per K step (+32 bytes inside the
+        // swizzled row); the first product of the slice does not accumulate
+        auto issue = [&](int i, float (&d)[SS_BN / 2]) {
+            const int s = i % ST;
+            mbar_wait(&full[s], (uint32_t)(i / ST) & 1u);
+            const uint32_t st_addr = smem_u32(smem + (size_t)s * SsCfg::STAGE);
+            const uint64_t da = make_smem_desc_sw128(st_addr + (uint32_t)wg * 64u * 128u);
+            const uint64_t db = make_smem_desc_sw128(st_addr + SsCfg::A_BYTES);
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 2; ++ks) {
+                const uint64_t ah = da + 2 * ks, al = ah + 4, bh = db + 2 * ks, bl = bh + 4;
+                wgmma_f16(d, al, bh, ks == 0 ? 0u : 1u);
+                wgmma_f16(d, ah, bl, 1u);
+                wgmma_f16(d, ah, bh, 1u);
+            }
+            wgmma_commit();
+        };
+        // slice i (the older of the two groups in flight) is done: free its stage, fold it (undo the power-of-two operand scales, exact)
+        auto retire = [&](int i, float (&d)[SS_BN / 2]) {
+            wgmma_wait<1>(d);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[i % ST]);
+#pragma unroll
+            for (int e = 0; e < SS_BN / 2; ++e) acc[e] = fmaf(d[e], osc, acc[e]);
+        };
+        for (int i = 0; i < nk; i += 2) {
+            issue(i, d0);
+            if (i > 0) retire(i - 1, d1);
+            if (i + 1 < nk) {
+                issue(i + 1, d1);
+                retire(i, d0);
+            }
+        }
+        if ((nk - 1) & 1) {
+            wgmma_wait<0>(d1);
+#pragma unroll
+            for (int e = 0; e < SS_BN / 2; ++e) acc[e] = fmaf(d1[e], osc, acc[e]);
+        } else {
+            wgmma_wait<0>(d0);
+#pragma unroll
+            for (int e = 0; e < SS_BN / 2; ++e) acc[e] = fmaf(d0[e], osc, acc[e]);
+        }
+
+        // ------------------------------------------------------------------ fragment -> row exchange through the (idle) operand ring
+        constexpr int LDS_ = SsCfg::LDS;
+        float* Cs = reinterpret_cast<float*>(smem);
+        consumer_sync();                        // every warpgroup's products have read their last stage
+        {
+            const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
+#pragma unroll
+            for (int j = 0; j < SS_BN / 8; ++j) {
+                *reinterpret_cast<float2*>(Cs + r0 * LDS_ + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
+                *reinterpret_cast<float2*>(Cs + (r0 + 8) * LDS_ + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
+            }
+        }
+        consumer_sync();
+        if (p.qkv_hp) {
+            // Q|K|V projection: thread = (row, column half), this thread's 64 columns of row m
+            const int row = (warp & 3) * 32 + lane, m = m0 + row, cbeg = wg * (SS_BN / 2);
+            float a64[64];
+#pragma unroll
+            for (int j = 0; j < 64; j += 4) {
+                const float4 t = *reinterpret_cast<const float4*>(Cs + row * LDS_ + cbeg + j);
+                a64[j] = t.x; a64[j + 1] = t.y; a64[j + 2] = t.z; a64[j + 3] = t.w;
+            }
+            const bool vec_ok = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
+            ss_store_row<64>(p, a64, m, n0 + cbeg, lane, vec_ok);
+        } else {
+            // plain store: warp w takes rows w, w + 8, ...; lane l columns [4 l, 4 l + 4) of the tile, so one store instruction writes a
+            // 512-byte segment of C (or four whole 128-byte lines of the output image) instead of 16 bytes in each of 32 rows
+            const int c = 4 * lane, n = n0 + c;
+            float bv[4], sc2[4], sh2[4];
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const bool in = n + e < p.N;
+                bv[e] = (in && p.bias) ? __ldg(p.bias + n + e) : 0.f;
+                sc2[e] = (in && p.act == GVD_ACT_RELU_AFFINE_RELU) ? __ldg(p.scale2 + n + e) : 0.f;
+                sh2[e] = (in && p.act == GVD_ACT_RELU_AFFINE_RELU) ? __ldg(p.shift2 + n + e) : 0.f;
+            }
+            const bool vec_ok = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
+            for (int r = warp; r < TC_BM; r += WG_CONSUMERS / 32) {
+                const int m = m0 + r;
+                if (m >= p.M) break;
+                const float4 t = *reinterpret_cast<const float4*>(Cs + r * LDS_ + c);
+                float v[4] = {t.x, t.y, t.z, t.w};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {                   // the operations of ss_store_row, in the same order
+                    float x = v[e];
+                    if (n + e < p.N) {
+                        if (p.bias) x += bv[e];
+                        if (p.act >= GVD_ACT_RELU) x = fmaxf(x, 0.f);
+                        if (p.act == GVD_ACT_RELU_AFFINE_RELU) x = fmaxf(fmaf(x, sc2[e], sh2[e]), 0.f);
+                    } else {
+                        x = 0.f;                                // padding columns of the image are zeros
+                    }
+                    v[e] = x;
+                }
+                if (p.C) {
+                    float* dst = p.C + (long long)m * p.ldc + n;
+                    if (vec_ok && n + 3 < p.N) {
+                        *reinterpret_cast<float4*>(dst) = make_float4(v[0], v[1], v[2], v[3]);
+                    } else {
+#pragma unroll
+                        for (int e = 0; e < 4; ++e)
+                            if (n + e < p.N) dst[e] = v[e];
+                    }
+                }
+                if (p.img && n < p.ld_img) {                    // 4 columns = 2 hi words + 2 lo words of one K slice of the next GEMM
+                    uint32_t h0, l0, h1, l1;
+                    f16x3_split_pair(v[0], v[1], p.img_scale, h0, l0);
+                    f16x3_split_pair(v[2], v[3], p.img_scale, h1, l1);
+                    uint32_t* w = p.img + (long long)m * p.ld_img + f16x3_word(n);
+                    *reinterpret_cast<uint2*>(w) = make_uint2(h0, h1);
+                    *reinterpret_cast<uint2*>(w + 16) = make_uint2(l0, l1);
+                }
+            }
+        }
+    }
+}
+
+template <bool F16>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
                const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapW0,
                const __grid_constant__ CUtensorMap mapW1, const __grid_constant__ CUtensorMap mapW2, const TcParams p) {
-    using Cfg = WgCfg<F16, BN>;
+    using Cfg = WgCfg<F16>;
     constexpr int ST = WG_STAGES;
-    constexpr bool WIDE = BN == 128;            // MODE_SS only: both operands arrive as operand images, nothing to convert
     extern __shared__ unsigned char smem_raw[];
     unsigned char* smem = reinterpret_cast<unsigned char*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~(uintptr_t)1023);
     uint64_t* full = reinterpret_cast<uint64_t*>(smem + (size_t)ST * Cfg::STAGE);
@@ -253,7 +433,7 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
     const int zb = p.ksplit ? 0 : blockIdx.z / p.nh, zh = p.ksplit ? 0 : blockIdx.z % p.nh;
     const int kz = p.ksplit * (int)blockIdx.z;
     const int m0 = blockIdx.y * TC_BM;
-    const int n0 = blockIdx.x * (p.nbox > 1 ? WG_UJ : BN);        // first output column / first hidden unit (gate-interleaved tiles)
+    const int n0 = blockIdx.x * (p.nbox > 1 ? WG_UJ : TC_BN);        // first output column / first hidden unit (gate-interleaved tiles)
 
     if (tid == 0) {
         for (int s = 0; s < ST; ++s) {
@@ -297,9 +477,9 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
 
     // ---------------------------------------------------------------------- consumer warpgroups (warps 0..7)
     const int wg = warp >> 2;
-    float acc[BN / 2];
+    float acc[TC_BN / 2];
 #pragma unroll
-    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+    for (int j = 0; j < TC_BN / 2; ++j) acc[j] = 0.f;
     const float* Fz = p.Fc ? p.Fc + (long long)blockIdx.z * p.ngrp * p.M : nullptr;
     {
         int i = 0;
@@ -309,9 +489,7 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                 const int s = i % ST;
                 mbar_wait(&full[s], (uint32_t)(i / ST) & 1u);
                 const uint32_t st_addr = smem_u32(smem + (size_t)s * Cfg::STAGE);
-                if constexpr (WIDE) {
-                    // both operands arrived as operand images: nothing to convert
-                } else if constexpr (F16) {
+                if constexpr (F16) {
                     // ---- raw fp32 slice -> operand image, in place: a 128-byte row of 32 floats becomes 64 B of hi halves | 64 B of lo halves.
                     // Chunk pair c2 (2 x 16 B = 8 floats) of a row -> hi chunk c2, lo chunk 4 + c2; the threads that share a row are
                     // neighbouring lanes of one warp: read, __syncwarp, write.
@@ -385,7 +563,7 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                     consumer_sync();
                 }
                 // ---- products of this warpgroup's 64 rows, small terms first: lo.hi, hi.lo, hi.hi per K step (+32 bytes inside the swizzled row)
-                float d[BN / 2];
+                float d[TC_BN / 2];
                 const uint64_t da = make_smem_desc_sw128(st_addr + (uint32_t)wg * 64u * 128u);
                 const uint64_t db = make_smem_desc_sw128(st_addr + Cfg::B_OFF);
                 wgmma_fence();
@@ -412,7 +590,7 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
                 __syncwarp();
                 if (lane == 0) mbar_arrive(&empty[s]);          // stage free once this warp's MMAs have read it
 #pragma unroll
-                for (int e = 0; e < BN / 2; ++e) {
+                for (int e = 0; e < TC_BN / 2; ++e) {
                     if constexpr (F16) acc[e] = fmaf(d[e], p.oscale, acc[e]);      // undo the power-of-two operand scales (exact)
                     else acc[e] += d[e];
                 }
@@ -427,26 +605,16 @@ wg_gemm_kernel(const __grid_constant__ CUtensorMap mapA0, const __grid_constant_
     {
         const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2), c0 = 2 * (lane & 3);
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
+        for (int j = 0; j < TC_BN / 8; ++j) {
             *reinterpret_cast<float2*>(Cs + r0 * LDS_ + 8 * j + c0) = make_float2(acc[4 * j], acc[4 * j + 1]);
             *reinterpret_cast<float2*>(Cs + (r0 + 8) * LDS_ + 8 * j + c0) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
         }
     }
     consumer_sync();
     const int q = warp & 3, row = q * 32 + lane, m = m0 + row;
-    const int cbeg = (warp >> 2) * (BN / 2);    // thread = (row, column half) in the modes that use all eight warps
+    const int cbeg = (warp >> 2) * (TC_BN / 2);    // thread = (row, column half) in the modes that use all eight warps
 
-    if constexpr (WIDE) {
-        // MODE_SS: this thread's 64 columns of row m
-        float a64[64];
-#pragma unroll
-        for (int j = 0; j < 64; j += 4) {
-            const float4 t = *reinterpret_cast<const float4*>(Cs + row * LDS_ + cbeg + j);
-            a64[j] = t.x; a64[j + 1] = t.y; a64[j + 2] = t.z; a64[j + 3] = t.w;
-        }
-        const bool vec_ok = (p.ss.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.ss.C) & 15) == 0);
-        ss_store_row<64>(p.ss, a64, m, n0 + cbeg, lane, vec_ok);
-    } else if (p.mode == MODE_STORE) {
+    if (p.mode == MODE_STORE) {
         // bias / activation, whole contiguous row segments per store instruction (128-bit, coalesced)
         const float* bias = p.bias ? p.bias + zb * p.sBb : nullptr;
         float* C = p.C + zb * p.sCb + zh * p.sCh;
@@ -658,33 +826,19 @@ __global__ void pack_f16x3_kernel(const float* __restrict__ W, long long ldw, in
     out[n * Kp + kb * 32 + 16 + pr] = f16x3_pack_pair(x0 - a0, x1 - a1);
 }
 
-// every mode but MODE_SS: 128 x 64 tiles
+// 128 x 64 tiles
 int launch_wg(const CUtensorMap* mA, const CUtensorMap* mW, const TcParams& p, dim3 grid, cudaStream_t st) {
     static bool attr_set = false;
     if (!attr_set) {
-        GVD_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<false, TC_BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<false, TC_BN>::SMEM));
-        GVD_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<true, TC_BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<true, TC_BN>::SMEM));
+        GVD_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<false>::SMEM));
+        GVD_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WgCfg<true>::SMEM));
         attr_set = true;
     }
-    GVD_REQUIRE(p.mode != MODE_SS, "tcgemm: MODE_SS runs on the 128-wide tiles (launch_wg_ss)");
     GVD_REQUIRE(p.f16 || (!p.apre && !p.wpre), "tcgemm: operand images belong to the fp16x3 products");
     if (p.f16)
-        GVD_CHECK_CUDA(gvd_launch(wg_gemm_kernel<true, TC_BN>, grid, dim3(WG_THREADS), WgCfg<true, TC_BN>::SMEM, st, mA[0], mA[1], mA[2], mW[0], mW[1], mW[2], p));
+        GVD_CHECK_CUDA(gvd_launch(wg_gemm_kernel<true>, grid, dim3(WG_THREADS), WgCfg<true>::SMEM, st, mA[0], mA[1], mA[2], mW[0], mW[1], mW[2], p));
     else
-        GVD_CHECK_CUDA(gvd_launch(wg_gemm_kernel<false, TC_BN>, grid, dim3(WG_THREADS), WgCfg<false, TC_BN>::SMEM, st, mA[0], mA[1], mA[2], mW[0], mW[1], mW[2], p));
-    GVD_CHECK_LAUNCH();
-    return 0;
-}
-// MODE_SS: 128 x 128 tiles, both operands fp16x3 images (the W tensor map's box has TC_BN_SS rows)
-int launch_wg_ss(const CUtensorMap* mA, const CUtensorMap* mW, const TcParams& p, dim3 grid, cudaStream_t st) {
-    using Cfg = WgCfg<true, TC_BN_SS>;
-    static bool attr_set = false;
-    if (!attr_set) {
-        GVD_CHECK_CUDA(cudaFuncSetAttribute(wg_gemm_kernel<true, TC_BN_SS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM));
-        attr_set = true;
-    }
-    GVD_REQUIRE(p.mode == MODE_SS && p.f16 && p.apre && p.wpre && p.nbox <= 1 && !p.ksplit, "tcgemm: the 128-wide tiles serve MODE_SS only");
-    GVD_CHECK_CUDA(gvd_launch(wg_gemm_kernel<true, TC_BN_SS>, grid, dim3(WG_THREADS), Cfg::SMEM, st, mA[0], mA[1], mA[2], mW[0], mW[1], mW[2], p));
+        GVD_CHECK_CUDA(gvd_launch(wg_gemm_kernel<false>, grid, dim3(WG_THREADS), WgCfg<false>::SMEM, st, mA[0], mA[1], mA[2], mW[0], mW[1], mW[2], p));
     GVD_CHECK_LAUNCH();
     return 0;
 }
@@ -861,19 +1015,13 @@ int gvd_gemm_f16ss(const float* Ap, long long lda, const float* Wp, long long ld
     GVD_REQUIRE(!img || (ld_img % 32 == 0 && ld_img >= N), "gemm_f16ss: the output image needs a 32-multiple pitch >= N");
     const int Kp = (K + 31) / 32 * 32;
     GVD_REQUIRE(lda >= Kp && ldw >= Kp, "gemm_f16ss: operand images must cover K rounded up to 32");
-    CUtensorMap mA[3], mW[3];
-    TcParams p{};
-    GVD_TRY(make_map(&mA[0], Ap, Kp, M, lda, 1, 0, 1, 0, TC_BM, &p.a_mul_h, &p.a_mul_b));
-    GVD_TRY(make_map(&mW[0], Wp, Kp, N, ldw, 1, 0, 1, 0, TC_BN_SS, &p.w_mul_h, &p.w_mul_b));
-    mA[1] = mA[2] = mA[0];
-    mW[1] = mW[2] = mW[0];
-    p.nseg = 1;
-    p.seg[0] = TcSeg{Kp, 0, 0};
-    p.M = M; p.N = N; p.nh = 1;
-    p.mode = MODE_SS;
-    p.f16 = 1; p.apre = p.wpre = 1; p.sa = p.sw = 1.f; p.oscale = 1.f / (GVD_F16_SA * GVD_F16_SW);
-    SsParams& s = p.ss;
+    CUtensorMap mA, mW;
+    int unused;
+    GVD_TRY(make_map(&mA, Ap, Kp, M, lda, 1, 0, 1, 0, TC_BM, &unused, &unused));
+    GVD_TRY(make_map(&mW, Wp, Kp, N, ldw, 1, 0, 1, 0, SS_BN, &unused, &unused));
+    SsParams s{};
     s.C = C; s.ldc = ldc; s.M = M; s.N = N;
+    s.nk = Kp / TC_BK; s.oscale = 1.f / (GVD_F16_SA * GVD_F16_SW);
     s.bias = bias; s.scale2 = scale2; s.shift2 = shift2; s.act = act;
     s.img = reinterpret_cast<uint32_t*>(img); s.ld_img = ld_img; s.img_scale = GVD_F16_SA;
     if (qkv) {
@@ -881,7 +1029,15 @@ int gvd_gemm_f16ss(const float* Ap, long long lda, const float* Wp, long long ld
         s.k_img = reinterpret_cast<uint32_t*>(qkv->k_img); s.vt_img = reinterpret_cast<uint32_t*>(qkv->vt_img);
         s.qkv_sk = qkv->sk; s.qkv_sv = qkv->sv;
     }
-    return launch_wg_ss(mA, mW, p, dim3(gvd_cdiv(N, TC_BN_SS), gvd_cdiv(M, TC_BM), 1), st);
+    static bool attr_set = false;
+    if (!attr_set) {
+        GVD_CHECK_CUDA(cudaFuncSetAttribute(ss_gemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SsCfg::SMEM));
+        attr_set = true;
+    }
+    const dim3 grid(gvd_cdiv(N, SS_BN), gvd_cdiv(M, TC_BM), 1);
+    GVD_CHECK_CUDA(gvd_launch(ss_gemm_kernel, grid, dim3(SS_THREADS), SsCfg::SMEM, st, mA, mW, s));
+    GVD_CHECK_LAUNCH();
+    return 0;
 }
 
 // C = act(alpha * A W^T + bias) with the GemmArgs contract of gvd_gemm.cuh (batched over (b,h))

@@ -71,13 +71,13 @@ __device__ __forceinline__ void wgmma_f16(float (&d)[64], uint64_t da, uint64_t 
         : WG_D64(d)
         : "l"(da), "l"(db), "r"(accumulate));
 }
+template <int N> __device__ __forceinline__ void wgmma_wait(float (&d)[64]) {
+    asm volatile("wgmma.wait_group.sync.aligned %64;" : WG_D64(d) : "n"(N) : "memory");
+}
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait0(float (&d)[32]) {
     asm volatile("wgmma.wait_group.sync.aligned 0;" : WG_D32(d) : : "memory");
-}
-__device__ __forceinline__ void wgmma_wait0(float (&d)[64]) {
-    asm volatile("wgmma.wait_group.sync.aligned 0;" : WG_D64(d) : : "memory");
 }
 // D[64 x 32], both operands in shared memory (the score product of the fused self-attention): fragment layout as above with j = 0..3
 __device__ __forceinline__ void wgmma_f16(float (&d)[16], uint64_t da, uint64_t db, uint32_t accumulate) {
@@ -123,7 +123,10 @@ template <int N> __device__ __forceinline__ void wgmma_wait(float (&d)[48]) {
     asm volatile("wgmma.wait_group.sync.aligned %48;" : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]) : "n"(N) : "memory");
 }
 
-// ------------------------------------------------------------------------------------ host side
+// register budget of a warp-specialized kernel: the producer warpgroup gives registers back, the consumer warpgroups take them
+template <int N> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ------------------------------------------------------------------------------------ host side
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                   const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
