@@ -81,7 +81,7 @@ def lib():
     L.gvd_op_linear.argtypes = [vp, i64, vp, i64, vp, vp, i64, ci, ci, ci, ci, vp]
     L.gvd_op_tanh.argtypes = [vp, vp, ci, vp]
     L.gvd_op_linear_tc.argtypes = [vp, i64, vp, i64, vp, vp, i64, ci, ci, ci, ci, vp]
-    L.gvd_op_linear_f16ss.argtypes = [vp, i64, vp, i64, vp, vp, i64, vp, ci, ci, ci, ci, vp]
+    L.gvd_op_linear_f16ss.argtypes = [vp, i64, vp, i64, vp, vp, i64, vp, ci, ci, ci, ci, ci, ci, ci, vp, vp, ci, vp]
     L.gvd_op_scores_tc.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, i64, vp]
     L.gvd_op_self_attention_tc.argtypes = [vp, vp, ci, ci, ci, ci, ci, ctypes.c_float, vp, vp, ci, vp]
     L.gvd_op_self_attention_fused.argtypes = [vp, vp, ci, ci, ci, ci, ci, ctypes.c_float, vp, ctypes.c_int64, vp]
@@ -688,14 +688,23 @@ def op_linear(A, W, bias=None, act=0, tc=False):
     return C
 
 
-def op_linear_f16ss(A, W, bias=None, act=0, want_img=False, want_c=True):
-    """The conversion-free persistent GEMM on its own; returns C [M,N] and / or the fp16x3 image of C as int32 words [M, rup32(N)]."""
+def op_linear_f16ss(A, W, bias=None, act=0, want_img=False, want_c=True, qkv=None):
+    """The conversion-free persistent GEMM on its own; returns C [M,N] and / or the fp16x3 image of C as int32 words [M, rup32(N)].
+    qkv = (nh, hs, R, C, k_img, vt_img, ref): the region encoder's Q|K|V projection into the caller's buffers (C [M, N] fp32, k_img
+    [M, nh, rup32(hs)] and vt_img [M / R, nh * hs, rup32(R)] int32 words); ref=True builds the images from the fp32 product with the
+    separate pack passes (and writes all of C), else the projection's epilogue writes them (and only Q, C[:, :nh * hs]).  Returns None."""
     M, K = A.shape
     N = W.shape[0]
+    p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
+    if qkv is not None:
+        nh, hs, R, C, k_img, vt_img, ref = qkv
+        check(lib().gvd_op_linear_f16ss(p(A), A.stride(0), p(W), W.stride(0), None, p(C), C.stride(0), None, M, N, K, 0,
+                                        nh, hs, R, p(k_img), p(vt_img), int(bool(ref)), _stream()))
+        return None
     C = torch.empty(M, N, dtype=torch.float32, device="cuda") if want_c else None
     img = torch.empty(M, (N + 31) // 32 * 32, dtype=torch.int32, device="cuda") if want_img else None
-    p = lambda t: ctypes.c_void_p(t.data_ptr()) if t is not None else None
-    check(lib().gvd_op_linear_f16ss(p(A), A.stride(0), p(W), W.stride(0), p(bias), p(C), N, p(img), M, N, K, int(act), _stream()))
+    check(lib().gvd_op_linear_f16ss(p(A), A.stride(0), p(W), W.stride(0), p(bias), p(C), N, p(img), M, N, K, int(act),
+                                    0, 0, 0, None, None, 0, _stream()))
     return (C, img) if want_img else C
 
 

@@ -1701,10 +1701,16 @@ extern "C" GVD_API int gvd_op_linear_tc(const float* A, int64_t lda, const float
     return gvd_gemm_nt_tc(g, 1, (cudaStream_t)stream);
 }
 // The conversion-free prologue GEMM (ss_gemm_kernel) on its own: both operands are packed into fp16x3 images here (scratch from the
-// stream-ordered allocator), optionally with the fp16x3 image of the output (img_out [M, rup32(N)] words) next to / instead of C.  Test hook.
+// stream-ordered allocator), optionally with the fp16x3 image of the output (img_out [M, rup32(N)] words) next to / instead of C.
+// nh > 0: the Q|K|V projection of the region encoder (N = 3 nh hs, clips of R rows, no bias / activation): Q to C[:, 0:HP), K to the
+// per-head image k_img [M, nh, rup32(hs)] words, V to the image of V^T per clip vt_img [M / R, HP, rup32(R)] words.  qkv_ref: the same
+// images from the fp32 product in C[M, N] followed by the pack passes of the unfused path.  Test hook.
 extern "C" GVD_API int gvd_op_linear_f16ss(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias, float* C, int64_t ldc,
-                                           float* img_out, int M, int N, int K, int act, void* stream) {
+                                           float* img_out, int M, int N, int K, int act, int nh, int hs, int R, float* k_img, float* vt_img,
+                                           int qkv_ref, void* stream) {
     GVD_REQUIRE(A && W && (C || img_out) && M > 0 && N > 0 && K > 0, "op_linear_f16ss: null argument");
+    GVD_REQUIRE(nh == 0 || (nh > 0 && hs > 0 && R > 0 && M % R == 0 && N == 3 * nh * hs && k_img && vt_img && C && !img_out),
+                "op_linear_f16ss: Q|K|V mode needs N = 3 nh hs, whole clips, C, k_img and vt_img");
     cudaStream_t st = (cudaStream_t)stream;
     const long long Kp = (K + 31) / 32 * 32, Np = (N + 31) / 32 * 32;
     float *Ai = nullptr, *Wi = nullptr;
@@ -1712,7 +1718,15 @@ extern "C" GVD_API int gvd_op_linear_f16ss(const float* A, int64_t lda, const fl
     GVD_CHECK_CUDA(cudaMallocAsync((void**)&Wi, (size_t)N * Kp * 4, st));
     int rc = gvd_pack_f16x3(A, lda, M, K, Ai, Kp, st, GVD_F16_SA);
     if (!rc) rc = gvd_pack_f16x3(W, ldw, N, K, Wi, Kp, st, GVD_F16_SW);
-    if (!rc) rc = gvd_gemm_f16ss(Ai, Kp, Wi, Kp, bias, nullptr, nullptr, act, C, ldc, M, N, K, st, img_out, img_out ? Np : 0);
+    const int HP = nh * hs, KH = (hs + 31) / 32 * 32, Rp = (R + 31) / 32 * 32;
+    if (!rc && nh && !qkv_ref) {
+        GvdQkvImages qi{HP, hs, KH, nh, R, Rp, k_img, vt_img, GVD_ATT_SK, GVD_ATT_SV};
+        rc = gvd_gemm_f16ss(Ai, Kp, Wi, Kp, bias, nullptr, nullptr, act, C, ldc, M, N, K, st, nullptr, 0, &qi);
+    } else if (!rc) {
+        rc = gvd_gemm_f16ss(Ai, Kp, Wi, Kp, bias, nullptr, nullptr, act, C, ldc, M, N, K, st, img_out, img_out ? Np : 0);
+        if (!rc && nh) rc = gvd_pack_heads_f16x3(C + HP, ldc, M, nh, hs, hs, KH, GVD_ATT_SK, k_img, st);
+        if (!rc && nh) rc = gvd_transpose_pack_f16x3(C + 2 * HP, vt_img, M / R, R, HP, (int)ldc, Rp, GVD_ATT_SV, st);
+    }
     cudaFreeAsync(Ai, st);
     cudaFreeAsync(Wi, st);
     return rc;

@@ -155,95 +155,77 @@ struct SsCfg {                                             // ss_gemm_kernel: bo
     static_assert(SMEM <= 232448, "shared-memory budget (227 KB per CTA)");
 };
 
-// Epilogue store of one thread's output row segment: acc[0..ACC) = columns [ncol0, ncol0 + ACC) of row m (thread <-> row, lane <-> row within the
-// warp).  Plain mode: bias / activation, fp32 C and / or the fp16x3 image of the output; Q|K|V mode (p.qkv_hp): Q as fp32, K as the per-head
-// image, V as the image of V^T (lane pairs exchange rows with one shuffle per column).
-template <int ACC>
-__device__ __forceinline__ void ss_store_row(const SsParams& p, const float (&acc)[ACC], const int m, const int ncol0, const int lane, const bool vec_ok) {
-    const int n0 = ncol0, cbeg = 0;
-    if (p.qkv_hp) {
-        // (warp-uniform branches: n is the same for every lane; lane <-> row, so lane ^ 1 holds the other row of an fp16 pair)
-        const bool row_ok = m < p.M;
-        const int HP = p.qkv_hp, HS = p.qkv_hs, KH = p.qkv_kh;
-        const int bclip = m / p.qkv_R, r = m - bclip * p.qkv_R;
-        float* dq = p.C + (long long)m * p.ldc;
-        uint32_t* dk = p.k_img + (long long)m * p.qkv_nh * KH;
-        uint32_t* dv = p.vt_img + (long long)bclip * HP * p.qkv_Rp + f16x3_word(r & ~1) + ((lane & 1) ? 16 : 0);
-        const bool last_pair = (r | 1) == p.qkv_R - 1 && (p.qkv_R & 31) != 0;         // this row pair also zeroes the words of rows [R, Rp)
-        const int vpad = 16 - ((p.qkv_R & 31) >> 1);
+// Q|K|V epilogue of ss_gemm_kernel (p.qkv_hp): stores the exchanged fp32 tile Cs (rows m0.., columns n0..) so that one store instruction
+// of a warp writes whole 128-byte lines.  Every output word belongs to exactly one tile: a 4-column group (never straddles a tile, a head or
+// Q / K / V: HS % 4 == HP % 4 == 0) to the tile holding its columns, the K padding words [HS, KH) of a head to the tile holding the head's
+// last group, the V^T pad rows [R, Rp) of a clip to the tile holding the clip's last row.  tests/test_qkv_epilogue_emulation.py runs this
+// plan over every tile of a launch on the CPU.
+__device__ __forceinline__ void ss_store_qkv(const SsParams& p, const float* Cs, const int m0, const int n0, const int warp, const int lane) {
+    constexpr int LDS_ = SsCfg::LDS, NW = WG_CONSUMERS / 32;
+    const int HP = p.qkv_hp, HS = p.qkv_hs, KH = p.qkv_kh, R = p.qkv_R, mend = min(m0 + TC_BM, p.M);
+    // Q (columns [0, HP) -> fp32 C): warp <-> row, lane l <-> columns [4 l, 4 l + 4), a 512-byte segment of C per instruction
+    if (n0 < HP) {
+        const int c = 4 * lane;
+        for (int r = warp; m0 + r < mend; r += NW)
+            if (n0 + c < HP)
+                *reinterpret_cast<float4*>(p.C + (long long)(m0 + r) * p.ldc + n0 + c) = *reinterpret_cast<const float4*>(Cs + r * LDS_ + c);
+    }
+    // K (columns [HP, 2HP) -> k_img[(m * nh + h) * KH + word(c)]): warp <-> row, lane <-> 4-word quad u of a head's image row, which holds
+    // the hi (u & 4 == 0) or lo words of the two groups at columns 32 (u >> 3) + 8 (u & 3) + {0, 4}; 32 consecutive quads are 4 whole lines
+    const int ka = max(n0, HP) - HP, kb = min(n0 + SS_BN, 2 * HP) - HP;        // this tile's K columns [ka, kb)
+    if (ka < kb) {
+        const int KQ = KH / 4, hlo = ka / HS, hhi = (kb - 1) / HS;
+        const int q0 = hlo * KQ + ((ka - hlo * HS) >> 5) * 8;                  // from the 32-column slice holding column ka ...
+        const int q1 = hhi * HS + HS - 4 < kb ? (hhi + 1) * KQ                  // ... to the end of head hhi's padding if its last group is here
+                                              : hhi * KQ + (((kb - 1 - hhi * HS) >> 5) + 1) * 8;
+        for (int r = warp; m0 + r < mend; r += NW) {
+            uint32_t* dk = p.k_img + (long long)(m0 + r) * p.qkv_nh * KH;
+            for (int q = q0 + lane; q < q1; q += 32) {
+                const int h = q / KQ, u = q - h * KQ, c = (u >> 3) * 32 + (u & 3) * 8, last = h * HS + HS - 4;
+                bool own[2];
+                uint32_t w[4];
 #pragma unroll
-        for (int j = 0; j < ACC; j += 4) {
-            const int n = n0 + cbeg + j;
-            if (n >= p.N) break;
-            const float v0 = acc[j], v1 = acc[j + 1], v2 = acc[j + 2], v3 = acc[j + 3];
-            if (n < HP) {
-                if (row_ok) *reinterpret_cast<float4*>(dq + n) = make_float4(v0, v1, v2, v3);
-            } else if (n < 2 * HP) {
-                const int kc = n - HP, h = kc / HS, c = kc - h * HS;
-                if (row_ok) {
+                for (int e = 0; e < 2; ++e) {
+                    const int g = c + 4 * e, kc = h * HS + g;
+                    own[e] = g < HS ? (kc >= ka && kc < kb) : (last >= ka && last < kb);
+                    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);                 // padding words are the split of zeros
+                    if (g < HS && own[e]) v = *reinterpret_cast<const float4*>(Cs + r * LDS_ + HP + kc - n0);
                     uint32_t h0, l0, h1, l1;
-                    f16x3_split_pair(v0, v1, p.qkv_sk, h0, l0);
-                    f16x3_split_pair(v2, v3, p.qkv_sk, h1, l1);
-                    uint32_t* w = dk + h * KH + f16x3_word(c);
-                    *reinterpret_cast<uint2*>(w) = make_uint2(h0, h1);
-                    *reinterpret_cast<uint2*>(w + 16) = make_uint2(l0, l1);
-                    if (c + 4 >= HS && HS < KH) {                        // last group of the head: zero the words of columns [HS, KH)
-                        uint32_t* z = dk + h * KH + f16x3_word(HS);
-                        for (int i = 0; i < (KH - HS) / 2; ++i) { z[i] = 0u; z[i + 16] = 0u; }
-                    }
+                    f16x3_split_pair(v.x, v.y, p.qkv_sk, h0, l0);
+                    f16x3_split_pair(v.z, v.w, p.qkv_sk, h1, l1);
+                    w[2 * e] = (u & 4) ? l0 : h0;
+                    w[2 * e + 1] = (u & 4) ? l1 : h1;
                 }
-            } else {
-                const int c = n - 2 * HP;
-                const float vv[4] = {v0, v1, v2, v3};
+                uint32_t* d = dk + h * KH + 4 * u;
+                if (own[0] && own[1]) *reinterpret_cast<uint4*>(d) = make_uint4(w[0], w[1], w[2], w[3]);
+                else if (own[0]) *reinterpret_cast<uint2*>(d) = make_uint2(w[0], w[1]);
+                else if (own[1]) *reinterpret_cast<uint2*>(d + 2) = make_uint2(w[2], w[3]);
+            }
+        }
+    }
+    // V (columns [2HP, 3HP) -> vt_img[(b * HP + c) * Rp + word(r)]): warp <-> (32-row line k of clip b, 4 columns), lane l <-> row 32 k + l.
+    // Lane pairs exchange their rows; the even lane stores the hi, the odd lane the lo word of the pair, so each store instruction writes
+    // one 128-byte line.  Pairs never straddle a tile (m0 % 128 == 0, R even).
+    const int va = max(n0, 2 * HP), vb = min(n0 + SS_BN, p.N);                 // this tile's V columns [va, vb)
+    if (va < vb) {
+        const int ng = (vb - va) / 4;
+        for (int b = m0 / R; b * R < mend; ++b) {
+            const int base = b * R, ra = max(m0, base) - base, rb = min(mend, base + R) - base;   // this tile's rows [ra, rb) of clip b
+            const int k0 = ra >> 5, nl = ((rb - 1) >> 5) - k0 + 1;
+            for (int t = warp; t < nl * ng; t += NW) {
+                const int k = k0 + t / ng, n = va + 4 * (t % ng), r = 32 * k + lane;
+                const bool own = r < R ? (r >= ra && r < rb) : rb == R;
+                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);                     // pad rows are the split of zeros
+                if (r < R && own) v = *reinterpret_cast<const float4*>(Cs + (base + r - m0) * LDS_ + n - n0);
+                const float vv[4] = {v.x, v.y, v.z, v.w};
+                uint32_t* d = p.vt_img + ((long long)b * HP + n - 2 * HP) * p.qkv_Rp + 32 * k + (lane & 1) * 16 + (lane >> 1);
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     const float o = __shfl_xor_sync(0xffffffffu, vv[e], 1);
                     uint32_t hi, lo;
                     if (lane & 1) f16x3_split_pair(o, vv[e], p.qkv_sv, hi, lo); else f16x3_split_pair(vv[e], o, p.qkv_sv, hi, lo);
-                    if (row_ok) {
-                        uint32_t* w = dv + (long long)(c + e) * p.qkv_Rp;      // even lane: hi word, odd lane: lo word of the pair (r & ~1, r | 1)
-                        *w = (lane & 1) ? lo : hi;
-                        if (last_pair) for (int i = 1; i <= vpad; ++i) w[i] = 0u;
-                    }
+                    if (own) d[(long long)e * p.qkv_Rp] = (lane & 1) ? lo : hi;
                 }
-            }
-        }
-    } else if (m < p.M) {
-        float* dst = p.C ? p.C + (long long)m * p.ldc + n0 + cbeg : nullptr;
-        uint32_t* idst = p.img ? p.img + (long long)m * p.ld_img : nullptr;
-#pragma unroll
-        for (int j = 0; j < ACC; j += 4) {
-            const int n = n0 + cbeg + j;
-            float v[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                float x = acc[j + e];
-                const int nn = n + e;
-                if (nn < p.N) {
-                    if (p.bias) x += __ldg(p.bias + nn);
-                    if (p.act >= GVD_ACT_RELU) x = fmaxf(x, 0.f);
-                    if (p.act == GVD_ACT_RELU_AFFINE_RELU) x = fmaxf(fmaf(x, __ldg(p.scale2 + nn), __ldg(p.shift2 + nn)), 0.f);
-                } else {
-                    x = 0.f;                                        // padding columns of the image are zeros
-                }
-                v[e] = x;
-            }
-            if (dst) {
-                if (vec_ok && n + 3 < p.N) {
-                    *reinterpret_cast<float4*>(dst + j) = make_float4(v[0], v[1], v[2], v[3]);
-                } else {
-#pragma unroll
-                    for (int e = 0; e < 4; ++e)
-                        if (n + e < p.N) dst[j + e] = v[e];
-                }
-            }
-            if (idst && n < p.ld_img) {                             // 4 columns = 2 hi words + 2 lo words of one K slice of the next GEMM
-                uint32_t h0, l0, h1, l1;
-                f16x3_split_pair(v[0], v[1], p.img_scale, h0, l0);
-                f16x3_split_pair(v[2], v[3], p.img_scale, h1, l1);
-                uint32_t* w = idst + f16x3_word(n);
-                *reinterpret_cast<uint2*>(w) = make_uint2(h0, h1);
-                *reinterpret_cast<uint2*>(w + 16) = make_uint2(l0, l1);
             }
         }
     }
@@ -354,16 +336,7 @@ ss_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
         }
         consumer_sync();
         if (p.qkv_hp) {
-            // Q|K|V projection: thread = (row, column half), this thread's 64 columns of row m
-            const int row = (warp & 3) * 32 + lane, m = m0 + row, cbeg = wg * (SS_BN / 2);
-            float a64[64];
-#pragma unroll
-            for (int j = 0; j < 64; j += 4) {
-                const float4 t = *reinterpret_cast<const float4*>(Cs + row * LDS_ + cbeg + j);
-                a64[j] = t.x; a64[j + 1] = t.y; a64[j + 2] = t.z; a64[j + 3] = t.w;
-            }
-            const bool vec_ok = (p.ldc % 4 == 0) && ((reinterpret_cast<uintptr_t>(p.C) & 15) == 0);
-            ss_store_row<64>(p, a64, m, n0 + cbeg, lane, vec_ok);
+            ss_store_qkv(p, Cs, m0, n0, warp, lane);
         } else {
             // plain store: warp w takes rows w, w + 8, ...; lane l columns [4 l, 4 l + 4) of the tile, so one store instruction writes a
             // 512-byte segment of C (or four whole 128-byte lines of the output image) instead of 16 bytes in each of 32 rows
@@ -383,7 +356,7 @@ ss_gemm_kernel(const __grid_constant__ CUtensorMap mapA, const __grid_constant__
                 const float4 t = *reinterpret_cast<const float4*>(Cs + r * LDS_ + c);
                 float v[4] = {t.x, t.y, t.z, t.w};
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {                   // the operations of ss_store_row, in the same order
+                for (int e = 0; e < 4; ++e) {
                     float x = v[e];
                     if (n + e < p.N) {
                         if (p.bias) x += bv[e];

@@ -192,9 +192,13 @@ GVD_API int gvd_op_self_attention_tc(const float* qkv, float* out, int nb, int n
 GVD_API int gvd_op_self_attention_fused(const float* qkv, float* out, int nb, int nh, int R, int hs, int HP, float scale, float* img,
                   int64_t img_ld, void* stream);
 /* the conversion-free prologue GEMM on its own (operands packed into fp16x3 images inside the call); img_out: optional fp16x3 image of
-   the output, [M, rup32(N)] 32-bit words (what the next GEMM would stream), C may then be NULL */
+   the output, [M, rup32(N)] 32-bit words (what the next GEMM would stream), C may then be NULL.  nh > 0: the region encoder's Q|K|V
+   projection (N = 3 * nh * hs, M a multiple of R, no bias / activation, img_out NULL): Q to C columns [0, nh * hs), K to the per-head
+   image k_img [M, nh, rup32(hs)] words, V to the V^T image vt_img [M / R, nh * hs, rup32(R)] words; qkv_ref != 0 builds the same images
+   from the fp32 product (all N columns of C) with the separate pack passes.  nh == 0: k_img, vt_img and qkv_ref are ignored */
 GVD_API int gvd_op_linear_f16ss(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias, float* C, int64_t ldc,
-                  float* img_out, int M, int N, int K, int act, void* stream);
+                  float* img_out, int M, int N, int K, int act, int nh, int hs, int R, float* k_img, float* vt_img, int qkv_ref,
+                  void* stream);
 /* one LSTMCell step (AttModel.py:139,160) from up to two dense input segments; backend 0 = CUDA cores, 1 = wgmma */
 GVD_API int gvd_op_lstm_step(int B, int H, const float* x0, int K0, const float* w0, int64_t ldw0, const float* x1, int K1,
                   const float* w1, int64_t ldw1, const float* bias1, const float* bias2, const float* c_prev,
