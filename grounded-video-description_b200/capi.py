@@ -14,13 +14,13 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgvd_b200.so")
 
 EXPORTS = [
-    "gvd_last_error", "gvd_version", "gvd_model_create", "gvd_model_destroy", "gvd_model_set_param",
+    "gvd_last_error", "gvd_version", "gvd_model_create", "gvd_model_create_mode", "gvd_model_destroy", "gvd_model_set_param",
     "gvd_model_num_params", "gvd_model_param_key", "gvd_model_finalize", "gvd_workspace_bytes",
     "gvd_workspace_tensor", "gvd_prologue_fwd", "gvd_decode_greedy", "gvd_decode_sample", "gvd_decode_step_fwd",
     "gvd_decode_reset_state", "gvd_sample_greedy_host", "gvd_op_linear", "gvd_op_tanh", "gvd_op_kernel_launches",
     "gvd_profile_enable", "gvd_profile_reset", "gvd_profile_count", "gvd_profile_entry",
     "gvd_op_linear_tc", "gvd_op_linear_f16ss", "gvd_op_skinny_partials", "gvd_op_reduce_lstm", "gvd_op_reduce_bias", "gvd_op_reduce_pick",
-    "gvd_op_reduce_sample", "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_attention", "gvd_op_beam_topk",
+    "gvd_op_reduce_sample", "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_attention", "gvd_op_attention_mode", "gvd_op_beam_topk",
     "gvd_op_row_argmax", "gvd_op_beam_search_scripted", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_self_attention_fused", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
     "gvd_tfm_workspace_bytes", "gvd_tfm_decode_greedy", "gvd_tfm_teacher_fwd",
     "gvd_grounding_extract", "gvd_grounding_eval", "gvd_plan_skinny_splits", "gvd_plan_h2d_chunks", "gvd_workspace_bytes_beam", "gvd_beam_decode", "gvd_workspace_bytes_teacher", "gvd_teacher_fwd",
@@ -55,6 +55,7 @@ def lib():
     L.gvd_last_error.restype = ctypes.c_char_p
     L.gvd_version.restype = ctypes.c_char_p
     L.gvd_model_create.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(vp)]
+    L.gvd_model_create_mode.argtypes = [ctypes.POINTER(Dims), ci, ctypes.POINTER(vp)]
     L.gvd_model_destroy.argtypes = [vp]
     L.gvd_model_destroy.restype = None
     L.gvd_model_set_param.argtypes = [vp, ctypes.c_char_p, vp, sz, vp]
@@ -100,6 +101,7 @@ def lib():
     L.gvd_op_gru_layer.argtypes = [ci, vp, vp, vp, vp, ci, ci, ci, vp, vp]
     L.gvd_op_attention.argtypes = [vp, vp, vp, vp, vp, vp, ci, vp, vp, vp, vp, vp, vp, vp, i64, vp, i64, vp, vp, vp, i64, vp, i64,
                                    ci, ci, ci, ci, ci, ci, ci, ci, vp]
+    L.gvd_op_attention_mode.argtypes = L.gvd_op_attention.argtypes[:-1] + [ci, vp, vp, vp, i64, vp]
     L.gvd_op_beam_topk.argtypes = [vp, i64, ci, ci, ci, vp, vp, vp]
     L.gvd_op_row_argmax.argtypes = [vp, i64, ci, ci, vp, vp]
     L.gvd_op_beam_search_scripted.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
@@ -159,6 +161,18 @@ def profile_read():
     return out
 
 
+# opt.att_input_mode of the top-down captioner -> GVD_ATT_INPUT_* (include/gvd_b200.h)
+ATT_INPUT_MODES = {"both": 0, "featmap": 1, "dual_region": 2}
+
+
+def att_input_mode_code(opt):
+    """The GVD_ATT_INPUT_* code of ``opt.att_input_mode`` for the top-down captioner (the transformer captioner's prologue and decode step
+    do not depend on it: 'both')."""
+    if getattr(opt, "att_model", "topdown") == "transformer":
+        return ATT_INPUT_MODES["both"]
+    return ATT_INPUT_MODES[getattr(opt, "att_input_mode", "both")]
+
+
 def dims_from_opt(opt):
     """Size fields misc/model.py:31-58 reads from ``opt``."""
     att_model = getattr(opt, "att_model", "topdown")
@@ -166,10 +180,9 @@ def dims_from_opt(opt):
         raise NotImplementedError("att_model=%r: 'topdown' and 'transformer' are on the accelerated path" % (att_model,))
     if att_model == "transformer" and getattr(opt, "att_input_mode", "both") not in ("both", "featmap", "region"):
         raise NotImplementedError("att_input_mode=%r" % (opt.att_input_mode,))          # model.py:571-576
-    for field, want in (("att_input_mode", "both"), ("t_attn_mode", "bigru"), ("transfer_mode", "cls"),
-                        ("region_attn_mode", "mix")):
-        if field == "att_input_mode" and att_model == "transformer":
-            continue                                   # selects the captioner's encoder outputs only; the prologue is the same
+    if att_model == "topdown" and getattr(opt, "att_input_mode", "both") not in ATT_INPUT_MODES:
+        raise NotImplementedError("att_input_mode=%r: the top-down captioner implements %s" % (opt.att_input_mode, sorted(ATT_INPUT_MODES)))
+    for field, want in (("t_attn_mode", "bigru"), ("transfer_mode", "cls"), ("region_attn_mode", "mix")):
         if getattr(opt, field, want) != want:
             raise NotImplementedError("%s=%r: only %r (the reference default, cfgs/anet_res101_vg_feat_10x100prop.yml) "
                                       "is implemented" % (field, getattr(opt, field), want))
@@ -189,11 +202,12 @@ class NativeModel:
     def __init__(self, opt):
         self._L = lib()
         self.dims = dims_from_opt(opt)
+        self.att_input_mode = att_input_mode_code(opt)
         self._h = ctypes.c_void_p()
         if not torch.cuda.is_available():
             raise GvdError("gvd_b200 has no CPU path: a CUDA device is required")
         self.device = torch.cuda.current_device()      # the weight arena and every workspace live on this device
-        check(self._L.gvd_model_create(ctypes.byref(self.dims), ctypes.byref(self._h)))
+        check(self._L.gvd_model_create_mode(ctypes.byref(self.dims), self.att_input_mode, ctypes.byref(self._h)))
         self._live = None                              # (B, T, beam, nbox) of the prologue whose outputs sit in the workspace
         self.R = self.dims.num_sampled_frm * self.dims.num_prop_per_frm
         self._ws = {}
@@ -626,22 +640,29 @@ def op_gru_layer(path, gi, Whh, bhh, sample_idx=None):
 
 
 def op_attention(p_pool, pool, p_conv, conv, w1, b1, w2, b2, att_mask, out_mask, z_out, partial, x_out, RC, TC, q=None, q_part=None,
-                 q_bias=None, ticket=None, x_pk=None, feat_div=1):
+                 q_bias=None, ticket=None, x_pk=None, feat_div=1, att_input_mode=None, gate_w=None, gate_b=None, gate_h=None):
     """The decode attention of B query rows through gvd_op_attention.  Features [B / feat_div, N, A | H]; q [B, 2A] or its split-K planes
     q_part [q_S, B, 2A] + q_bias [2A]; att_mask [B / feat_div, R+1]; out_mask [B / feat_div, R+1] or a [B / feat_div, R+1] column window
     of a wider mask (its row pitch is passed); z_out [B, R] and x_out [B, H] (x_pk [B, rup32(H)] int32 words) may be column windows of
-    wider buffers; partial [B, nch, H+4]; ticket [B] int32 (None: the separate combine kernel)."""
+    wider buffers; partial [B, nch, H+4]; ticket [B] int32 (None: the separate combine kernel).  att_input_mode 'both' / 'featmap'
+    (None: gvd_op_attention, i.e. 'both'); with 'featmap' x_out = att and `pool` may be None.  'dual_region': q = [attention2_dual query |
+    attention2 query], w1 / b1 the dual alpha_net, p_conv / conv may be None, partial [B, 2 nch_r, H+4], the gate gate_w [H], gate_b [1] over
+    the rows of gate_h [B, H] (dense rows, any pitch)."""
     Bf, R, A = p_pool.shape
-    T, H = conv.shape[1], conv.shape[2]
+    T, H = (conv.shape[1], conv.shape[2]) if conv is not None else (1, x_out.shape[-1])
     B = (q if q is not None else q_part[0]).shape[0]
     q_S = q_part.shape[0] if q_part is not None else 0
     if out_mask.stride(1) != 1 or att_mask.stride(1) != 1 or att_mask.stride(0) != R + 1:
         raise GvdError("masks must have dense rows, att_mask a pitch of R+1")
-    check(lib().gvd_op_attention(
-        _dev(p_pool, torch.float32, "p_pool"), _dev(pool, torch.float32, "pool"), _dev(p_conv, torch.float32, "p_conv"),
-        _dev(conv, torch.float32, "conv"), _ptr(q), _ptr(q_part), q_S, _ptr(q_bias), _ptr(w1), _ptr(b1), _ptr(w2), _ptr(b2), _ptr(att_mask),
-        _ptr(out_mask), out_mask.stride(0), _ptr(z_out), _pitch(z_out), _ptr(partial), _ptr(ticket), _ptr(x_out), _pitch(x_out), _ptr(x_pk),
-        _pitch(x_pk), B, R, T, A, H, int(RC), int(TC), int(feat_div), _stream()))
+    args = (_dev(p_pool, torch.float32, "p_pool"), _dev(pool, torch.float32, "pool") if pool is not None else None,
+            _dev(p_conv, torch.float32, "p_conv") if p_conv is not None else None, _dev(conv, torch.float32, "conv") if conv is not None else None, _ptr(q), _ptr(q_part), q_S, _ptr(q_bias), _ptr(w1), _ptr(b1),
+            _ptr(w2), _ptr(b2), _ptr(att_mask), _ptr(out_mask), out_mask.stride(0), _ptr(z_out), _pitch(z_out), _ptr(partial), _ptr(ticket),
+            _ptr(x_out), _pitch(x_out), _ptr(x_pk), _pitch(x_pk), B, R, T, A, H, int(RC), int(TC), int(feat_div))
+    if att_input_mode is None:
+        check(lib().gvd_op_attention(*args, _stream()))
+    else:
+        check(lib().gvd_op_attention_mode(*args, ATT_INPUT_MODES[att_input_mode], _ptr(gate_w), _ptr(gate_b), _ptr(gate_h), _pitch(gate_h),
+                                          _stream()))
 
 
 def op_beam_topk(logits, K):

@@ -186,6 +186,7 @@ struct LoopKey { int B, T, backend; void* ws; size_t ws_bytes; };   // what a ca
 
 struct gvd_model {
     gvd_dims_t d;
+    int att_mode = GVD_ATT_INPUT_BOTH;   // opt.att_input_mode (GVD_ATT_INPUT_*): what the language LSTM reads, AttModel.py:144-156
     int R, G, NC, FCX, FCXp, PIN, PINp, NCp, Vp, HS, HP, nheads, rgb, motion;
     std::vector<int> head_off, head_size;
     std::vector<Param> params;
@@ -235,7 +236,13 @@ static void add_param(gvd_model* m, const std::string& key, size_t numel) {
 }
 
 extern "C" GVD_API int gvd_model_create(const gvd_dims_t* dims, gvd_model_t** out) {
+    return gvd_model_create_mode(dims, GVD_ATT_INPUT_BOTH, out);
+}
+
+extern "C" GVD_API int gvd_model_create_mode(const gvd_dims_t* dims, int att_input_mode, gvd_model_t** out) {
     GVD_REQUIRE(dims && out, "model_create: null argument");
+    GVD_REQUIRE(att_input_mode == GVD_ATT_INPUT_BOTH || att_input_mode == GVD_ATT_INPUT_FEATMAP || att_input_mode == GVD_ATT_INPUT_DUAL_REGION,
+                "model_create: att_input_mode %d is not implemented (0 = 'both', 1 = 'featmap', 2 = 'dual_region')", att_input_mode);
     const gvd_dims_t& d = *dims;
     GVD_REQUIRE(d.rnn_size % 4 == 0 && d.rnn_size >= 8 && d.rnn_size <= 1024, "rnn_size must be a multiple of 4 in [8,1024] (got %d)",
                 d.rnn_size);
@@ -249,6 +256,7 @@ extern "C" GVD_API int gvd_model_create(const gvd_dims_t* dims, gvd_model_t** ou
     GVD_REQUIRE(d.unk_idx >= 0 && d.unk_idx < d.vocab_size, "unk_idx out of range");
     gvd_model* m = new gvd_model();
     m->d = d;
+    m->att_mode = att_input_mode;
     const int H = d.rnn_size, A = d.att_hid_size, E = d.input_encoding_size, V = d.vocab_size, D = d.detect_size;
     m->R = d.num_sampled_frm * d.num_prop_per_frm;
     GVD_REQUIRE(!d.obj_interact || m->R % 4 == 0, "obj_interact needs R %% 4 == 0 (R=%d)", m->R);
@@ -310,6 +318,11 @@ extern "C" GVD_API int gvd_model_create(const gvd_dims_t* dims, gvd_model_t** ou
     for (const char* a : {"attention", "attention2"}) {
         add_param(m, std::string("core.") + a + ".h2att.weight", (size_t)A * H); add_param(m, std::string("core.") + a + ".h2att.bias", A);
         add_param(m, std::string("core.") + a + ".alpha_net.weight", A); add_param(m, std::string("core.") + a + ".alpha_net.bias", 1);
+    }
+    if (att_input_mode == GVD_ATT_INPUT_DUAL_REGION) {   // AttModel.py:126-128
+        add_param(m, "core.attention2_dual.h2att.weight", (size_t)A * H); add_param(m, "core.attention2_dual.h2att.bias", A);
+        add_param(m, "core.attention2_dual.alpha_net.weight", A); add_param(m, "core.attention2_dual.alpha_net.bias", 1);
+        add_param(m, "core.dual_pointer.0.weight", H); add_param(m, "core.dual_pointer.0.bias", 1);
     }
     // present in the checkpoint but never used by the forward pass (AttModel.py:130-131, quirk Q10)
     add_param(m, "core.i2h_2.weight", (size_t)H * 2 * H); add_param(m, "core.i2h_2.bias", H);
@@ -421,9 +434,11 @@ extern "C" GVD_API int gvd_model_finalize(gvd_model_t* m, void* stream) {
         relu_copy_kernel<<<gvd_cdiv(n, 256), 256, 0, st>>>(m->P("vis_embed.0.weight"), m->vis_relu, n);
         GVD_CHECK_LAUNCH();
     }
-    GVD_CHECK_CUDA(cudaMemcpyAsync(m->h2att_w, m->P("core.attention.h2att.weight"), (size_t)A * H * 4, cudaMemcpyDeviceToDevice, st));
+    // the query GEMM's first slot: the temporal query, or in dual_region (no temporal attention) attention2_dual's
+    const std::string q0 = m->att_mode == GVD_ATT_INPUT_DUAL_REGION ? "core.attention2_dual" : "core.attention";
+    GVD_CHECK_CUDA(cudaMemcpyAsync(m->h2att_w, m->P(q0 + ".h2att.weight"), (size_t)A * H * 4, cudaMemcpyDeviceToDevice, st));
     GVD_CHECK_CUDA(cudaMemcpyAsync(m->h2att_w + (size_t)A * H, m->P("core.attention2.h2att.weight"), (size_t)A * H * 4, cudaMemcpyDeviceToDevice, st));
-    GVD_CHECK_CUDA(cudaMemcpyAsync(m->h2att_b, m->P("core.attention.h2att.bias"), A * 4, cudaMemcpyDeviceToDevice, st));
+    GVD_CHECK_CUDA(cudaMemcpyAsync(m->h2att_b, m->P(q0 + ".h2att.bias"), A * 4, cudaMemcpyDeviceToDevice, st));
     GVD_CHECK_CUDA(cudaMemcpyAsync(m->h2att_b + A, m->P("core.attention2.h2att.bias"), A * 4, cudaMemcpyDeviceToDevice, st));
     add2_kernel<<<gvd_cdiv(4 * H, 256), 256, 0, st>>>(m->P("core.att_lstm.bias_ih"), m->P("core.att_lstm.bias_hh"), m->att_bias_sum, 4 * H);
     GVD_CHECK_LAUNCH();
@@ -642,7 +657,7 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     w.h_lang = (float*)take(2 * BD * H * 4);
     w.c_lang = (float*)take(BD * H * 4);
     w.q = (float*)take(BD * 2 * A * 4);
-    w.partial = (float*)take(BD * (w.nch_r + w.nch_t) * (H + 4) * 4);
+    w.partial = (float*)take(BD * std::max(w.nch_r + w.nch_t, m->att_mode == GVD_ATT_INPUT_DUAL_REGION ? 2 * w.nch_r : 0) * (H + 4) * 4);
     w.x_lang = (float*)take(BD * H * 4);
     w.logits = (float*)take(BD * m->Vp * 4);
     w.it = (long long*)take(BD * 8);
@@ -995,8 +1010,8 @@ static int frame_stages(const gvd_model* m, const WS& w, int B, int T, const flo
     GVD_STAGE("clip.frame_mean", gvd_frame_mean(segs_feat, w.fc_mean, B, T, FC, st));
     GVD_STAGE("clip.vector", gvd_clip_vector(w.fc_mean, num, m->P("seg_info_embed.0.weight"), m->P("seg_info_embed.0.bias"), w.xcat, B, FC, 50, m->FCXp, st));
     GVD_STAGE("clip.fc_embed", gvd_linear(w.xcat, m->FCXp, m->fc_embed_w, m->FCXp, m->P("fc_embed.0.bias"), w.fc_feats, H, B, H, m->FCXp, GVD_ACT_RELU, st));
-    // P7 frame branch (model.py:556-565)
-    GVD_TRY(frame_branch_fwd(m, w, B, T, segs_feat, sample_idx, st));
+    // P7 frame branch (model.py:556-565); dual_region reads no frame features (model.py:393: dummies)
+    if (m->att_mode != GVD_ATT_INPUT_DUAL_REGION) GVD_TRY(frame_branch_fwd(m, w, B, T, segs_feat, sample_idx, st));
     // constant part of the attention-LSTM gates: W_ih[:, :H] fc_feats + b_ih + b_hh (fc_feats is the same at every step)
     GVD_STAGE("decode.pre_att", gvd_linear(w.fc_feats, H, m->P("core.att_lstm.weight_ih"), H + E, m->att_bias_sum, w.pre_att, 4 * H, B, 4 * H, H, GVD_ACT_NONE, st));
     return 0;
@@ -1182,16 +1197,20 @@ static int core_step(const gvd_model* m, const WS& w, int B, int T, int step, co
         a.p_pool = w.p_pool; a.pool = w.pool_feats; a.p_conv = w.p_conv; a.conv = w.conv; a.q = w.q;
         if (q_S) { a.q = nullptr; a.q_part = w.q_part; a.q_S = q_S; a.q_plane = (long long)B * 2 * A; a.q_bias = m->h2att_b; }
         a.w1 = m->P("core.attention.alpha_net.weight"); a.b1 = m->P("core.attention.alpha_net.bias");
+        if (m->att_mode == GVD_ATT_INPUT_DUAL_REGION) {
+            a.w1 = m->P("core.attention2_dual.alpha_net.weight"); a.b1 = m->P("core.attention2_dual.alpha_net.bias");
+            a.gate_w = m->P("core.dual_pointer.0.weight"); a.gate_b = m->P("core.dual_pointer.0.bias"); a.gate_h = h_att_nxt; a.gate_ld = H;
+        }
         a.w2 = m->P("core.attention2.alpha_net.weight"); a.b2 = m->P("core.attention2.alpha_net.bias");
         a.att_mask = att_mask; a.out_mask = out_mask; a.z_out = z_out; a.z_stride_b = z_stride_b;
         a.partial = w.partial; a.B = B; a.R = R; a.T = T; a.A = A; a.H = H; a.RC = w.RC; a.TC = w.TC; a.feat_div = div;
-        a.out_mask_stride = out_mask_stride;
+        a.out_mask_stride = out_mask_stride; a.mode = m->att_mode;
         a.ticket = w.ticket; a.x_out = w.x_lang;         // chunk partials are merged by the last CTA of each row (no combine launch)
         if (skinny) { a.x_out = w.xcat_lang; a.x_ld = 3 * H; }   // ... straight into the language LSTM's concatenated input
         if (sk16) { a.x_pk = w.xp_lang; a.x_pk_ld = 3 * H; }
         GVD_STAGE("decode.attn_partial", gvd_attn_partial(a, st));
     }
-    {   // language LSTM: input cat(att + att2, h_att) (AttModel.py:147-160)
+    {   // language LSTM: input cat(att + att2, h_att), featmap cat(att, h_att) (AttModel.py:144-160): x_lang as the attention kernel merged it
         LstmArgs a{};
         a.nseg = 3;
         a.seg[0] = LstmSeg{w.x_lang, H, nullptr, 0, m->P("core.lang_lstm.weight_ih"), 2 * H, H};
@@ -1852,13 +1871,18 @@ extern "C" GVD_API int gvd_op_gru_layer(int path, const float* gi, const float* 
 // The decode attention (attn_partial_kernel) with every AttnArgs field the decode step sets.  ticket != NULL: the last chunk CTA of each row
 // merges the partials (the decode step's fused path; the caller zeroes the tickets once); ticket == NULL: attn_combine_kernel merges them
 // after the partial launch, into x_out at pitch H.  Test hook.
-extern "C" GVD_API int gvd_op_attention(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
-                                        const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
-                                        const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
-                                        int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
-                                        int B, int R, int T, int A, int H, int RC, int TC, int feat_div, void* stream) {
-    GVD_REQUIRE(p_pool && pool && p_conv && conv && w1 && b1 && w2 && b2 && att_mask && out_mask && z_out && partial && x_out && B >= 1 &&
-                R >= 1 && T >= 1 && feat_div >= 1 && B % feat_div == 0, "op_attention: bad arguments");
+extern "C" GVD_API int gvd_op_attention_mode(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                                             const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
+                                             const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
+                                             int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
+                                             int B, int R, int T, int A, int H, int RC, int TC, int feat_div, int att_input_mode,
+                                             const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld, void* stream) {
+    GVD_REQUIRE(att_input_mode == GVD_ATT_INPUT_BOTH || att_input_mode == GVD_ATT_INPUT_FEATMAP || att_input_mode == GVD_ATT_INPUT_DUAL_REGION,
+                "op_attention: unknown att_input_mode %d", att_input_mode);
+    const bool dual = att_input_mode == GVD_ATT_INPUT_DUAL_REGION;
+    GVD_REQUIRE(p_pool && (pool || att_input_mode == GVD_ATT_INPUT_FEATMAP) && ((p_conv && conv) || dual) && w1 && b1 && w2 && b2 && att_mask &&
+                out_mask && z_out && partial && x_out && B >= 1 && R >= 1 && T >= 1 && feat_div >= 1 && B % feat_div == 0, "op_attention: bad arguments");
+    GVD_REQUIRE(!dual || (ticket && gate_w && gate_b && gate_h && gate_ld >= H), "op_attention: dual_region needs the tickets and the gate");
     GVD_REQUIRE(q ? !q_part : (q_part && q_bias && q_S >= 1), "op_attention: give either q or (q_part, q_S >= 1, q_bias)");
     GVD_REQUIRE(z_stride_b >= R && (out_mask_stride == 0 || out_mask_stride >= R + 1), "op_attention: bad z / out_mask pitch");
     GVD_REQUIRE(x_ld == 0 || (x_ld >= H && x_ld % 4 == 0), "op_attention: x_ld must be 0 or a multiple of 4 covering H");
@@ -1870,13 +1894,24 @@ extern "C" GVD_API int gvd_op_attention(const float* p_pool, const float* pool, 
     a.w1 = w1; a.b1 = b1; a.w2 = w2; a.b2 = b2;
     a.att_mask = att_mask; a.out_mask = out_mask; a.out_mask_stride = out_mask_stride; a.z_out = z_out; a.z_stride_b = z_stride_b;
     a.partial = partial; a.ticket = ticket; a.x_out = x_out; a.x_ld = x_ld; a.x_pk = x_pk; a.x_pk_ld = x_pk_ld;
-    a.B = B; a.R = R; a.T = T; a.A = A; a.H = H; a.RC = RC; a.TC = TC; a.feat_div = feat_div;
+    a.B = B; a.R = R; a.T = T; a.A = A; a.H = H; a.RC = RC; a.TC = TC; a.feat_div = feat_div; a.mode = att_input_mode;
+    a.gate_w = gate_w; a.gate_b = gate_b; a.gate_h = gate_h; a.gate_ld = gate_ld;
     cudaStream_t st = (cudaStream_t)stream;
     GVD_TRY(gvd_attn_partial(a, st));
     if (ticket) return 0;
     int nch_r, nch_t;
     gvd_attn_chunks(R, T, RC, TC, &nch_r, &nch_t);
-    return gvd_attn_combine(partial, x_out, B, H, nch_r, nch_t, st);
+    return gvd_attn_combine(partial, x_out, B, H, nch_r, nch_t, att_input_mode, st);
+}
+extern "C" GVD_API int gvd_op_attention(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                                        const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
+                                        const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
+                                        int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
+                                        int B, int R, int T, int A, int H, int RC, int TC, int feat_div, void* stream) {
+    GVD_REQUIRE(pool, "op_attention: bad arguments");
+    return gvd_op_attention_mode(p_pool, pool, p_conv, conv, q, q_part, q_S, q_bias, w1, b1, w2, b2, att_mask, out_mask, out_mask_stride, z_out,
+                                 z_stride_b, partial, ticket, x_out, x_ld, x_pk, x_pk_ld, B, R, T, A, H, RC, TC, feat_div, GVD_ATT_INPUT_BOTH,
+                                 nullptr, nullptr, nullptr, 0, stream);
 }
 // beam_topk / row_argmax on their own.  Test hooks.
 extern "C" GVD_API int gvd_op_beam_topk(const float* logits, int64_t ld, int rows, int V, int K, float* topv, int* topi, void* stream) {

@@ -10,8 +10,14 @@
 //                          warps do  w.tanh(p+q)  (warp-shuffle reduce), the chunk softmax
 //                          numerators and the weighted feature sum.  Every feature byte is read
 //                          from HBM exactly once per step.
+//                          att_input_mode 'featmap' (AttModel.py:145-146): the region chunks stop
+//                          after the scores, so the region features are not read at all.
+//                          'dual_region' (AttModel.py:153-156): both region attentions share one
+//                          pass over the region rows (two scores per p_pool row, two weighted
+//                          sums per pool row); the merging CTA applies the dual_pointer gate.
 //   attn_combine_kernel  : merges the chunk partials (flash-decoding style) into att + att2.
 //   greedy_pick_kernel   : log_softmax + top-2 + UNK rule (misc/model.py:590-594,615).
+#include "../../include/gvd_b200.h"
 #include "gvd_kernels.cuh"
 
 namespace {
@@ -148,6 +154,176 @@ constexpr int ATT_THREADS = (ATT_CWARPS + 1) * 32;
 
 __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(ATT_CWARPS * 32) : "memory"); }
 
+// att_input_mode 'dual_region', consumer warps of one region chunk: attention2 (query slot 1, w2 / b2) and attention2_dual (query slot 0,
+// w1 / b1) over the same stream of p_pool / pool rows and the same masks; the returned logits (z_out) are attention2's.  Shared memory
+// after the generic query area: q1[A] w1[A] q2[A] w2[A] z2[MAXC] e2[MAXC] ml2[4].
+__device__ __forceinline__ void attn_dual_consumer(const AttnArgs& a, int nch_r, int b, int fb, int c, int r0, int nrows, int n_pa, int n_pb,
+                                                int rows_pa, int rows_pb, unsigned char* smem, uint64_t* full, uint64_t* empty, float* z_s,
+                                                float* e_s, float* ml, float* qs) {
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int A = a.A, H = a.H;
+    float* ws = qs + A;
+    float* qd = ws + A;
+    float* wd = qd + A;
+    float* zd_s = wd + A;
+    float* ed_s = zd_s + ATT_MAXC;
+    float* mld = ed_s + ATT_MAXC;
+    for (int i = tid; i < 2 * A; i += ATT_CWARPS * 32) {
+        float v;
+        if (a.q) {
+            v = a.q[(long long)b * 2 * A + i];
+        } else {
+            v = __ldg(a.q_bias + i);
+            for (int s = 0; s < a.q_S; ++s) v += __ldcg(a.q_part + s * a.q_plane + (long long)b * 2 * A + i);
+        }
+        if (i < A) qd[i] = v; else qs[i - A] = v;
+    }
+    for (int i = tid; i < A; i += ATT_CWARPS * 32) { ws[i] = a.w2[i]; wd[i] = a.w1[i]; }
+    consumer_bar();
+    const float bias = __ldg(a.b2), bias_d = __ldg(a.b1);
+
+    // phase A: both score vectors from one read of each projected row
+    for (int i = 0; i < n_pa; ++i) {
+        const int s = i % ATT_NST;
+        const uint32_t ph = (uint32_t)(i / ATT_NST) & 1u;
+        mbar_wait(&full[s], ph);
+        const float* st = reinterpret_cast<const float*>(smem + (size_t)s * ATT_STAGE_BYTES);
+        const int row0 = i * rows_pa, nr = min(rows_pa, nrows - row0);
+        for (int rr = warp; rr < nr; rr += ATT_CWARPS) {
+            const float* pr = st + (long long)rr * A;
+            float sum = 0.f, sum_d = 0.f;
+            for (int a0 = lane * 4; a0 < A; a0 += 128) {
+                const float4 v = *reinterpret_cast<const float4*>(pr + a0);
+                const float4 qv = *reinterpret_cast<const float4*>(qs + a0), wv = *reinterpret_cast<const float4*>(ws + a0);
+                const float4 qv2 = *reinterpret_cast<const float4*>(qd + a0), wv2 = *reinterpret_cast<const float4*>(wd + a0);
+                sum = fmaf(wv.x, tanh_mufu(v.x + qv.x), sum);
+                sum = fmaf(wv.y, tanh_mufu(v.y + qv.y), sum);
+                sum = fmaf(wv.z, tanh_mufu(v.z + qv.z), sum);
+                sum = fmaf(wv.w, tanh_mufu(v.w + qv.w), sum);
+                sum_d = fmaf(wv2.x, tanh_mufu(v.x + qv2.x), sum_d);
+                sum_d = fmaf(wv2.y, tanh_mufu(v.y + qv2.y), sum_d);
+                sum_d = fmaf(wv2.z, tanh_mufu(v.z + qv2.z), sum_d);
+                sum_d = fmaf(wv2.w, tanh_mufu(v.w + qv2.w), sum_d);
+            }
+            sum = warp_sum(sum);
+            sum_d = warp_sum(sum_d);
+            if (lane == 0) {
+                float z = sum + bias, zd = sum_d + bias_d;
+                const int rl = row0 + rr;
+                const long long mi = (long long)fb * (a.R + 1) + 1 + r0 + rl;
+                const long long oi = a.out_mask_stride ? (long long)fb * a.out_mask_stride + 1 + r0 + rl : mi;
+                const bool am = a.att_mask[mi] != 0, om = a.out_mask[oi] != 0;
+                if (am) { z = GVD_MIN_VALUE; zd = GVD_MIN_VALUE; }                      // AttModel.py:99, both attentions
+                a.z_out[(long long)b * a.z_stride_b + r0 + rl] = (am || om) ? GVD_MIN_VALUE : z;
+                z_s[rl] = z;
+                zd_s[rl] = zd;
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
+    }
+    consumer_bar();
+    if (warp < 2) {
+        const float* zz = warp ? zd_s : z_s;
+        float* ee = warp ? ed_s : e_s;
+        float m = -INFINITY;
+        for (int r = lane; r < nrows; r += 32) m = fmaxf(m, zz[r]);
+        m = warp_max(m);
+        float l = 0.f;
+        for (int r = lane; r < nrows; r += 32) {
+            const float e = expf(zz[r] - m);
+            ee[r] = e;
+            l += e;
+        }
+        l = warp_sum(l);
+        if (lane == 0) { (warp ? mld : ml)[0] = m; (warp ? mld : ml)[1] = l; }
+    }
+    consumer_bar();
+
+    // phase B: both unnormalised weighted sums from one read of each feature row
+    const int h0 = tid * 4;
+    const bool active = h0 < H;
+    float4 acc = make_float4(0.f, 0.f, 0.f, 0.f), acc_d = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int j = 0; j < n_pb; ++j) {
+        const int i = n_pa + j, s = i % ATT_NST;
+        const uint32_t ph = (uint32_t)(i / ATT_NST) & 1u;
+        mbar_wait(&full[s], ph);
+        const float* st = reinterpret_cast<const float*>(smem + (size_t)s * ATT_STAGE_BYTES);
+        const int row0 = j * rows_pb, nr = min(rows_pb, nrows - row0);
+        if (active) {
+            for (int rr = 0; rr < nr; ++rr) {
+                const float e = e_s[row0 + rr], ed = ed_s[row0 + rr];
+                const float4 v = *reinterpret_cast<const float4*>(st + (long long)rr * H + h0);
+                acc.x = fmaf(e, v.x, acc.x); acc.y = fmaf(e, v.y, acc.y); acc.z = fmaf(e, v.z, acc.z); acc.w = fmaf(e, v.w, acc.w);
+                acc_d.x = fmaf(ed, v.x, acc_d.x); acc_d.y = fmaf(ed, v.y, acc_d.y); acc_d.z = fmaf(ed, v.z, acc_d.z); acc_d.w = fmaf(ed, v.w, acc_d.w);
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
+    }
+    const int nrec = 2 * nch_r;
+    float* out = a.partial + ((long long)b * nrec + c) * (H + 4);
+    float* out_d = a.partial + ((long long)b * nrec + nch_r + c) * (H + 4);
+    if (tid == 0) { out[0] = ml[0]; out[1] = ml[1]; out_d[0] = mld[0]; out_d[1] = mld[1]; }
+    if (active) {
+        *reinterpret_cast<float4*>(out + 4 + h0) = acc;
+        *reinterpret_cast<float4*>(out_d + 4 + h0) = acc_d;
+    }
+    // ---- fused merge by the last chunk CTA of the row (fixed chunk order), then the gate
+    __threadfence();
+    consumer_bar();
+    int* flag = reinterpret_cast<int*>(ml + 2);
+    if (tid == 0) *flag = (atomicAdd(a.ticket + b, 1) == nch_r - 1) ? 1 : 0;
+    consumer_bar();
+    if (*flag == 0) return;
+    __threadfence();
+    // g = sigmoid(dual_pointer(h_att)) (AttModel.py:155): per-thread partial dot, warp sums, the 8 warp sums added in warp order
+    float gd = 0.f;
+    if (active) {
+        const float4 hv = *reinterpret_cast<const float4*>(a.gate_h + (long long)b * a.gate_ld + h0);
+        const float4 wv = __ldg(reinterpret_cast<const float4*>(a.gate_w + h0));
+        gd = fmaf(wv.x, hv.x, gd); gd = fmaf(wv.y, hv.y, gd); gd = fmaf(wv.z, hv.z, gd); gd = fmaf(wv.w, hv.w, gd);
+    }
+    gd = warp_sum(gd);
+    if (lane == 0) zd_s[warp] = gd;
+    consumer_bar();
+    float glogit = __ldg(a.gate_b);
+    for (int wv = 0; wv < ATT_CWARPS; ++wv) glogit += zd_s[wv];
+    const float g = sigmoid_acc(glogit);
+    const float* base = a.partial + (long long)b * nrec * (H + 4);
+    if (active) {
+        float4 r[2];
+#pragma unroll
+        for (int part = 0; part < 2; ++part) {                 // attention2 chunks, then attention2_dual chunks
+            const int c0 = part * nch_r, c1 = c0 + nch_r;
+            float M = -INFINITY;
+            for (int cc = c0; cc < c1; ++cc) M = fmaxf(M, __ldcg(base + (long long)cc * (H + 4)));
+            float L = 0.f;
+            float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
+            for (int cc = c0; cc < c1; ++cc) {
+                const float* pc = base + (long long)cc * (H + 4);
+                const float sc = expf(__ldcg(pc) - M);
+                L = fmaf(__ldcg(pc + 1), sc, L);
+                const float4 v = __ldcg(reinterpret_cast<const float4*>(pc + 4 + h0));
+                s4.x = fmaf(v.x, sc, s4.x); s4.y = fmaf(v.y, sc, s4.y); s4.z = fmaf(v.z, sc, s4.z); s4.w = fmaf(v.w, sc, s4.w);
+            }
+            r[part] = make_float4(s4.x / L, s4.y / L, s4.z / L, s4.w / L);
+        }
+        const float h = 1.f - g;                               // dual_p * att2 + (1 - dual_p) * att2_dual (AttModel.py:156)
+        const float4 res = make_float4(g * r[0].x + h * r[1].x, g * r[0].y + h * r[1].y, g * r[0].z + h * r[1].z, g * r[0].w + h * r[1].w);
+        *reinterpret_cast<float4*>(a.x_out + (long long)b * (a.x_ld ? a.x_ld : H) + h0) = res;
+        if (a.x_pk) {
+            uint32_t hi0, lo0, hi1, lo1;
+            f16x3_split_pair(res.x, res.y, GVD_F16_SA, hi0, lo0);
+            f16x3_split_pair(res.z, res.w, GVD_F16_SA, hi1, lo1);
+            uint32_t* d = reinterpret_cast<uint32_t*>(a.x_pk) + (long long)b * a.x_pk_ld + f16x3_word(h0);
+            *reinterpret_cast<uint2*>(d) = make_uint2(hi0, hi1);
+            *reinterpret_cast<uint2*>(d + 16) = make_uint2(lo0, lo1);
+        }
+    }
+    if (tid == 0) a.ticket[b] = 0;
+}
+
 template <int AJ>   // AJ = A/128 when A is 128*{1..4}: queries/weights live in registers; 0 = generic (shared memory)
 __global__ void __launch_bounds__(ATT_THREADS) attn_partial_kernel(AttnArgs a, int nch_r, int nch_t) {
     extern __shared__ __align__(128) unsigned char smem[];
@@ -172,7 +348,9 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_partial_kernel(AttnArgs a, i
     const float* p_rows = (region ? a.p_pool : a.p_conv) + ((long long)fb * N + r0) * A;
     const float* f_rows = (region ? a.pool : a.conv) + ((long long)fb * N + r0) * H;
     const int rows_pa = ATT_STAGE_BYTES / (A * 4), rows_pb = ATT_STAGE_BYTES / (H * 4);
-    const int n_pa = (nrows + rows_pa - 1) / rows_pa, n_pb = (nrows + rows_pb - 1) / rows_pb;
+    const bool featmap = a.mode == GVD_ATT_INPUT_FEATMAP, dual = a.mode == GVD_ATT_INPUT_DUAL_REGION;
+    // featmap: a region chunk's weighted sum never reaches the language LSTM, so its feature rows are not streamed (phase B is empty)
+    const int n_pa = (nrows + rows_pa - 1) / rows_pa, n_pb = (featmap && region) ? 0 : (nrows + rows_pb - 1) / rows_pb;
 
     if (tid == 0) {
         for (int s = 0; s < ATT_NST; ++s) {
@@ -212,6 +390,10 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_partial_kernel(AttnArgs a, i
 
     // ---------------------------------------------------------------- consumers
     pdl_wait();                                       // queries come from the predecessor kernel
+    if (dual) {
+        attn_dual_consumer(a, nch_r, b, fb, c, r0, nrows, n_pa, n_pb, rows_pa, rows_pb, smem, full, empty, z_s, e_s, ml, qs);
+        return;
+    }
     const float* w = region ? a.w2 : a.w1;
     const float bias = region ? __ldg(a.b2) : __ldg(a.b1);
     float4 q4[AJ > 0 ? AJ : 1], w4[AJ > 0 ? AJ : 1];
@@ -326,7 +508,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_partial_kernel(AttnArgs a, i
     }
     float* out = a.partial + ((long long)b * nch + c) * (H + 4);
     if (tid == 0) { out[0] = ml[0]; out[1] = ml[1]; }
-    if (active) *reinterpret_cast<float4*>(out + 4 + h0) = acc;
+    if (active && n_pb > 0) *reinterpret_cast<float4*>(out + 4 + h0) = acc;     // (featmap region chunks: no weighted sum to store)
     if (a.ticket == nullptr) return;
     // ---- fused combine: the last CTA of this row to finish merges all chunk partials (flash-decoding style).
     // Fixed merge order (chunk index), so the result does not depend on which CTA happens to be last.
@@ -342,6 +524,7 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_partial_kernel(AttnArgs a, i
         float4 res = make_float4(0.f, 0.f, 0.f, 0.f);
 #pragma unroll
         for (int part = 0; part < 2; ++part) {
+            if (part == 1 && featmap) break;                               // featmap: x = att
             const int c0 = part ? 0 : nch_r, c1 = part ? nch_r : nch;      // temporal chunks, then region chunks
             float M = -INFINITY;
             for (int cc = c0; cc < c1; ++cc) M = fmaxf(M, __ldcg(base + (long long)cc * (H + 4)));
@@ -369,15 +552,14 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_partial_kernel(AttnArgs a, i
     if (tid == 0) a.ticket[b] = 0;                       // ready for the next step
 }
 
-// merge chunk partials: att = sum_c acc_c e^{m_c - M} / sum_c l_c e^{m_c - M}; x = att(temporal) + att2(region)
+// merge chunk partials: att = sum_c acc_c e^{m_c - M} / sum_c l_c e^{m_c - M}; x = att(temporal) + att2(region) (featmap: att only)
 __global__ void __launch_bounds__(256) attn_combine_kernel(const float* __restrict__ partial, float* __restrict__ x_out, int H,
-                                                           int nch_r, int nch_t) {
+                                                           int nch_r, int nch_t, int nparts) {
     const int b = blockIdx.x, nch = nch_r + nch_t;
     const float* base = partial + (long long)b * nch * (H + 4);
     for (int h = threadIdx.x; h < H; h += blockDim.x) {
         float res = 0.f;
-#pragma unroll
-        for (int part = 0; part < 2; ++part) {
+        for (int part = 0; part < nparts; ++part) {
             const int c0 = part ? 0 : nch_r, c1 = part ? nch_r : nch;   // part 0: temporal chunks, part 1: region chunks
             float M = -INFINITY;
             for (int c = c0; c < c1; ++c) M = fmaxf(M, base[(long long)c * (H + 4)]);
@@ -475,19 +657,24 @@ int gvd_attn_chunks(int R, int T, int RC, int TC, int* nch_r, int* nch_t) {
     return 0;
 }
 
-static size_t attn_smem_bytes(int A) {
+static size_t attn_smem_bytes(int A, bool dual) {
     return (size_t)ATT_NST * ATT_STAGE_BYTES + (2 * ATT_MAXC + 4) * sizeof(float) + 2 * ATT_NST * sizeof(uint64_t) +
-           2 * (size_t)A * sizeof(float) + 16;
+           2 * (size_t)A * sizeof(float) + 16 + (dual ? (2 * (size_t)A + 2 * ATT_MAXC + 4) * sizeof(float) : 0);
 }
 
 int gvd_attn_partial(const AttnArgs& a, cudaStream_t st) {
+    GVD_REQUIRE(a.mode == GVD_ATT_INPUT_BOTH || a.mode == GVD_ATT_INPUT_FEATMAP || a.mode == GVD_ATT_INPUT_DUAL_REGION,
+                "attn: unknown att_input_mode %d", a.mode);
+    const bool dual = a.mode == GVD_ATT_INPUT_DUAL_REGION;
+    GVD_REQUIRE(!dual || (a.ticket && a.gate_w && a.gate_b && a.gate_h && a.gate_ld >= a.H), "attn: dual_region needs the fused merge and the gate");
     GVD_REQUIRE(a.A % 4 == 0 && a.H % 4 == 0, "attn: A and H must be multiples of 4");
     GVD_REQUIRE(a.A * 4 <= ATT_STAGE_BYTES && a.H * 4 <= ATT_STAGE_BYTES, "attn: row larger than a pipeline stage");
     GVD_REQUIRE(a.H <= ATT_CWARPS * 32 * 4, "attn: H=%d > %d not supported", a.H, ATT_CWARPS * 32 * 4);
     GVD_REQUIRE(a.RC >= 1 && a.RC <= ATT_MAXC && a.TC >= 1 && a.TC <= ATT_MAXC, "attn: chunk rows must be in [1,%d]", ATT_MAXC);
     int nch_r, nch_t;
     gvd_attn_chunks(a.R, a.T, a.RC, a.TC, &nch_r, &nch_t);
-    const size_t smem = attn_smem_bytes(a.A);
+    if (dual) nch_t = 0;                         // no temporal attention (AttModel.py:126-128: the frame features are dummies)
+    const size_t smem = attn_smem_bytes(a.A, dual);
     const unsigned grid = (unsigned)a.B * (unsigned)(nch_r + nch_t);
     const int aj = (a.A % 128 == 0 && a.A / 128 <= 4) ? a.A / 128 : 0;
 #define GVD_ATT_LAUNCH(AJ)                                                                                         \
@@ -508,8 +695,8 @@ int gvd_attn_partial(const AttnArgs& a, cudaStream_t st) {
     return 0;
 }
 
-int gvd_attn_combine(const float* partial, float* x_out, int B, int H, int nch_r, int nch_t, cudaStream_t st) {
-    attn_combine_kernel<<<B, 256, 0, st>>>(partial, x_out, H, nch_r, nch_t);
+int gvd_attn_combine(const float* partial, float* x_out, int B, int H, int nch_r, int nch_t, int mode, cudaStream_t st) {
+    attn_combine_kernel<<<B, 256, 0, st>>>(partial, x_out, H, nch_r, nch_t, mode == GVD_ATT_INPUT_FEATMAP ? 1 : 2);
     GVD_CHECK_LAUNCH();
     return 0;
 }

@@ -62,10 +62,18 @@ struct AttnArgs {
     int B, R, T, A, H;
     int RC, TC;                                 // rows per region / temporal chunk (<= 128)
     int feat_div;                               // rows sharing one clip's features/masks (beam rows); 0/1 = one per row
+    int mode;                                   // GVD_ATT_INPUT_* (include/gvd_b200.h): BOTH x = att + att2; FEATMAP x = att, the region
+                                                //   chunks compute their masked logits (z_out) only and never read `pool`; DUAL_REGION: no
+                                                //   temporal chunks, each region chunk scores its rows against both region queries (q = [dual
+                                                //   query | attention2 query], w1/b1 = attention2_dual.alpha_net) in ONE pass over p_pool / pool,
+                                                //   records [B, 2 * nch_r, H + 4] (attention2 chunks, then the dual ones); the merge writes
+                                                //   x = g att2 + (1 - g) att2_dual, g = sigmoid(gate_w . gate_h[b] + gate_b)
+    const float* gate_w; const float* gate_b;   // DUAL_REGION: core.dual_pointer.0  [H], [1]
+    const float* gate_h; long long gate_ld;     //   h_att rows (pitch gate_ld)
 };
 int gvd_attn_chunks(int R, int T, int RC, int TC, int* nch_r, int* nch_t);
 int gvd_attn_partial(const AttnArgs& a, cudaStream_t st);
-int gvd_attn_combine(const float* partial, float* x_out, int B, int H, int nch_r, int nch_t, cudaStream_t st);
+int gvd_attn_combine(const float* partial, float* x_out, int B, int H, int nch_r, int nch_t, int mode, cudaStream_t st);
 int gvd_greedy_pick(const float* logits, long long ld, int B, int V, int unk_idx, long long* it_out, long long* seq_out,
                     float* logp_out, long long out_stride, const float* embed, float* xt, int E, cudaStream_t st, long long ld_xt = 0);
 int gvd_tanh_test(const float* x, float* y, int n, cudaStream_t st);

@@ -28,6 +28,9 @@ class TopDownCore(nn.Module):
         self.lang_lstm = nn.LSTMCell(opt.rnn_size * 2, opt.rnn_size)
         self.attention = _AttentionParams(opt)
         self.attention2 = _AttentionParams(opt)
+        if opt.att_input_mode == "dual_region":                 # AttModel.py:126-128
+            self.attention2_dual = _AttentionParams(opt)
+            self.dual_pointer = nn.Sequential(nn.Linear(opt.rnn_size, 1), nn.Sigmoid())
         # present in every reference checkpoint, never used by forward (AttModel.py:130-131)
         self.i2h_2 = nn.Linear(opt.rnn_size * 2, opt.rnn_size)
         self.h2h_2 = nn.Linear(opt.rnn_size, opt.rnn_size)

@@ -63,7 +63,8 @@ class AttModel(CaptionModel):
         self._dims = capi.dims_from_opt(opt)      # raises NotImplementedError for modes off the hot path
         import types
         self.opt_ns = types.SimpleNamespace(rnn_size=opt.rnn_size, seq_length=opt.seq_length, vocab_size=opt.vocab_size,
-                                            num_sampled_frm=opt.num_sampled_frm, obj_interact=getattr(opt, "obj_interact", False))
+                                            num_sampled_frm=opt.num_sampled_frm, obj_interact=getattr(opt, "obj_interact", False),
+                                            att_input_mode=self.att_input_mode)
         self.vis_encoding_size = 2048
         self.pool_feat_size = self.att_feat_size + 300 + self.detect_size + 1
 
@@ -150,6 +151,7 @@ class AttModel(CaptionModel):
         o.num_sampled_frm, o.num_prop_per_frm = d.num_sampled_frm, d.num_prop_per_frm
         o.att_feat_size, o.fc_feat_size, o.obj_interact = d.att_feat_size, d.fc_feat_size, bool(d.obj_interact)
         o.wtoi = {"UNK": str(d.unk_idx)}
+        o.att_model, o.att_input_mode = self.att_model, self.att_input_mode     # the language LSTM's input (AttModel.py:144-156)
         return o
 
     @staticmethod
@@ -288,9 +290,10 @@ class AttModel(CaptionModel):
         named = [(k, p) for k, p in self.named_parameters()]
         W_extra = {k: v for k, v in self.state_dict(keep_vars=True).items() if "running_" in k}
         losses = mle_losses(self._train_step, self.opt_ns, inp, host, named, W_extra)
-        with torch.no_grad():
-            update_bn_running_stats(self._train_step, self.att_embed_aux[0].running_mean, self.att_embed_aux[0].running_var)
-            self.att_embed_aux[0].num_batches_tracked += 1
+        if self.att_input_mode != "dual_region":        # dual_region never runs att_embed_aux (model.py:393): its statistics stay
+            with torch.no_grad():
+                update_bn_running_stats(self._train_step, self.att_embed_aux[0].running_mean, self.att_embed_aux[0].running_var)
+                self.att_embed_aux[0].num_batches_tracked += 1
         return losses
 
     def _forward_tfm(self, segs_feat, gt_seq, ppls, num, ppls_feat, sample_idx, pnt_mask):

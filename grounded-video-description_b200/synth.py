@@ -125,6 +125,10 @@ def state_dict_spec(opt):
     for name in ("attention", "attention2"):
         lin("core.%s.h2att" % name, A, H)
         lin("core.%s.alpha_net" % name, 1, A)
+    if getattr(opt, "att_input_mode", "both") == "dual_region":        # AttModel.py:126-128, registered after attention2
+        lin("core.attention2_dual.h2att", A, H)
+        lin("core.attention2_dual.alpha_net", 1, A)
+        lin("core.dual_pointer.0", 1, H)
     lin("core.i2h_2", H, 2 * H)
     lin("core.h2h_2", H, H)
     return spec
@@ -134,6 +138,7 @@ def state_dict_spec(opt):
 # (default init gives 4-6 distinct tokens per batch, SURVEY.md section 7 "hard parts")
 _SCALE = {"logit.weight": 10.0, "logit.bias": 0.5, "embed.0.weight": 4.0,
           "core.attention.alpha_net.weight": 8.0, "core.attention2.alpha_net.weight": 8.0,
+          "core.attention2_dual.alpha_net.weight": 8.0, "core.dual_pointer.0.weight": 8.0,     # dual_region: the gate spans (0, 1) across clips
           "core.att_lstm.weight_ih": 3.0, "core.lang_lstm.weight_ih": 4.0, "core.lang_lstm.weight_hh": 0.5}
 # transformer captioner: sharp attention (so that the caption depends on the clip), a small tied embedding (so that the position, not the
 # previous token, dominates the residual stream: with the default init every caption is one token repeated)

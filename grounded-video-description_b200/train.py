@@ -115,24 +115,29 @@ class TrainStep:
         self._acc(grads, p + ".bias_hh", bsum)
         return ops.mm_nn(dgates, W[p + ".weight_ih"]), ops.mm_nn(dgates, W[p + ".weight_hh"]), dc
 
-    def _attn_fwd(self, p_feats, feats, q, w, b, mask):
+    def _attn_fwd(self, p_feats, feats, q, w, b, mask, need_out=True):
+        """need_out = False: the scores only (att_input_mode 'featmap' discards the region attention's weighted sum, AttModel.py:145-146)."""
         ops = self.ops
         s = ops.att_scores(p_feats, q, w, b)
         if mask is not None:
             s = ops.masked_fill(s, mask, MIN_VALUE)
         a = ops.softmax(s, 1.0)
-        out = ops.bmm_nn(a.unsqueeze(1), feats).squeeze(1)                 # [B,1,N] x [B,N,H]
+        out = ops.bmm_nn(a.unsqueeze(1), feats).squeeze(1) if need_out else None     # [B,1,N] x [B,N,H]
         return out, s, dict(a=a, mask=mask, q=q)
 
     def _attn_bwd(self, dout, ds_extra, tp, p_feats, feats, w, dfeats_acc):
-        """dfeats_acc [B,N,H] += a (x) dout in place (the gradient of the attended features, summed over the decode steps)."""
+        """dfeats_acc [B,N,H] += a (x) dout in place (the gradient of the attended features, summed over the decode steps).
+        dout = None: the weighted sum reached no loss, only the scores did (ds_extra)."""
         ops = self.ops
         a = tp["a"]
-        ops.outer_rows_acc_(dfeats_acc, a, dout)
-        da = ops.bmm_nt(dout.unsqueeze(1), feats).squeeze(1)               # [B,1,H] x [B,N,H]^T -> [B,1,N]
-        ds = ops.softmax_bwd(da, a, 1.0)
-        if ds_extra is not None:
-            ds = ops.add(ds, ds_extra)
+        if dout is None:
+            ds = ds_extra
+        else:
+            ops.outer_rows_acc_(dfeats_acc, a, dout)
+            da = ops.bmm_nt(dout.unsqueeze(1), feats).squeeze(1)           # [B,1,H] x [B,N,H]^T -> [B,1,N]
+            ds = ops.softmax_bwd(da, a, 1.0)
+            if ds_extra is not None:
+                ds = ops.add(ds, ds_extra)
         if tp["mask"] is not None:
             ds = ops.masked_fill(ds, tp["mask"], 0.0)
         dpre, dq, dw, db = ops.att_scores_bwd(ds, p_feats, tp["q"], w)
@@ -305,9 +310,25 @@ class TrainStep:
             dseg_h = ops.relu_bwd(D_(ops.ln_bwd(dxcat[:, pt["fc"].shape[1]:].contiguous(), pt["ln_seg"], seg_h), "lm", "seg_info"), seg_h)
             self._lin_bwd(dseg_h, pt["seg_in"], W, "seg_info_embed.0", grads, need_dx=False)
 
-        if dpool_feats is None:
+        if dpool_feats is None and dsimT is None:
             return
-        pool_feats, g_pool, simT, loc, pmask = pt["pool_feats"], pt["g_pool"], pt["simT"], pt["loc"], pt["pmask"]
+        g_pool, simT, pmask = pt["g_pool"], pt["simT"], pt["pmask"]
+        if dpool_feats is not None:
+            dg_pool, dsimT = self._pool_bwd(pt, W, opt, grads, D_, dpool_feats, dp_pool, dg_pool, dsimT)
+        n_g = g_pool.shape[-1]
+        dsim_raw = ops.masked_fill(ops.softmax_bwd(dsimT, simT, 1.0), pmask.unsqueeze(-1).expand_as(simT), 0.0)      # B, R, C
+        dsr2, gp2 = dsim_raw.reshape(-1, dsim_raw.shape[-1]), g_pool.reshape(-1, n_g)
+        dg_sim = ops.mm_nn(dsr2, pt["Wc"]).reshape(tuple(g_pool.shape))
+        dg_pool = dg_sim if dg_pool is None else ops.add(dg_pool, dg_sim)
+        self._acc(grads, "vis_embed.0.weight", ops.relu_bwd(D_(ops.mm_tn(dsr2, gp2), "lm", "vis_cls"), W["vis_embed.0.weight"]))
+        self._acc(grads, "vis_classifiers_bias", ops.colsum(dsr2))
+        self._lin_bwd(ops.relu_bwd(D_(dg_pool, "lm", "fc7"), g_pool), pt["ppls_feat"], W, "ctx2pool_grd.0", grads, need_dx=False)
+
+    def _pool_bwd(self, pt, W, opt, grads, D_, dpool_feats, dp_pool, dg_pool, dsimT):
+        """Backward of the region features (ctx2pool, obj_interact, pool_embed, loc_fc) into the gradients of g_pool and of the similarity."""
+        ops = self.ops
+        H = opt.rnn_size
+        pool_feats, g_pool, simT, loc = pt["pool_feats"], pt["g_pool"], pt["simT"], pt["loc"]
         dpool = ops.add(dpool_feats, self._lin_bwd(dp_pool, pool_feats, W, "ctx2pool", grads)) if dp_pool is not None else dpool_feats
         if opt.obj_interact:
             sizes = head_chunks(H)
@@ -343,12 +364,7 @@ class TrainStep:
         self._lin_bwd(dloc, pt["loc_in"], W, "loc_fc.0", grads, need_dx=False)
         dsim_ln = ops.ln_bwd(dpool_in[..., n_g + n_l:].contiguous(), pt["ln_sim"], simT)
         dsimT = dsim_ln if dsimT is None else ops.add(dsimT, dsim_ln)
-        dsim_raw = ops.masked_fill(ops.softmax_bwd(dsimT, simT, 1.0), pmask.unsqueeze(-1).expand_as(simT), 0.0)      # B, R, C
-        dsr2, gp2 = dsim_raw.reshape(-1, dsim_raw.shape[-1]), g_pool.reshape(-1, n_g)
-        dg_pool = ops.add(dg_pool, ops.mm_nn(dsr2, pt["Wc"]).reshape(tuple(g_pool.shape)))
-        self._acc(grads, "vis_embed.0.weight", ops.relu_bwd(D_(ops.mm_tn(dsr2, gp2), "lm", "vis_cls"), W["vis_embed.0.weight"]))
-        self._acc(grads, "vis_classifiers_bias", ops.colsum(dsr2))
-        self._lin_bwd(ops.relu_bwd(D_(dg_pool, "lm", "fc7"), g_pool), pt["ppls_feat"], W, "ctx2pool_grd.0", grads, need_dx=False)
+        return dg_pool, dsimT
 
     # ------------------------------------------------------------------ the step
     def forward(self, W, opt, inp, host=None):
@@ -383,7 +399,10 @@ class TrainStep:
         txt_mask_d = ops.to_device(txt_mask_h)
         cls_idx = ops.to_device(cls_idx_h.reshape(-1).contiguous())
 
-        pt = self._prologue_fwd(W, opt, inp, pmask, keep_d, D_)
+        mode = getattr(opt, "att_input_mode", "both")
+        featmap = mode == "featmap"                     # language LSTM input cat(att, h_att) (AttModel.py:145-146)
+        dual = mode == "dual_region"                    # cat(g att2 + (1 - g) att2_dual, h_att), no frame branch (AttModel.py:153-156, model.py:393)
+        pt = self._prologue_fwd(W, opt, inp, pmask, keep_d, D_, frames=not dual)
         fc_feats, g_pool, simT, pool_feats, p_pool, conv, p_conv = (pt[k] for k in ("fc_feats", "g_pool", "simT", "pool_feats", "p_pool", "conv",
                                                                                       "p_conv"))
 
@@ -391,6 +410,8 @@ class TrainStep:
         tgt = ops.host_targets(self, opt, inp, host)                                     # overlaps, class targets, per-step labels / masks
         a1w, a1b = W["core.attention.alpha_net.weight"], W["core.attention.alpha_net.bias"]
         a2w, a2b = W["core.attention2.alpha_net.weight"], W["core.attention2.alpha_net.bias"]
+        if dual:
+            adw, adb = W["core.attention2_dual.alpha_net.weight"], W["core.attention2_dual.alpha_net.bias"]
         h_att = c_att = h_lang = c_lang = ops.zeros((B, H))
         steps, outs, z_list = [], [], []
         for i in range(S):                                                               # S: the reference's early exit (model.py:425)
@@ -399,15 +420,31 @@ class TrainStep:
             xt = D_(ops.relu(emb_raw), "lm", "embed", i)
             x_att = ops.cat((fc_feats, xt), 1)
             h_att2, c_att2, t_att = self._lstm_fwd(x_att, h_att, c_att, W, "core.att_lstm")
-            q1 = ops.lin(h_att2, W["core.attention.h2att.weight"], W["core.attention.h2att.bias"], False)
-            att, _, t_a1 = self._attn_fwd(p_conv, conv, q1, a1w, a1b, None)
+            if not dual:
+                q1 = ops.lin(h_att2, W["core.attention.h2att.weight"], W["core.attention.h2att.bias"], False)
+                att, _, t_a1 = self._attn_fwd(p_conv, conv, q1, a1w, a1b, None)
             q2 = ops.lin(h_att2, W["core.attention2.h2att.weight"], W["core.attention2.h2att.bias"], False)
-            att2, z, t_a2 = self._attn_fwd(p_pool, pool_feats, q2, a2w, a2b, pmask)
+            att2, z, t_a2 = self._attn_fwd(p_pool, pool_feats, q2, a2w, a2b, pmask, need_out=not featmap)
             fmask = tgt["fm"][i]                                                         # B, R (bool): frame mask | proposal mask
             z_out = ops.masked_fill(z, fmask, MIN_VALUE)
-            x_lang = ops.cat((ops.add(att, att2), h_att2), 1)
+            st = dict(tok=tok, emb_raw=emb_raw, t_att=t_att, t_a2=t_a2, h_att2=h_att2, fmask=fmask)
+            if dual:
+                qd = ops.lin(h_att2, W["core.attention2_dual.h2att.weight"], W["core.attention2_dual.h2att.bias"], False)
+                att2d, _, t_ad = self._attn_fwd(p_pool, pool_feats, qd, adw, adb, pmask)
+                # g = sigmoid(dual_pointer(h_att)) as column 0 of softmax([logit, 0]); column 1 is 1 - g
+                # (the single-output Linear as a row dot product: no GEMM with one output column)
+                wpE = W["core.dual_pointer.0.weight"].expand(B, H).contiguous()
+                glog = ops.add(ops.rowsum(ops.mul(h_att2, wpE)).reshape(B, 1), W["core.dual_pointer.0.bias"].reshape(1, 1).expand(B, 1).contiguous())
+                gp = ops.softmax(ops.cat((glog, ops.zeros((B, 1))), 1), 1.0)
+                gE, hE = (gp[:, k:k + 1].expand(B, H).contiguous() for k in (0, 1))
+                x_lang = ops.cat((ops.add(ops.mul(gE, att2), ops.mul(hE, att2d)), h_att2), 1)
+                st.update(t_ad=t_ad, att2=att2, att2d=att2d, gp=gp, gE=gE, hE=hE, wpE=wpE)
+            else:
+                x_lang = ops.cat((att if featmap else ops.add(att, att2), h_att2), 1)
+                st.update(t_a1=t_a1)
             h_lang2, c_lang2, t_lang = self._lstm_fwd(x_lang, h_lang, c_lang, W, "core.lang_lstm")
-            steps.append(dict(tok=tok, emb_raw=emb_raw, t_att=t_att, t_a1=t_a1, t_a2=t_a2, t_lang=t_lang, h_att2=h_att2, fmask=fmask))
+            st.update(t_lang=t_lang)
+            steps.append(st)
             outs.append(D_(h_lang2, "lm", "lang_out", i))                                  # AttModel.py:161: the state keeps the un-dropped h
             z_list.append(z_out)
             h_att, c_att, h_lang, c_lang = h_att2, c_att2, h_lang2, c_lang2
@@ -429,6 +466,9 @@ class TrainStep:
             """Explicit backward of  w_lm lm + w_att2 att2 + w_grd grd + w_cls cls  (weights = the upstream gradients of the four
             losses): one pass, linear in the weights.  Returns {parameter key: gradient}."""
             grads = {}
+            # featmap: the region attention reaches the loss through its logits only, so with w_att2 = w_grd = 0 the region branch gets no
+            # gradient at all (None in the reference: Adam skips it)
+            region_grad = not featmap or bool(w_att2) or bool(w_grd)
             # ========================================================== backward, loss heads
             douts = self._lin_bwd(ops.scale(dlogits, w_lm), outs_t, W, "logit", grads)
             dz_all = ops.zeros(tuple(z_all.shape))
@@ -442,11 +482,11 @@ class TrainStep:
                 demb = ops.relu_bwd(D_(ops.bmm_nn(dgrd, g_pool), "lm", "vis_word"), emb_cls_raw)   # [B,S,R] [B,R,D] -> [B,S,D]
                 self._acc(grads, "vis_embed.0.weight", ops.index_add_rows(W["vis_embed.0.weight"].shape[0], cls_idx, demb.reshape(B * S, -1)))
                 self._acc(grads, "vis_classifiers_bias", ops.index_add_rows(W["vis_classifiers_bias"].shape[0], cls_idx, ops.rowsum(dgrd.reshape(B * S, -1)).reshape(-1, 1)).reshape(-1))
-            dsimT = ops.scale(dsimT_unit, w_cls) if w_cls else ops.zeros(tuple(simT.shape))
+            dsimT = ops.scale(dsimT_unit, w_cls) if w_cls else (ops.zeros(tuple(simT.shape)) if region_grad else None)
 
             # ========================================================== backward, BPTT over the decode steps
             dp_pool, dpool_feats = ops.zeros(tuple(p_pool.shape)), ops.zeros(tuple(pool_feats.shape))
-            dp_conv, dconv = ops.zeros(tuple(p_conv.shape)), ops.zeros(tuple(conv.shape))
+            dp_conv, dconv = (None, None) if dual else (ops.zeros(tuple(p_conv.shape)), ops.zeros(tuple(conv.shape)))
             dfc_feats = ops.zeros(tuple(fc_feats.shape))
             E = W["embed.0.weight"].shape[1]
             dembed = ops.zeros(tuple(W["embed.0.weight"].shape))
@@ -458,22 +498,43 @@ class TrainStep:
                                                                "core.lang_lstm", grads)
                 datt_sum = dx_lang[:, :H].contiguous()
                 dh_att = ops.add(dx_lang[:, H:].contiguous(), dh_att_n)
-                dz = ops.masked_fill(dz_all[:, i].contiguous(), st["fmask"], 0.0)
-                dpp, dq2, dw2, db2 = self._attn_bwd(datt_sum, dz, st["t_a2"], p_pool, pool_feats, a2w, dpool_feats)
-                dp_pool = ops.add(dp_pool, dpp)
-                self._acc(grads, "core.attention2.alpha_net.weight", dw2.reshape(1, -1))
-                self._acc(grads, "core.attention2.alpha_net.bias", db2.reshape(1))
-                dh_att = ops.add(dh_att, self._lin_bwd(dq2, st["h_att2"], W, "core.attention2.h2att", grads))
-                dpc, dq1, dw1, db1 = self._attn_bwd(datt_sum, None, st["t_a1"], p_conv, conv, a1w, dconv)
-                dp_conv = ops.add(dp_conv, dpc)
-                self._acc(grads, "core.attention.alpha_net.weight", dw1.reshape(1, -1))
-                self._acc(grads, "core.attention.alpha_net.bias", db1.reshape(1))
-                dh_att = ops.add(dh_att, self._lin_bwd(dq1, st["h_att2"], W, "core.attention.h2att", grads))
+                datt2 = datt_sum
+                if dual:
+                    # x = g att2 + (1 - g) att2_dual: d att2 = g dx, d att2_dual = (1 - g) dx, d logit = g (1 - g) sum_h dx (att2 - att2_dual)
+                    datt2 = ops.mul(st["gE"], datt_sum)
+                    dgd = ops.mul(st["hE"], datt_sum)
+                    dg = ops.rowsum(ops.mul(datt_sum, ops.add(st["att2"], ops.scale(st["att2d"], -1.0)))).reshape(B, 1)
+                    gp = st["gp"]
+                    dglog = ops.mul(dg, ops.mul(gp[:, 0:1].contiguous(), gp[:, 1:2].contiguous()))
+                    dglogE = dglog.expand(B, H).contiguous()
+                    self._acc(grads, "core.dual_pointer.0.weight", ops.colsum(ops.mul(dglogE, st["h_att2"])).reshape(1, H))
+                    self._acc(grads, "core.dual_pointer.0.bias", ops.sum_all(dglog))
+                    dh_att = ops.add(dh_att, ops.mul(dglogE, st["wpE"]))
+                    dpd, dqd, dwd, dbd = self._attn_bwd(dgd, None, st["t_ad"], p_pool, pool_feats, adw, dpool_feats)
+                    dp_pool = ops.add(dp_pool, dpd)
+                    self._acc(grads, "core.attention2_dual.alpha_net.weight", dwd.reshape(1, -1))
+                    self._acc(grads, "core.attention2_dual.alpha_net.bias", dbd.reshape(1))
+                    dh_att = ops.add(dh_att, self._lin_bwd(dqd, st["h_att2"], W, "core.attention2_dual.h2att", grads))
+                if region_grad:
+                    dz = ops.masked_fill(dz_all[:, i].contiguous(), st["fmask"], 0.0)
+                    dpp, dq2, dw2, db2 = self._attn_bwd(None if featmap else datt2, dz, st["t_a2"], p_pool, pool_feats, a2w, dpool_feats)
+                    dp_pool = ops.add(dp_pool, dpp)
+                    self._acc(grads, "core.attention2.alpha_net.weight", dw2.reshape(1, -1))
+                    self._acc(grads, "core.attention2.alpha_net.bias", db2.reshape(1))
+                    dh_att = ops.add(dh_att, self._lin_bwd(dq2, st["h_att2"], W, "core.attention2.h2att", grads))
+                if not dual:
+                    dpc, dq1, dw1, db1 = self._attn_bwd(datt_sum, None, st["t_a1"], p_conv, conv, a1w, dconv)
+                    dp_conv = ops.add(dp_conv, dpc)
+                    self._acc(grads, "core.attention.alpha_net.weight", dw1.reshape(1, -1))
+                    self._acc(grads, "core.attention.alpha_net.bias", db1.reshape(1))
+                    dh_att = ops.add(dh_att, self._lin_bwd(dq1, st["h_att2"], W, "core.attention.h2att", grads))
                 dx_att, dh_att_n, dc_att_n = self._lstm_bwd(dh_att, dc_att_n, st["t_att"], W, "core.att_lstm", grads)
                 dfc_feats = ops.add(dfc_feats, dx_att[:, :H].contiguous())
                 dembed = ops.add(dembed, ops.index_add_rows(dembed.shape[0], st["tok"], ops.relu_bwd(D_(dx_att[:, H:H + E].contiguous(), "lm", "embed", i), st["emb_raw"])))
             self._acc(grads, "embed.0.weight", dembed)
 
+            if not region_grad:
+                dpool_feats = dp_pool = dg_pool = None
             self._prologue_bwd(pt, W, opt, grads, D_, dconv=dconv, dp_conv=dp_conv, dfc_feats=dfc_feats, dpool_feats=dpool_feats, dp_pool=dp_pool,
                                dg_pool=dg_pool, dsimT=dsimT)
             return grads

@@ -50,7 +50,21 @@ GVD_API const char* gvd_last_error(void);
 GVD_API const char* gvd_version(void);
 
 /* ---- model / weights: replaces nn.Module construction + load_state_dict (main.py:616,638) */
-GVD_API int gvd_model_create(const gvd_dims_t* dims, gvd_model_t** out);
+GVD_API int gvd_model_create(const gvd_dims_t* dims, gvd_model_t** out);   /* att_input_mode 'both' */
+/* opt.att_input_mode of the top-down captioner (opts.py:58-59, AttModel.py:140-156): what the language LSTM reads next to h_att.
+ *   BOTH    (0) att + att2: temporal attention over the frame features plus region attention over the proposals;
+ *   FEATMAP (1) att only: the region attention still yields its masked logits (the returned att2 weights, the grounding and the
+ *               attention / grounding losses), but its weighted sum over the region features is never formed, so the decode step does
+ *               not read them.  Same parameters (state_dict) as BOTH.
+ *   DUAL_REGION (2) g att2 + (1 - g) att2_dual, g = sigmoid(dual_pointer(h_att)): two region attentions over the same features and
+ *               masks, read in one pass; the returned logits are the first one's.  No temporal attention: the prologue skips the frame
+ *               branch (att_embed, BatchNorm, bi-GRU, ctx2att).  The parameter list gains core.attention2_dual.{h2att,alpha_net}.* and
+ *               core.dual_pointer.0.* (after core.attention2.*, before core.i2h_2.*).
+ * 'region' is not implemented: gvd_model_create_mode rejects it. */
+#define GVD_ATT_INPUT_BOTH 0
+#define GVD_ATT_INPUT_FEATMAP 1
+#define GVD_ATT_INPUT_DUAL_REGION 2
+GVD_API int gvd_model_create_mode(const gvd_dims_t* dims, int att_input_mode, gvd_model_t** out);
 GVD_API void gvd_model_destroy(gvd_model_t* m);
 /* Copy one state_dict entry (by its reference key, e.g. "core.att_lstm.weight_ih") from a
  * DEVICE fp32 buffer of `numel` elements into the model's packed weight arena. */
@@ -250,6 +264,17 @@ GVD_API int gvd_op_attention(const float* p_pool, const float* pool, const float
                   int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2, const float* b2, const uint8_t* att_mask,
                   const uint8_t* out_mask, int64_t out_mask_stride, float* z_out, int64_t z_stride_b, float* partial, int* ticket, float* x_out,
                   int64_t x_ld, float* x_pk, int64_t x_pk_ld, int B, int R, int T, int A, int H, int RC, int TC, int feat_div, void* stream);
+/* gvd_op_attention_mode: the same with att_input_mode GVD_ATT_INPUT_* (gvd_op_attention = BOTH).  FEATMAP: x_out = att; the region
+ *   chunks write z_out and their (max, sum) words only (their weighted-sum words are not written), and `pool` may be NULL.
+ *   DUAL_REGION: q = [attention2_dual query | attention2 query], w1 / b1 = attention2_dual.alpha_net, w2 / b2 = attention2.alpha_net;
+ *   p_conv / conv unused (may be NULL); partial [B, 2 ceil(R/RC), H+4] (attention2 chunks, then attention2_dual chunks); ticket required;
+ *   x_out = g att2 + (1 - g) att2_dual with g = sigmoid(gate_w . gate_h[b * gate_ld ..] + gate_b[0]) (dual_pointer, [H] and [1]). */
+GVD_API int gvd_op_attention_mode(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                  const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2, const float* b2,
+                  const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out, int64_t z_stride_b, float* partial,
+                  int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld, int B, int R, int T, int A, int H, int RC, int TC,
+                  int feat_div, int att_input_mode, const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld,
+                  void* stream);
 /* beam_topk: per row of logits [rows, V] (pitch ld) the K <= 8 (K <= V) best words, value descending, ties to the lower index:
  *   topv [rows, K] = their log_softmax, topi [rows, K].  NaN words are skipped; a pick that finds only NaN left takes the lowest untaken
  *   index, so an all-NaN row gives 0 .. K-1 (as a stable torch.sort(descending=True) does).  Rows only partly NaN differ from torch,
