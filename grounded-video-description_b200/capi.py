@@ -14,18 +14,18 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgvd_b200.so")
 
 EXPORTS = [
-    "gvd_last_error", "gvd_version", "gvd_model_create", "gvd_model_create_mode", "gvd_model_destroy", "gvd_model_set_param",
+    "gvd_last_error", "gvd_version", "gvd_model_create", "gvd_model_create_mode", "gvd_model_create_modes", "gvd_model_destroy", "gvd_model_set_param",
     "gvd_model_num_params", "gvd_model_param_key", "gvd_model_finalize", "gvd_workspace_bytes",
     "gvd_workspace_tensor", "gvd_prologue_fwd", "gvd_decode_greedy", "gvd_decode_sample", "gvd_decode_step_fwd",
     "gvd_decode_reset_state", "gvd_sample_greedy_host", "gvd_op_linear", "gvd_op_tanh", "gvd_op_kernel_launches",
     "gvd_profile_enable", "gvd_profile_reset", "gvd_profile_count", "gvd_profile_entry",
     "gvd_op_linear_tc", "gvd_op_linear_f16ss", "gvd_op_skinny_partials", "gvd_op_reduce_lstm", "gvd_op_reduce_bias", "gvd_op_reduce_pick",
-    "gvd_op_reduce_sample", "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_attention", "gvd_op_attention_mode", "gvd_op_beam_topk",
+    "gvd_op_reduce_sample", "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_attention", "gvd_op_attention_mode", "gvd_op_attention_form", "gvd_op_beam_topk",
     "gvd_op_row_argmax", "gvd_op_beam_search_scripted", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_self_attention_fused", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
     "gvd_tfm_workspace_bytes", "gvd_tfm_decode_greedy", "gvd_tfm_teacher_fwd",
     "gvd_grounding_extract", "gvd_grounding_eval", "gvd_plan_skinny_splits", "gvd_plan_h2d_chunks", "gvd_workspace_bytes_beam", "gvd_beam_decode", "gvd_workspace_bytes_teacher", "gvd_teacher_fwd",
     # training-step primitives (csrc/gvd_train.cu; bound in train_ops.py)
-    "gvd_tr_adam_first_step", "gvd_tr_adam_flat", "gvd_tr_grad_norm", "gvd_tr_sumsq_scratch_bytes", "gvd_tr_att_scores_bwd", "gvd_tr_att_scores_fwd", "gvd_tr_bn_bwd", "gvd_tr_bn_normalize", "gvd_tr_cls_nll", "gvd_tr_colsum", "gvd_tr_count_inv", "gvd_tr_scalar_mul", "gvd_tr_dropout", "gvd_tr_ew", "gvd_tr_gather_rows", "gvd_tr_gemm_nt_batched", "gvd_tr_gru_cell_bwd", "gvd_tr_gru_cell_fwd", "gvd_tr_index_add_rows", "gvd_tr_lm_nll", "gvd_tr_ln_bwd", "gvd_tr_ln_fwd", "gvd_tr_ln_star_bwd", "gvd_tr_ln_star_fwd", "gvd_tr_lstm_cell_bwd", "gvd_tr_lstm_cell_fwd", "gvd_tr_mean_dim1", "gvd_tr_mha_bwd", "gvd_tr_mha_fwd", "gvd_tr_outer_rows", "gvd_tr_outer_rows_acc", "gvd_tr_pos_nll", "gvd_tr_rowsum", "gvd_tr_softmax_bwd", "gvd_tr_softmax_fwd", "gvd_tr_sum_all", "gvd_tr_targets", "gvd_tr_transpose",
+    "gvd_tr_adam_first_step", "gvd_tr_adam_flat", "gvd_tr_grad_norm", "gvd_tr_sumsq_scratch_bytes", "gvd_tr_att_scores_bwd", "gvd_tr_att_scores_fwd", "gvd_tr_att_scores_mul_bwd", "gvd_tr_att_scores_mul_fwd", "gvd_tr_bn_bwd", "gvd_tr_bn_normalize", "gvd_tr_cls_nll", "gvd_tr_colsum", "gvd_tr_count_inv", "gvd_tr_scalar_mul", "gvd_tr_dropout", "gvd_tr_ew", "gvd_tr_gather_rows", "gvd_tr_gemm_nt_batched", "gvd_tr_gru_cell_bwd", "gvd_tr_gru_cell_fwd", "gvd_tr_index_add_rows", "gvd_tr_lm_nll", "gvd_tr_ln_bwd", "gvd_tr_ln_fwd", "gvd_tr_ln_star_bwd", "gvd_tr_ln_star_fwd", "gvd_tr_lstm_cell_bwd", "gvd_tr_lstm_cell_fwd", "gvd_tr_mean_dim1", "gvd_tr_mha_bwd", "gvd_tr_mha_fwd", "gvd_tr_outer_rows", "gvd_tr_outer_rows_acc", "gvd_tr_pos_nll", "gvd_tr_rowsum", "gvd_tr_softmax_bwd", "gvd_tr_softmax_fwd", "gvd_tr_sum_all", "gvd_tr_targets", "gvd_tr_transpose",
 ]
 
 
@@ -56,6 +56,7 @@ def lib():
     L.gvd_version.restype = ctypes.c_char_p
     L.gvd_model_create.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(vp)]
     L.gvd_model_create_mode.argtypes = [ctypes.POINTER(Dims), ci, ctypes.POINTER(vp)]
+    L.gvd_model_create_modes.argtypes = [ctypes.POINTER(Dims), ci, ci, ctypes.POINTER(vp)]
     L.gvd_model_destroy.argtypes = [vp]
     L.gvd_model_destroy.restype = None
     L.gvd_model_set_param.argtypes = [vp, ctypes.c_char_p, vp, sz, vp]
@@ -102,6 +103,7 @@ def lib():
     L.gvd_op_attention.argtypes = [vp, vp, vp, vp, vp, vp, ci, vp, vp, vp, vp, vp, vp, vp, i64, vp, i64, vp, vp, vp, i64, vp, i64,
                                    ci, ci, ci, ci, ci, ci, ci, ci, vp]
     L.gvd_op_attention_mode.argtypes = L.gvd_op_attention.argtypes[:-1] + [ci, vp, vp, vp, i64, vp]
+    L.gvd_op_attention_form.argtypes = L.gvd_op_attention_mode.argtypes[:-1] + [ci, vp]
     L.gvd_op_beam_topk.argtypes = [vp, i64, ci, ci, ci, vp, vp, vp]
     L.gvd_op_row_argmax.argtypes = [vp, i64, ci, ci, vp, vp]
     L.gvd_op_beam_search_scripted.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
@@ -173,6 +175,25 @@ def att_input_mode_code(opt):
     return ATT_INPUT_MODES[getattr(opt, "att_input_mode", "both")]
 
 
+# opt.region_attn_mode -> GVD_REGION_ATTN_* (include/gvd_b200.h): the region attention's score, AttModel.py:79-96
+REGION_ATTN_MODES = {"mix": 0, "mix_mul": 1, "dp": 2}
+# the reference's other values cannot run there, so they are refused with the reason
+_REGION_ATTN_REFUSED = {
+    "add": "'add' builds a model-level alpha_net = Linear(att_hid_size, 1) that the grounding applies to 2048-wide vectors "
+           "(model.py:55-56,256-261): it fails unless att_hid_size == 2048",
+    "cat": "'cat': Attention2.forward reads an undefined `xt` (AttModel.py:87)",
+}
+
+
+def region_attn_mode_code(opt):
+    """The GVD_REGION_ATTN_* code of ``opt.region_attn_mode``.  The transformer captioner builds the same Attention2 parameters (its
+    state_dict follows the mode) but its decode never runs them."""
+    mode = getattr(opt, "region_attn_mode", "mix")
+    if mode not in REGION_ATTN_MODES:
+        raise NotImplementedError("region_attn_mode=%r: %s" % (mode, _REGION_ATTN_REFUSED.get(mode, "implemented: %s" % sorted(REGION_ATTN_MODES))))
+    return REGION_ATTN_MODES[mode]
+
+
 def dims_from_opt(opt):
     """Size fields misc/model.py:31-58 reads from ``opt``."""
     att_model = getattr(opt, "att_model", "topdown")
@@ -182,7 +203,8 @@ def dims_from_opt(opt):
         raise NotImplementedError("att_input_mode=%r" % (opt.att_input_mode,))          # model.py:571-576
     if att_model == "topdown" and getattr(opt, "att_input_mode", "both") not in ATT_INPUT_MODES:
         raise NotImplementedError("att_input_mode=%r: the top-down captioner implements %s" % (opt.att_input_mode, sorted(ATT_INPUT_MODES)))
-    for field, want in (("t_attn_mode", "bigru"), ("transfer_mode", "cls"), ("region_attn_mode", "mix")):
+    region_attn_mode_code(opt)
+    for field, want in (("t_attn_mode", "bigru"), ("transfer_mode", "cls")):
         if getattr(opt, field, want) != want:
             raise NotImplementedError("%s=%r: only %r (the reference default, cfgs/anet_res101_vg_feat_10x100prop.yml) "
                                       "is implemented" % (field, getattr(opt, field), want))
@@ -203,11 +225,12 @@ class NativeModel:
         self._L = lib()
         self.dims = dims_from_opt(opt)
         self.att_input_mode = att_input_mode_code(opt)
+        self.region_attn_mode = region_attn_mode_code(opt)
         self._h = ctypes.c_void_p()
         if not torch.cuda.is_available():
             raise GvdError("gvd_b200 has no CPU path: a CUDA device is required")
         self.device = torch.cuda.current_device()      # the weight arena and every workspace live on this device
-        check(self._L.gvd_model_create_mode(ctypes.byref(self.dims), self.att_input_mode, ctypes.byref(self._h)))
+        check(self._L.gvd_model_create_modes(ctypes.byref(self.dims), self.att_input_mode, self.region_attn_mode, ctypes.byref(self._h)))
         self._live = None                              # (B, T, beam, nbox) of the prologue whose outputs sit in the workspace
         self.R = self.dims.num_sampled_frm * self.dims.num_prop_per_frm
         self._ws = {}
@@ -640,14 +663,16 @@ def op_gru_layer(path, gi, Whh, bhh, sample_idx=None):
 
 
 def op_attention(p_pool, pool, p_conv, conv, w1, b1, w2, b2, att_mask, out_mask, z_out, partial, x_out, RC, TC, q=None, q_part=None,
-                 q_bias=None, ticket=None, x_pk=None, feat_div=1, att_input_mode=None, gate_w=None, gate_b=None, gate_h=None):
+                 q_bias=None, ticket=None, x_pk=None, feat_div=1, att_input_mode=None, gate_w=None, gate_b=None, gate_h=None,
+                 region_attn_mode=None):
     """The decode attention of B query rows through gvd_op_attention.  Features [B / feat_div, N, A | H]; q [B, 2A] or its split-K planes
     q_part [q_S, B, 2A] + q_bias [2A]; att_mask [B / feat_div, R+1]; out_mask [B / feat_div, R+1] or a [B / feat_div, R+1] column window
     of a wider mask (its row pitch is passed); z_out [B, R] and x_out [B, H] (x_pk [B, rup32(H)] int32 words) may be column windows of
     wider buffers; partial [B, nch, H+4]; ticket [B] int32 (None: the separate combine kernel).  att_input_mode 'both' / 'featmap'
     (None: gvd_op_attention, i.e. 'both'); with 'featmap' x_out = att and `pool` may be None.  'dual_region': q = [attention2_dual query |
     attention2 query], w1 / b1 the dual alpha_net, p_conv / conv may be None, partial [B, 2 nch_r, H+4], the gate gate_w [H], gate_b [1] over
-    the rows of gate_h [B, H] (dense rows, any pitch)."""
+    the rows of gate_h [B, H] (dense rows, any pitch).  region_attn_mode 'mix' / 'mix_mul' / 'dp' (None: 'mix' through gvd_op_attention(_mode));
+    in 'dp' the region alpha_net (w2 / b2, and w1 / b1 in 'dual_region') may be None."""
     Bf, R, A = p_pool.shape
     T, H = (conv.shape[1], conv.shape[2]) if conv is not None else (1, x_out.shape[-1])
     B = (q if q is not None else q_part[0]).shape[0]
@@ -658,7 +683,10 @@ def op_attention(p_pool, pool, p_conv, conv, w1, b1, w2, b2, att_mask, out_mask,
             _dev(p_conv, torch.float32, "p_conv") if p_conv is not None else None, _dev(conv, torch.float32, "conv") if conv is not None else None, _ptr(q), _ptr(q_part), q_S, _ptr(q_bias), _ptr(w1), _ptr(b1),
             _ptr(w2), _ptr(b2), _ptr(att_mask), _ptr(out_mask), out_mask.stride(0), _ptr(z_out), _pitch(z_out), _ptr(partial), _ptr(ticket),
             _ptr(x_out), _pitch(x_out), _ptr(x_pk), _pitch(x_pk), B, R, T, A, H, int(RC), int(TC), int(feat_div))
-    if att_input_mode is None:
+    if region_attn_mode is not None:
+        check(lib().gvd_op_attention_form(*args, ATT_INPUT_MODES[att_input_mode or "both"], _ptr(gate_w), _ptr(gate_b), _ptr(gate_h),
+                                          _pitch(gate_h), REGION_ATTN_MODES[region_attn_mode], _stream()))
+    elif att_input_mode is None:
         check(lib().gvd_op_attention(*args, _stream()))
     else:
         check(lib().gvd_op_attention_mode(*args, ATT_INPUT_MODES[att_input_mode], _ptr(gate_w), _ptr(gate_b), _ptr(gate_h), _pitch(gate_h),

@@ -187,6 +187,7 @@ struct LoopKey { int B, T, backend; void* ws; size_t ws_bytes; };   // what a ca
 struct gvd_model {
     gvd_dims_t d;
     int att_mode = GVD_ATT_INPUT_BOTH;   // opt.att_input_mode (GVD_ATT_INPUT_*): what the language LSTM reads, AttModel.py:144-156
+    int region_form = GVD_REGION_ATTN_MIX;   // opt.region_attn_mode (GVD_REGION_ATTN_*): the region attentions' score, AttModel.py:79-96
     int R, G, NC, FCX, FCXp, PIN, PINp, NCp, Vp, HS, HP, nheads, rgb, motion;
     std::vector<int> head_off, head_size;
     std::vector<Param> params;
@@ -240,7 +241,13 @@ extern "C" GVD_API int gvd_model_create(const gvd_dims_t* dims, gvd_model_t** ou
 }
 
 extern "C" GVD_API int gvd_model_create_mode(const gvd_dims_t* dims, int att_input_mode, gvd_model_t** out) {
+    return gvd_model_create_modes(dims, att_input_mode, GVD_REGION_ATTN_MIX, out);
+}
+
+extern "C" GVD_API int gvd_model_create_modes(const gvd_dims_t* dims, int att_input_mode, int region_attn_mode, gvd_model_t** out) {
     GVD_REQUIRE(dims && out, "model_create: null argument");
+    GVD_REQUIRE(region_attn_mode == GVD_REGION_ATTN_MIX || region_attn_mode == GVD_REGION_ATTN_MIX_MUL || region_attn_mode == GVD_REGION_ATTN_DP,
+                "model_create: region_attn_mode %d is not implemented (0 = 'mix', 1 = 'mix_mul', 2 = 'dp')", region_attn_mode);
     GVD_REQUIRE(att_input_mode == GVD_ATT_INPUT_BOTH || att_input_mode == GVD_ATT_INPUT_FEATMAP || att_input_mode == GVD_ATT_INPUT_DUAL_REGION,
                 "model_create: att_input_mode %d is not implemented (0 = 'both', 1 = 'featmap', 2 = 'dual_region')", att_input_mode);
     const gvd_dims_t& d = *dims;
@@ -257,6 +264,7 @@ extern "C" GVD_API int gvd_model_create_mode(const gvd_dims_t* dims, int att_inp
     gvd_model* m = new gvd_model();
     m->d = d;
     m->att_mode = att_input_mode;
+    m->region_form = region_attn_mode;
     const int H = d.rnn_size, A = d.att_hid_size, E = d.input_encoding_size, V = d.vocab_size, D = d.detect_size;
     m->R = d.num_sampled_frm * d.num_prop_per_frm;
     GVD_REQUIRE(!d.obj_interact || m->R % 4 == 0, "obj_interact needs R %% 4 == 0 (R=%d)", m->R);
@@ -315,13 +323,16 @@ extern "C" GVD_API int gvd_model_create_mode(const gvd_dims_t* dims, int att_inp
     add_param(m, "core.att_lstm.bias_ih", 4 * H); add_param(m, "core.att_lstm.bias_hh", 4 * H);
     add_param(m, "core.lang_lstm.weight_ih", (size_t)4 * H * 2 * H); add_param(m, "core.lang_lstm.weight_hh", (size_t)4 * H * H);
     add_param(m, "core.lang_lstm.bias_ih", 4 * H); add_param(m, "core.lang_lstm.bias_hh", 4 * H);
+    const bool region_alpha = region_attn_mode != GVD_REGION_ATTN_DP;   // 'dp' builds Attention2 without alpha_net (AttModel.py:62-65)
     for (const char* a : {"attention", "attention2"}) {
         add_param(m, std::string("core.") + a + ".h2att.weight", (size_t)A * H); add_param(m, std::string("core.") + a + ".h2att.bias", A);
-        add_param(m, std::string("core.") + a + ".alpha_net.weight", A); add_param(m, std::string("core.") + a + ".alpha_net.bias", 1);
+        if (std::string(a) == "attention" || region_alpha) {
+            add_param(m, std::string("core.") + a + ".alpha_net.weight", A); add_param(m, std::string("core.") + a + ".alpha_net.bias", 1);
+        }
     }
     if (att_input_mode == GVD_ATT_INPUT_DUAL_REGION) {   // AttModel.py:126-128
         add_param(m, "core.attention2_dual.h2att.weight", (size_t)A * H); add_param(m, "core.attention2_dual.h2att.bias", A);
-        add_param(m, "core.attention2_dual.alpha_net.weight", A); add_param(m, "core.attention2_dual.alpha_net.bias", 1);
+        if (region_alpha) { add_param(m, "core.attention2_dual.alpha_net.weight", A); add_param(m, "core.attention2_dual.alpha_net.bias", 1); }
         add_param(m, "core.dual_pointer.0.weight", H); add_param(m, "core.dual_pointer.0.bias", 1);
     }
     // present in the checkpoint but never used by the forward pass (AttModel.py:130-131, quirk Q10)
@@ -1204,7 +1215,7 @@ static int core_step(const gvd_model* m, const WS& w, int B, int T, int step, co
         a.w2 = m->P("core.attention2.alpha_net.weight"); a.b2 = m->P("core.attention2.alpha_net.bias");
         a.att_mask = att_mask; a.out_mask = out_mask; a.z_out = z_out; a.z_stride_b = z_stride_b;
         a.partial = w.partial; a.B = B; a.R = R; a.T = T; a.A = A; a.H = H; a.RC = w.RC; a.TC = w.TC; a.feat_div = div;
-        a.out_mask_stride = out_mask_stride; a.mode = m->att_mode;
+        a.out_mask_stride = out_mask_stride; a.mode = m->att_mode; a.form = m->region_form;   // (dp: P() of the absent alpha_net keys is NULL)
         a.ticket = w.ticket; a.x_out = w.x_lang;         // chunk partials are merged by the last CTA of each row (no combine launch)
         if (skinny) { a.x_out = w.xcat_lang; a.x_ld = 3 * H; }   // ... straight into the language LSTM's concatenated input
         if (sk16) { a.x_pk = w.xp_lang; a.x_pk_ld = 3 * H; }
@@ -1871,17 +1882,20 @@ extern "C" GVD_API int gvd_op_gru_layer(int path, const float* gi, const float* 
 // The decode attention (attn_partial_kernel) with every AttnArgs field the decode step sets.  ticket != NULL: the last chunk CTA of each row
 // merges the partials (the decode step's fused path; the caller zeroes the tickets once); ticket == NULL: attn_combine_kernel merges them
 // after the partial launch, into x_out at pitch H.  Test hook.
-extern "C" GVD_API int gvd_op_attention_mode(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+extern "C" GVD_API int gvd_op_attention_form(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
                                              const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
                                              const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
                                              int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
                                              int B, int R, int T, int A, int H, int RC, int TC, int feat_div, int att_input_mode,
-                                             const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld, void* stream) {
+                                             const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld, int region_attn_mode,
+                                             void* stream) {
     GVD_REQUIRE(att_input_mode == GVD_ATT_INPUT_BOTH || att_input_mode == GVD_ATT_INPUT_FEATMAP || att_input_mode == GVD_ATT_INPUT_DUAL_REGION,
                 "op_attention: unknown att_input_mode %d", att_input_mode);
-    const bool dual = att_input_mode == GVD_ATT_INPUT_DUAL_REGION;
-    GVD_REQUIRE(p_pool && (pool || att_input_mode == GVD_ATT_INPUT_FEATMAP) && ((p_conv && conv) || dual) && w1 && b1 && w2 && b2 && att_mask &&
-                out_mask && z_out && partial && x_out && B >= 1 && R >= 1 && T >= 1 && feat_div >= 1 && B % feat_div == 0, "op_attention: bad arguments");
+    GVD_REQUIRE(region_attn_mode == GVD_REGION_ATTN_MIX || region_attn_mode == GVD_REGION_ATTN_MIX_MUL || region_attn_mode == GVD_REGION_ATTN_DP,
+                "op_attention: unknown region_attn_mode %d", region_attn_mode);
+    const bool dual = att_input_mode == GVD_ATT_INPUT_DUAL_REGION, dp = region_attn_mode == GVD_REGION_ATTN_DP;
+    GVD_REQUIRE(p_pool && (pool || att_input_mode == GVD_ATT_INPUT_FEATMAP) && ((p_conv && conv) || dual) && ((w1 && b1) || (dual && dp)) &&
+                ((w2 && b2) || dp) && att_mask && out_mask && z_out && partial && x_out && B >= 1 && R >= 1 && T >= 1 && feat_div >= 1 && B % feat_div == 0, "op_attention: bad arguments");
     GVD_REQUIRE(!dual || (ticket && gate_w && gate_b && gate_h && gate_ld >= H), "op_attention: dual_region needs the tickets and the gate");
     GVD_REQUIRE(q ? !q_part : (q_part && q_bias && q_S >= 1), "op_attention: give either q or (q_part, q_S >= 1, q_bias)");
     GVD_REQUIRE(z_stride_b >= R && (out_mask_stride == 0 || out_mask_stride >= R + 1), "op_attention: bad z / out_mask pitch");
@@ -1895,13 +1909,25 @@ extern "C" GVD_API int gvd_op_attention_mode(const float* p_pool, const float* p
     a.att_mask = att_mask; a.out_mask = out_mask; a.out_mask_stride = out_mask_stride; a.z_out = z_out; a.z_stride_b = z_stride_b;
     a.partial = partial; a.ticket = ticket; a.x_out = x_out; a.x_ld = x_ld; a.x_pk = x_pk; a.x_pk_ld = x_pk_ld;
     a.B = B; a.R = R; a.T = T; a.A = A; a.H = H; a.RC = RC; a.TC = TC; a.feat_div = feat_div; a.mode = att_input_mode;
-    a.gate_w = gate_w; a.gate_b = gate_b; a.gate_h = gate_h; a.gate_ld = gate_ld;
+    a.gate_w = gate_w; a.gate_b = gate_b; a.gate_h = gate_h; a.gate_ld = gate_ld; a.form = region_attn_mode;
+    if (dp) { a.w2 = a.b2 = nullptr; if (dual) a.w1 = a.b1 = nullptr; }          // the kernel must not need them
     cudaStream_t st = (cudaStream_t)stream;
     GVD_TRY(gvd_attn_partial(a, st));
     if (ticket) return 0;
     int nch_r, nch_t;
     gvd_attn_chunks(R, T, RC, TC, &nch_r, &nch_t);
     return gvd_attn_combine(partial, x_out, B, H, nch_r, nch_t, att_input_mode, st);
+}
+extern "C" GVD_API int gvd_op_attention_mode(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                                             const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
+                                             const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
+                                             int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
+                                             int B, int R, int T, int A, int H, int RC, int TC, int feat_div, int att_input_mode,
+                                             const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld, void* stream) {
+    GVD_REQUIRE(w1 && b1 && w2 && b2, "op_attention: bad arguments");
+    return gvd_op_attention_form(p_pool, pool, p_conv, conv, q, q_part, q_S, q_bias, w1, b1, w2, b2, att_mask, out_mask, out_mask_stride, z_out,
+                                 z_stride_b, partial, ticket, x_out, x_ld, x_pk, x_pk_ld, B, R, T, A, H, RC, TC, feat_div, att_input_mode, gate_w,
+                                 gate_b, gate_h, gate_ld, GVD_REGION_ATTN_MIX, stream);
 }
 extern "C" GVD_API int gvd_op_attention(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
                                         const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,

@@ -15,6 +15,10 @@
 //                          'dual_region' (AttModel.py:153-156): both region attentions share one
 //                          pass over the region rows (two scores per p_pool row, two weighted
 //                          sums per pool row); the merging CTA applies the dual_pointer gate.
+//                          region_attn_mode (AttModel.py:79-96) is a template parameter of the
+//                          region chunks' score: ADD w.tanh(p+q)+b ('mix'), MUL w.tanh(p*q)+b
+//                          ('mix_mul') or DOT p.q ('dp': no alpha_net, w / b never read).  The
+//                          temporal chunks are additive in every mode.
 //   attn_combine_kernel  : merges the chunk partials (flash-decoding style) into att + att2.
 //   greedy_pick_kernel   : log_softmax + top-2 + UNK rule (misc/model.py:590-594,615).
 #include "../../include/gvd_b200.h"
@@ -154,9 +158,21 @@ constexpr int ATT_THREADS = (ATT_CWARPS + 1) * 32;
 
 __device__ __forceinline__ void consumer_bar() { asm volatile("bar.sync 1, %0;" ::"n"(ATT_CWARPS * 32) : "memory"); }
 
+template <int F> struct FormTag { static constexpr int value = F; };
+
+// one term of a row's score in form F (GVD_REGION_ATTN_*): acc + w tanh(p + q), acc + w tanh(p q), or acc + p q (w unused)
+template <int F>
+__device__ __forceinline__ float att_term(float w, float p, float q, float acc) {
+    if (F == GVD_REGION_ATTN_MIX) return fmaf(w, tanh_mufu(p + q), acc);
+    if (F == GVD_REGION_ATTN_MIX_MUL) return fmaf(w, tanh_mufu(p * q), acc);
+    return fmaf(p, q, acc);
+}
+
 // att_input_mode 'dual_region', consumer warps of one region chunk: attention2 (query slot 1, w2 / b2) and attention2_dual (query slot 0,
 // w1 / b1) over the same stream of p_pool / pool rows and the same masks; the returned logits (z_out) are attention2's.  Shared memory
-// after the generic query area: q1[A] w1[A] q2[A] w2[A] z2[MAXC] e2[MAXC] ml2[4].
+// after the generic query area: q1[A] w1[A] q2[A] w2[A] z2[MAXC] e2[MAXC] ml2[4].  Both attentions score in form F (DOT: w1 / w2 / b1 / b2
+// are not read).
+template <int F>
 __device__ __forceinline__ void attn_dual_consumer(const AttnArgs& a, int nch_r, int b, int fb, int c, int r0, int nrows, int n_pa, int n_pb,
                                                 int rows_pa, int rows_pb, unsigned char* smem, uint64_t* full, uint64_t* empty, float* z_s,
                                                 float* e_s, float* ml, float* qs) {
@@ -178,9 +194,10 @@ __device__ __forceinline__ void attn_dual_consumer(const AttnArgs& a, int nch_r,
         }
         if (i < A) qd[i] = v; else qs[i - A] = v;
     }
-    for (int i = tid; i < A; i += ATT_CWARPS * 32) { ws[i] = a.w2[i]; wd[i] = a.w1[i]; }
+    if (F != GVD_REGION_ATTN_DP)
+        for (int i = tid; i < A; i += ATT_CWARPS * 32) { ws[i] = a.w2[i]; wd[i] = a.w1[i]; }
     consumer_bar();
-    const float bias = __ldg(a.b2), bias_d = __ldg(a.b1);
+    const float bias = F == GVD_REGION_ATTN_DP ? 0.f : __ldg(a.b2), bias_d = F == GVD_REGION_ATTN_DP ? 0.f : __ldg(a.b1);
 
     // phase A: both score vectors from one read of each projected row
     for (int i = 0; i < n_pa; ++i) {
@@ -196,14 +213,14 @@ __device__ __forceinline__ void attn_dual_consumer(const AttnArgs& a, int nch_r,
                 const float4 v = *reinterpret_cast<const float4*>(pr + a0);
                 const float4 qv = *reinterpret_cast<const float4*>(qs + a0), wv = *reinterpret_cast<const float4*>(ws + a0);
                 const float4 qv2 = *reinterpret_cast<const float4*>(qd + a0), wv2 = *reinterpret_cast<const float4*>(wd + a0);
-                sum = fmaf(wv.x, tanh_mufu(v.x + qv.x), sum);
-                sum = fmaf(wv.y, tanh_mufu(v.y + qv.y), sum);
-                sum = fmaf(wv.z, tanh_mufu(v.z + qv.z), sum);
-                sum = fmaf(wv.w, tanh_mufu(v.w + qv.w), sum);
-                sum_d = fmaf(wv2.x, tanh_mufu(v.x + qv2.x), sum_d);
-                sum_d = fmaf(wv2.y, tanh_mufu(v.y + qv2.y), sum_d);
-                sum_d = fmaf(wv2.z, tanh_mufu(v.z + qv2.z), sum_d);
-                sum_d = fmaf(wv2.w, tanh_mufu(v.w + qv2.w), sum_d);
+                sum = att_term<F>(wv.x, v.x, qv.x, sum);
+                sum = att_term<F>(wv.y, v.y, qv.y, sum);
+                sum = att_term<F>(wv.z, v.z, qv.z, sum);
+                sum = att_term<F>(wv.w, v.w, qv.w, sum);
+                sum_d = att_term<F>(wv2.x, v.x, qv2.x, sum_d);
+                sum_d = att_term<F>(wv2.y, v.y, qv2.y, sum_d);
+                sum_d = att_term<F>(wv2.z, v.z, qv2.z, sum_d);
+                sum_d = att_term<F>(wv2.w, v.w, qv2.w, sum_d);
             }
             sum = warp_sum(sum);
             sum_d = warp_sum(sum_d);
@@ -324,8 +341,40 @@ __device__ __forceinline__ void attn_dual_consumer(const AttnArgs& a, int nch_r,
     if (tid == 0) a.ticket[b] = 0;
 }
 
-template <int AJ>   // AJ = A/128 when A is 128*{1..4}: queries/weights live in registers; 0 = generic (shared memory)
-__global__ void __launch_bounds__(ATT_THREADS) attn_partial_kernel(AttnArgs a, int nch_r, int nch_t) {
+// one warp's score sum of the projected row pr (before the warp reduction), form F
+template <int AJ, int F>
+__device__ __forceinline__ float att_row_sum(const float* pr, const float4* q4, const float4* w4, const float* qs, const float* ws, int A,
+                                             int lane) {
+    float sum = 0.f;
+    if (AJ > 0) {
+#pragma unroll
+        for (int j = 0; j < AJ; ++j) {
+            const float4 v = *reinterpret_cast<const float4*>(pr + lane * 4 + 128 * j);
+            sum = att_term<F>(w4[j].x, v.x, q4[j].x, sum);
+            sum = att_term<F>(w4[j].y, v.y, q4[j].y, sum);
+            sum = att_term<F>(w4[j].z, v.z, q4[j].z, sum);
+            sum = att_term<F>(w4[j].w, v.w, q4[j].w, sum);
+        }
+    } else {
+        for (int a0 = lane * 4; a0 < A; a0 += 128) {
+            const float4 v = *reinterpret_cast<const float4*>(pr + a0);
+            const float4 qv = *reinterpret_cast<const float4*>(qs + a0);
+            const float4 wv = F == GVD_REGION_ATTN_DP ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(ws + a0);
+            sum = att_term<F>(wv.x, v.x, qv.x, sum);
+            sum = att_term<F>(wv.y, v.y, qv.y, sum);
+            sum = att_term<F>(wv.z, v.z, qv.z, sum);
+            sum = att_term<F>(wv.w, v.w, qv.w, sum);
+        }
+    }
+    return sum;
+}
+
+// AJ = A/128 when A is 128*{1..4}: queries/weights live in registers; 0 = generic (shared memory).
+// FORM = GVD_REGION_ATTN_* of the region chunks (the temporal chunks are always additive).  The shared-memory ring allows 2 CTAs per SM; the
+// mul / dp instantiations say so (minBlocks 2, up to 113 registers), which keeps ptxas from spilling their second phase-A loop; mix keeps
+// the bounds it always had.
+template <int AJ, int FORM>
+__global__ void __launch_bounds__(ATT_THREADS, FORM == GVD_REGION_ATTN_MIX ? 0 : 2) attn_partial_kernel(AttnArgs a, int nch_r, int nch_t) {
     extern __shared__ __align__(128) unsigned char smem[];
     float* z_s = reinterpret_cast<float*>(smem + ATT_NST * ATT_STAGE_BYTES);
     float* e_s = z_s + ATT_MAXC;
@@ -391,11 +440,12 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_partial_kernel(AttnArgs a, i
     // ---------------------------------------------------------------- consumers
     pdl_wait();                                       // queries come from the predecessor kernel
     if (dual) {
-        attn_dual_consumer(a, nch_r, b, fb, c, r0, nrows, n_pa, n_pb, rows_pa, rows_pb, smem, full, empty, z_s, e_s, ml, qs);
+        attn_dual_consumer<FORM>(a, nch_r, b, fb, c, r0, nrows, n_pa, n_pb, rows_pa, rows_pb, smem, full, empty, z_s, e_s, ml, qs);
         return;
     }
     const float* w = region ? a.w2 : a.w1;
-    const float bias = region ? __ldg(a.b2) : __ldg(a.b1);
+    const bool has_w = !(FORM == GVD_REGION_ATTN_DP && region);      // dp: the region attention has no alpha_net (w2 / b2 are NULL)
+    const float bias = region ? (FORM == GVD_REGION_ATTN_DP ? 0.f : __ldg(a.b2)) : __ldg(a.b1);
     float4 q4[AJ > 0 ? AJ : 1], w4[AJ > 0 ? AJ : 1];
     const float* q = a.q ? a.q + (long long)b * 2 * A + (region ? A : 0) : qs;
     if (!a.q) {
@@ -412,61 +462,47 @@ __global__ void __launch_bounds__(ATT_THREADS) attn_partial_kernel(AttnArgs a, i
 #pragma unroll
         for (int j = 0; j < AJ; ++j) {
             q4[j] = *reinterpret_cast<const float4*>(q + lane * 4 + 128 * j);
-            w4[j] = __ldg(reinterpret_cast<const float4*>(w + lane * 4 + 128 * j));
+            w4[j] = has_w ? __ldg(reinterpret_cast<const float4*>(w + lane * 4 + 128 * j)) : make_float4(0.f, 0.f, 0.f, 0.f);
         }
     } else {
         if (a.q) { for (int i = tid; i < A; i += ATT_CWARPS * 32) qs[i] = q[i]; }
-        for (int i = tid; i < A; i += ATT_CWARPS * 32) ws[i] = w[i];
+        if (has_w) for (int i = tid; i < A; i += ATT_CWARPS * 32) ws[i] = w[i];
         consumer_bar();
     }
 
-    // phase A: scores  z_r = w . tanh(p_r + q) + bias
-    for (int i = 0; i < n_pa; ++i) {
-        const int s = i % ATT_NST;
-        const uint32_t ph = (uint32_t)(i / ATT_NST) & 1u;
-        mbar_wait(&full[s], ph);
-        const float* st = reinterpret_cast<const float*>(smem + (size_t)s * ATT_STAGE_BYTES);
-        const int row0 = i * rows_pa, nr = min(rows_pa, nrows - row0);
-        for (int rr = warp; rr < nr; rr += ATT_CWARPS) {
-            const float* pr = st + (long long)rr * A;
-            float sum = 0.f;
-            if (AJ > 0) {
-#pragma unroll
-                for (int j = 0; j < AJ; ++j) {
-                    const float4 v = *reinterpret_cast<const float4*>(pr + lane * 4 + 128 * j);
-                    sum = fmaf(w4[j].x, tanh_mufu(v.x + q4[j].x), sum);
-                    sum = fmaf(w4[j].y, tanh_mufu(v.y + q4[j].y), sum);
-                    sum = fmaf(w4[j].z, tanh_mufu(v.z + q4[j].z), sum);
-                    sum = fmaf(w4[j].w, tanh_mufu(v.w + q4[j].w), sum);
-                }
-            } else {
-                for (int a0 = lane * 4; a0 < A; a0 += 128) {
-                    const float4 v = *reinterpret_cast<const float4*>(pr + a0);
-                    const float4 qv = *reinterpret_cast<const float4*>(qs + a0);
-                    const float4 wv = *reinterpret_cast<const float4*>(ws + a0);
-                    sum = fmaf(wv.x, tanh_mufu(v.x + qv.x), sum);
-                    sum = fmaf(wv.y, tanh_mufu(v.y + qv.y), sum);
-                    sum = fmaf(wv.z, tanh_mufu(v.z + qv.z), sum);
-                    sum = fmaf(wv.w, tanh_mufu(v.w + qv.w), sum);
+    // phase A: scores  z_r = w . tanh(p_r + q) + bias  (region chunks: w . tanh(p_r * q) + bias or p_r . q in the other forms).  One loop
+    // per form a CTA can run: the form is uniform over the CTA, so no row pays for the other one
+    auto phase_a = [&](auto form) {
+        constexpr int F = decltype(form)::value;
+        for (int i = 0; i < n_pa; ++i) {
+            const int s = i % ATT_NST;
+            const uint32_t ph = (uint32_t)(i / ATT_NST) & 1u;
+            mbar_wait(&full[s], ph);
+            const float* st = reinterpret_cast<const float*>(smem + (size_t)s * ATT_STAGE_BYTES);
+            const int row0 = i * rows_pa, nr = min(rows_pa, nrows - row0);
+            for (int rr = warp; rr < nr; rr += ATT_CWARPS) {
+                const float* pr = st + (long long)rr * A;
+                float sum = att_row_sum<AJ, F>(pr, q4, w4, qs, ws, A, lane);
+                sum = warp_sum(sum);
+                if (lane == 0) {
+                    float z = sum + bias;
+                    const int rl = row0 + rr;
+                    if (region) {
+                        const long long mi = (long long)fb * (a.R + 1) + 1 + r0 + rl;
+                        const long long oi = a.out_mask_stride ? (long long)fb * a.out_mask_stride + 1 + r0 + rl : mi;
+                        const bool am = a.att_mask[mi] != 0, om = a.out_mask[oi] != 0;
+                        if (am) z = GVD_MIN_VALUE;                               // AttModel.py:99
+                        a.z_out[(long long)b * a.z_stride_b + r0 + rl] = (am || om) ? GVD_MIN_VALUE : z;   // AttModel.py:100,103
+                    }
+                    z_s[rl] = z;
                 }
             }
-            sum = warp_sum(sum);
-            if (lane == 0) {
-                float z = sum + bias;
-                const int rl = row0 + rr;
-                if (region) {
-                    const long long mi = (long long)fb * (a.R + 1) + 1 + r0 + rl;
-                    const long long oi = a.out_mask_stride ? (long long)fb * a.out_mask_stride + 1 + r0 + rl : mi;
-                    const bool am = a.att_mask[mi] != 0, om = a.out_mask[oi] != 0;
-                    if (am) z = GVD_MIN_VALUE;                               // AttModel.py:99
-                    a.z_out[(long long)b * a.z_stride_b + r0 + rl] = (am || om) ? GVD_MIN_VALUE : z;   // AttModel.py:100,103
-                }
-                z_s[rl] = z;
-            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);
         }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[s]);
-    }
+    };
+    if (FORM != GVD_REGION_ATTN_MIX && region) phase_a(FormTag<FORM>{});
+    else phase_a(FormTag<GVD_REGION_ATTN_MIX>{});
     consumer_bar();
     if (warp == 0) {
         float m = -INFINITY;
@@ -667,6 +703,10 @@ int gvd_attn_partial(const AttnArgs& a, cudaStream_t st) {
                 "attn: unknown att_input_mode %d", a.mode);
     const bool dual = a.mode == GVD_ATT_INPUT_DUAL_REGION;
     GVD_REQUIRE(!dual || (a.ticket && a.gate_w && a.gate_b && a.gate_h && a.gate_ld >= a.H), "attn: dual_region needs the fused merge and the gate");
+    GVD_REQUIRE(a.form == GVD_REGION_ATTN_MIX || a.form == GVD_REGION_ATTN_MIX_MUL || a.form == GVD_REGION_ATTN_DP,
+                "attn: unknown region_attn_mode %d", a.form);
+    const bool region_w = a.form != GVD_REGION_ATTN_DP;                // dp: no region alpha_net
+    GVD_REQUIRE((dual ? (!region_w || (a.w1 && a.b1)) : (a.w1 && a.b1)) && (!region_w || (a.w2 && a.b2)), "attn: missing alpha_net weights");
     GVD_REQUIRE(a.A % 4 == 0 && a.H % 4 == 0, "attn: A and H must be multiples of 4");
     GVD_REQUIRE(a.A * 4 <= ATT_STAGE_BYTES && a.H * 4 <= ATT_STAGE_BYTES, "attn: row larger than a pipeline stage");
     GVD_REQUIRE(a.H <= ATT_CWARPS * 32 * 4, "attn: H=%d > %d not supported", a.H, ATT_CWARPS * 32 * 4);
@@ -677,19 +717,26 @@ int gvd_attn_partial(const AttnArgs& a, cudaStream_t st) {
     const size_t smem = attn_smem_bytes(a.A, dual);
     const unsigned grid = (unsigned)a.B * (unsigned)(nch_r + nch_t);
     const int aj = (a.A % 128 == 0 && a.A / 128 <= 4) ? a.A / 128 : 0;
-#define GVD_ATT_LAUNCH(AJ)                                                                                         \
-    do {                                                                                                           \
-        GVD_CHECK_CUDA(cudaFuncSetAttribute(attn_partial_kernel<AJ>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                                            (int)smem));                                                           \
-        GVD_CHECK_CUDA(gvd_launch(attn_partial_kernel<AJ>, dim3(grid), dim3(ATT_THREADS), smem, st, a, nch_r, nch_t)); \
+#define GVD_ATT_LAUNCH(AJ, F)                                                                                         \
+    do {                                                                                                              \
+        GVD_CHECK_CUDA(cudaFuncSetAttribute(attn_partial_kernel<AJ, F>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
+                                            (int)smem));                                                              \
+        GVD_CHECK_CUDA(gvd_launch(attn_partial_kernel<AJ, F>, dim3(grid), dim3(ATT_THREADS), smem, st, a, nch_r, nch_t)); \
+    } while (0)
+#define GVD_ATT_FORMS(AJ)                                                                   \
+    do {                                                                                    \
+        if (a.form == GVD_REGION_ATTN_MIX_MUL) GVD_ATT_LAUNCH(AJ, GVD_REGION_ATTN_MIX_MUL); \
+        else if (a.form == GVD_REGION_ATTN_DP) GVD_ATT_LAUNCH(AJ, GVD_REGION_ATTN_DP);      \
+        else GVD_ATT_LAUNCH(AJ, GVD_REGION_ATTN_MIX);                                       \
     } while (0)
     switch (aj) {
-        case 1: GVD_ATT_LAUNCH(1); break;
-        case 2: GVD_ATT_LAUNCH(2); break;
-        case 3: GVD_ATT_LAUNCH(3); break;
-        case 4: GVD_ATT_LAUNCH(4); break;
-        default: GVD_ATT_LAUNCH(0); break;
+        case 1: GVD_ATT_FORMS(1); break;
+        case 2: GVD_ATT_FORMS(2); break;
+        case 3: GVD_ATT_FORMS(3); break;
+        case 4: GVD_ATT_FORMS(4); break;
+        default: GVD_ATT_FORMS(0); break;
     }
+#undef GVD_ATT_FORMS
 #undef GVD_ATT_LAUNCH
     GVD_CHECK_LAUNCH();
     return 0;

@@ -49,7 +49,7 @@ struct AttnArgs {
     const float* q;                             // [B, 2A] : temporal query | region query (h2att outputs)
     const float* q_part; int q_S; long long q_plane; const float* q_bias;   // or (q == nullptr) its split-K partials [S][B][2A] + bias: summed here
     const float* w1; const float* b1;           // core.attention.alpha_net   [A], [1]
-    const float* w2; const float* b2;           // core.attention2.alpha_net  [A], [1]
+    const float* w2; const float* b2;           // core.attention2.alpha_net  [A], [1] (NULL in region_attn_mode 'dp')
     const unsigned char* att_mask;              // [B, R+1] softmax mask (leading legacy column)
     const unsigned char* out_mask;              // [B, R+1] additionally applied to the returned logits
     long long out_mask_stride;                  // row stride of out_mask in bytes (0 = R+1): per-step slices of a [B,S,R+1] mask
@@ -70,6 +70,8 @@ struct AttnArgs {
                                                 //   x = g att2 + (1 - g) att2_dual, g = sigmoid(gate_w . gate_h[b] + gate_b)
     const float* gate_w; const float* gate_b;   // DUAL_REGION: core.dual_pointer.0  [H], [1]
     const float* gate_h; long long gate_ld;     //   h_att rows (pitch gate_ld)
+    int form;                                   // GVD_REGION_ATTN_* (include/gvd_b200.h): the region attentions' score (the temporal one is
+                                                //   additive in every mode); DP reads no region alpha_net (w2 / b2, and w1 / b1 in DUAL_REGION)
 };
 int gvd_attn_chunks(int R, int T, int RC, int TC, int* nch_r, int* nch_t);
 int gvd_attn_partial(const AttnArgs& a, cudaStream_t st);

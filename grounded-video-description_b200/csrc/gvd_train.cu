@@ -348,6 +348,34 @@ __global__ void att_scores_bwd_kernel(const float* __restrict__ ds, const float*
     }
 }
 
+// multiplicative scores ('mix_mul', AttModel.py:81-82): s[b,n] = w . tanh(p[b,n,:] * q[b,:]) + bias
+__global__ void att_scores_mul_fwd_kernel(const float* __restrict__ p, const float* __restrict__ q, const float* __restrict__ w,
+                                          const float* __restrict__ bias, float* __restrict__ s, int N, int A, long long rows) {
+    const long long row = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;      // one warp per (b, n)
+    const int lane = threadIdx.x & 31;
+    if (row >= rows) return;
+    const long long b = row / N;
+    float acc = 0.f;
+    for (int a = lane; a < A; a += 32) acc += w[a] * tanhf(p[row * A + a] * q[b * A + a]);
+    acc = warp_sum(acc);
+    if (lane == 0) s[row] = acc + bias[0];
+}
+// dpre = ds[b,n] w[a] (1 - t^2):  dp[b,n,a] = dpre q[b,a],  dqt[b,n,a] = dpre p[b,n,a],  dst[b,n,a] = ds[b,n] t   (t recomputed; the sums over
+// n / rows are the colsum kernel's, so nothing here accumulates across threads)
+__global__ void att_scores_mul_bwd_kernel(const float* __restrict__ ds, const float* __restrict__ p, const float* __restrict__ q,
+                                          const float* __restrict__ w, float* __restrict__ dp, float* __restrict__ dqt, float* __restrict__ dst, int N,
+                                          int A, long long total) {
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
+        const int a = (int)(i % A);
+        const long long row = i / A, b = row / N;
+        const float pv = p[i], qv = q[b * A + a], t = tanhf(pv * qv), d = ds[row];
+        const float dpre = d * w[a] * (1.f - t * t);
+        dp[i] = dpre * qv;
+        dqt[i] = dpre * pv;
+        dst[i] = d * t;
+    }
+}
+
 // ---------------------------------------------------------------- embeddings
 __global__ void gather_rows_kernel(const float* __restrict__ table, const long long* __restrict__ idx, float* __restrict__ out, int D, long long total) {
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x)
@@ -616,6 +644,19 @@ GVD_API int gvd_tr_att_scores_fwd(const float* p, const float* q, const float* w
 GVD_API int gvd_tr_att_scores_bwd(const float* ds, const float* p, const float* q, const float* w, float* dpre, float* dst, int B, int N, int A, void* st) {
     const long long total = (long long)B * N * A;
     att_scores_bwd_kernel<<<grid_for(total), TB, 0, ST(st)>>>(ds, p, q, w, dpre, dst, N, A, total);
+    LAUNCH_OK();
+}
+GVD_API int gvd_tr_att_scores_mul_fwd(const float* p, const float* q, const float* w, const float* bias, float* s, int B, int N, int A, void* st) {
+    GVD_REQUIRE(p && q && w && bias && s, "tr_att_scores_mul_fwd: null argument");
+    const long long rows = (long long)B * N;
+    att_scores_mul_fwd_kernel<<<gvd_cdiv(rows * 32, TB), TB, 0, ST(st)>>>(p, q, w, bias, s, N, A, rows);
+    LAUNCH_OK();
+}
+GVD_API int gvd_tr_att_scores_mul_bwd(const float* ds, const float* p, const float* q, const float* w, float* dp, float* dqt, float* dst, int B, int N,
+                                      int A, void* st) {
+    GVD_REQUIRE(ds && p && q && w && dp && dqt && dst, "tr_att_scores_mul_bwd: null argument");
+    const long long total = (long long)B * N * A;
+    att_scores_mul_bwd_kernel<<<grid_for(total), TB, 0, ST(st)>>>(ds, p, q, w, dp, dqt, dst, N, A, total);
     LAUNCH_OK();
 }
 GVD_API int gvd_tr_gather_rows(const float* table, const int64_t* idx, float* out, long long M, int D, void* st) {

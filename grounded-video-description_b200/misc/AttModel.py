@@ -13,12 +13,14 @@ except ImportError:
 
 
 class _AttentionParams(nn.Module):
-    """h2att + alpha_net of Attention / Attention2 (AttModel.py:22-31, 56-68; additive 'mix' mode)."""
+    """h2att + alpha_net of Attention / Attention2 (AttModel.py:22-31, 56-68).  alpha_net=False: Attention2 in region_attn_mode 'dp' (a
+    plain dot product p . q, AttModel.py:62-65,95-96), which has no alpha_net."""
 
-    def __init__(self, opt):
+    def __init__(self, opt, alpha_net=True):
         super().__init__()
         self.h2att = nn.Linear(opt.rnn_size, opt.att_hid_size)
-        self.alpha_net = nn.Linear(opt.att_hid_size, 1)
+        if alpha_net:
+            self.alpha_net = nn.Linear(opt.att_hid_size, 1)
 
 
 class TopDownCore(nn.Module):
@@ -27,9 +29,10 @@ class TopDownCore(nn.Module):
         self.att_lstm = nn.LSTMCell(opt.input_encoding_size + opt.rnn_size, opt.rnn_size)
         self.lang_lstm = nn.LSTMCell(opt.rnn_size * 2, opt.rnn_size)
         self.attention = _AttentionParams(opt)
-        self.attention2 = _AttentionParams(opt)
+        region_alpha = getattr(opt, "region_attn_mode", "mix") != "dp"
+        self.attention2 = _AttentionParams(opt, region_alpha)
         if opt.att_input_mode == "dual_region":                 # AttModel.py:126-128
-            self.attention2_dual = _AttentionParams(opt)
+            self.attention2_dual = _AttentionParams(opt, region_alpha)
             self.dual_pointer = nn.Sequential(nn.Linear(opt.rnn_size, 1), nn.Sigmoid())
         # present in every reference checkpoint, never used by forward (AttModel.py:130-131)
         self.i2h_2 = nn.Linear(opt.rnn_size * 2, opt.rnn_size)

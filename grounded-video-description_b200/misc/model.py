@@ -47,6 +47,7 @@ class AttModel(CaptionModel):
         self.seq_per_img = opt.seq_per_img
         self.itod = opt.itod
         self.att_input_mode = opt.att_input_mode
+        self.region_attn_mode = getattr(opt, "region_attn_mode", "mix")
         self.transfer_mode = opt.transfer_mode
         self.test_mode = opt.test_mode
         self.enable_BUTD = opt.enable_BUTD
@@ -64,7 +65,7 @@ class AttModel(CaptionModel):
         import types
         self.opt_ns = types.SimpleNamespace(rnn_size=opt.rnn_size, seq_length=opt.seq_length, vocab_size=opt.vocab_size,
                                             num_sampled_frm=opt.num_sampled_frm, obj_interact=getattr(opt, "obj_interact", False),
-                                            att_input_mode=self.att_input_mode)
+                                            att_input_mode=self.att_input_mode, region_attn_mode=self.region_attn_mode)
         self.vis_encoding_size = 2048
         self.pool_feat_size = self.att_feat_size + 300 + self.detect_size + 1
 
@@ -152,6 +153,7 @@ class AttModel(CaptionModel):
         o.att_feat_size, o.fc_feat_size, o.obj_interact = d.att_feat_size, d.fc_feat_size, bool(d.obj_interact)
         o.wtoi = {"UNK": str(d.unk_idx)}
         o.att_model, o.att_input_mode = self.att_model, self.att_input_mode     # the language LSTM's input (AttModel.py:144-156)
+        o.region_attn_mode = self.region_attn_mode                              # the region attention's score (AttModel.py:79-96)
         return o
 
     @staticmethod

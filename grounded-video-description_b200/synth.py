@@ -122,12 +122,15 @@ def state_dict_spec(opt):
         spec.append(("core.%s.weight_hh" % name, (4 * H, H), "uniform", H))
         spec.append(("core.%s.bias_ih" % name, (4 * H,), "uniform", H))
         spec.append(("core.%s.bias_hh" % name, (4 * H,), "uniform", H))
+    region_alpha = getattr(opt, "region_attn_mode", "mix") != "dp"      # 'dp': Attention2 has no alpha_net (AttModel.py:62-65)
     for name in ("attention", "attention2"):
         lin("core.%s.h2att" % name, A, H)
-        lin("core.%s.alpha_net" % name, 1, A)
+        if name == "attention" or region_alpha:
+            lin("core.%s.alpha_net" % name, 1, A)
     if getattr(opt, "att_input_mode", "both") == "dual_region":        # AttModel.py:126-128, registered after attention2
         lin("core.attention2_dual.h2att", A, H)
-        lin("core.attention2_dual.alpha_net", 1, A)
+        if region_alpha:
+            lin("core.attention2_dual.alpha_net", 1, A)
         lin("core.dual_pointer.0", 1, H)
     lin("core.i2h_2", H, 2 * H)
     lin("core.h2h_2", H, H)

@@ -18,7 +18,7 @@ The primitive set `ops` (all tensors fp32, contiguous, on the device of `ops`):
     bmm_nt / bmm_nn / bmm_tn        batched versions on [b, ., .]
     colsum(x2d), sum_all(x)
     relu_bwd(dy, y), ln / ln_bwd, ln_star / ln_star_bwd, softmax / softmax_bwd
-    lstm_cell / lstm_cell_bwd, gru_cell / gru_cell_bwd, att_scores / att_scores_bwd, outer_rows
+    lstm_cell / lstm_cell_bwd, gru_cell / gru_cell_bwd, att_scores / att_scores_bwd, att_scores_mul / att_scores_mul_bwd, outer_rows
     gather_rows / index_add_rows, lm_nll, pos_nll, cls_nll, bn_train / bn_train_bwd
     add, mul, scale, masked_fill, zeros_like / zeros, cat, clip_adam
 """
@@ -115,19 +115,27 @@ class TrainStep:
         self._acc(grads, p + ".bias_hh", bsum)
         return ops.mm_nn(dgates, W[p + ".weight_ih"]), ops.mm_nn(dgates, W[p + ".weight_hh"]), dc
 
-    def _attn_fwd(self, p_feats, feats, q, w, b, mask, need_out=True):
-        """need_out = False: the scores only (att_input_mode 'featmap' discards the region attention's weighted sum, AttModel.py:145-146)."""
+    def _attn_fwd(self, p_feats, feats, q, w, b, mask, need_out=True, form="mix"):
+        """need_out = False: the scores only (att_input_mode 'featmap' discards the region attention's weighted sum, AttModel.py:145-146).
+        form: the score of region_attn_mode (AttModel.py:79-96): 'mix' w . tanh(p + q) + b, 'mix_mul' w . tanh(p * q) + b, 'dp' p . q (w, b
+        unused)."""
         ops = self.ops
-        s = ops.att_scores(p_feats, q, w, b)
+        if form == "dp":
+            s = ops.bmm_nn(p_feats, q.unsqueeze(2)).squeeze(2)                 # [B,N,A] x [B,A,1]
+        elif form == "mix_mul":
+            s = ops.att_scores_mul(p_feats, q, w, b)
+        else:
+            s = ops.att_scores(p_feats, q, w, b)
         if mask is not None:
             s = ops.masked_fill(s, mask, MIN_VALUE)
         a = ops.softmax(s, 1.0)
         out = ops.bmm_nn(a.unsqueeze(1), feats).squeeze(1) if need_out else None     # [B,1,N] x [B,N,H]
-        return out, s, dict(a=a, mask=mask, q=q)
+        return out, s, dict(a=a, mask=mask, q=q, form=form)
 
     def _attn_bwd(self, dout, ds_extra, tp, p_feats, feats, w, dfeats_acc):
         """dfeats_acc [B,N,H] += a (x) dout in place (the gradient of the attended features, summed over the decode steps).
-        dout = None: the weighted sum reached no loss, only the scores did (ds_extra)."""
+        dout = None: the weighted sum reached no loss, only the scores did (ds_extra).  Returns (dp_feats, dq, dw, db); dw = db = None in
+        the form 'dp' (no alpha_net)."""
         ops = self.ops
         a = tp["a"]
         if dout is None:
@@ -140,6 +148,10 @@ class TrainStep:
                 ds = ops.add(ds, ds_extra)
         if tp["mask"] is not None:
             ds = ops.masked_fill(ds, tp["mask"], 0.0)
+        if tp["form"] == "dp":                                              # s = p . q:  dp = ds (x) q,  dq = sum_n ds p
+            return ops.outer_rows(ds, tp["q"]), ops.bmm_nn(ds.unsqueeze(1), p_feats).squeeze(1), None, None
+        if tp["form"] == "mix_mul":
+            return ops.att_scores_mul_bwd(ds, p_feats, tp["q"], w)
         dpre, dq, dw, db = ops.att_scores_bwd(ds, p_feats, tp["q"], w)
         return dpre, dq, dw, db
 
@@ -402,6 +414,7 @@ class TrainStep:
         mode = getattr(opt, "att_input_mode", "both")
         featmap = mode == "featmap"                     # language LSTM input cat(att, h_att) (AttModel.py:145-146)
         dual = mode == "dual_region"                    # cat(g att2 + (1 - g) att2_dual, h_att), no frame branch (AttModel.py:153-156, model.py:393)
+        form = getattr(opt, "region_attn_mode", "mix")  # the region attentions' score (AttModel.py:79-96); the temporal one is additive
         pt = self._prologue_fwd(W, opt, inp, pmask, keep_d, D_, frames=not dual)
         fc_feats, g_pool, simT, pool_feats, p_pool, conv, p_conv = (pt[k] for k in ("fc_feats", "g_pool", "simT", "pool_feats", "p_pool", "conv",
                                                                                       "p_conv"))
@@ -409,9 +422,9 @@ class TrainStep:
         # ========================================================== forward, teacher-forced loop
         tgt = ops.host_targets(self, opt, inp, host)                                     # overlaps, class targets, per-step labels / masks
         a1w, a1b = W["core.attention.alpha_net.weight"], W["core.attention.alpha_net.bias"]
-        a2w, a2b = W["core.attention2.alpha_net.weight"], W["core.attention2.alpha_net.bias"]
+        a2w, a2b = W.get("core.attention2.alpha_net.weight"), W.get("core.attention2.alpha_net.bias")          # (None in 'dp')
         if dual:
-            adw, adb = W["core.attention2_dual.alpha_net.weight"], W["core.attention2_dual.alpha_net.bias"]
+            adw, adb = W.get("core.attention2_dual.alpha_net.weight"), W.get("core.attention2_dual.alpha_net.bias")
         h_att = c_att = h_lang = c_lang = ops.zeros((B, H))
         steps, outs, z_list = [], [], []
         for i in range(S):                                                               # S: the reference's early exit (model.py:425)
@@ -424,13 +437,13 @@ class TrainStep:
                 q1 = ops.lin(h_att2, W["core.attention.h2att.weight"], W["core.attention.h2att.bias"], False)
                 att, _, t_a1 = self._attn_fwd(p_conv, conv, q1, a1w, a1b, None)
             q2 = ops.lin(h_att2, W["core.attention2.h2att.weight"], W["core.attention2.h2att.bias"], False)
-            att2, z, t_a2 = self._attn_fwd(p_pool, pool_feats, q2, a2w, a2b, pmask, need_out=not featmap)
+            att2, z, t_a2 = self._attn_fwd(p_pool, pool_feats, q2, a2w, a2b, pmask, need_out=not featmap, form=form)
             fmask = tgt["fm"][i]                                                         # B, R (bool): frame mask | proposal mask
             z_out = ops.masked_fill(z, fmask, MIN_VALUE)
             st = dict(tok=tok, emb_raw=emb_raw, t_att=t_att, t_a2=t_a2, h_att2=h_att2, fmask=fmask)
             if dual:
                 qd = ops.lin(h_att2, W["core.attention2_dual.h2att.weight"], W["core.attention2_dual.h2att.bias"], False)
-                att2d, _, t_ad = self._attn_fwd(p_pool, pool_feats, qd, adw, adb, pmask)
+                att2d, _, t_ad = self._attn_fwd(p_pool, pool_feats, qd, adw, adb, pmask, form=form)
                 # g = sigmoid(dual_pointer(h_att)) as column 0 of softmax([logit, 0]); column 1 is 1 - g
                 # (the single-output Linear as a row dot product: no GEMM with one output column)
                 wpE = W["core.dual_pointer.0.weight"].expand(B, H).contiguous()
@@ -512,15 +525,17 @@ class TrainStep:
                     dh_att = ops.add(dh_att, ops.mul(dglogE, st["wpE"]))
                     dpd, dqd, dwd, dbd = self._attn_bwd(dgd, None, st["t_ad"], p_pool, pool_feats, adw, dpool_feats)
                     dp_pool = ops.add(dp_pool, dpd)
-                    self._acc(grads, "core.attention2_dual.alpha_net.weight", dwd.reshape(1, -1))
-                    self._acc(grads, "core.attention2_dual.alpha_net.bias", dbd.reshape(1))
+                    if dwd is not None:
+                        self._acc(grads, "core.attention2_dual.alpha_net.weight", dwd.reshape(1, -1))
+                        self._acc(grads, "core.attention2_dual.alpha_net.bias", dbd.reshape(1))
                     dh_att = ops.add(dh_att, self._lin_bwd(dqd, st["h_att2"], W, "core.attention2_dual.h2att", grads))
                 if region_grad:
                     dz = ops.masked_fill(dz_all[:, i].contiguous(), st["fmask"], 0.0)
                     dpp, dq2, dw2, db2 = self._attn_bwd(None if featmap else datt2, dz, st["t_a2"], p_pool, pool_feats, a2w, dpool_feats)
                     dp_pool = ops.add(dp_pool, dpp)
-                    self._acc(grads, "core.attention2.alpha_net.weight", dw2.reshape(1, -1))
-                    self._acc(grads, "core.attention2.alpha_net.bias", db2.reshape(1))
+                    if dw2 is not None:
+                        self._acc(grads, "core.attention2.alpha_net.weight", dw2.reshape(1, -1))
+                        self._acc(grads, "core.attention2.alpha_net.bias", db2.reshape(1))
                     dh_att = ops.add(dh_att, self._lin_bwd(dq2, st["h_att2"], W, "core.attention2.h2att", grads))
                 if not dual:
                     dpc, dq1, dw1, db1 = self._attn_bwd(datt_sum, None, st["t_a1"], p_conv, conv, a1w, dconv)

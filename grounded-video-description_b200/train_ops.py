@@ -41,6 +41,8 @@ _SIGS = {
     "gvd_tr_gru_cell_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _ci, _ci, _vp],
     "gvd_tr_att_scores_fwd": [_vp, _vp, _vp, _vp, _vp, _ci, _ci, _ci, _vp],
     "gvd_tr_att_scores_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _ci, _ci, _ci, _vp],
+    "gvd_tr_att_scores_mul_fwd": [_vp, _vp, _vp, _vp, _vp, _ci, _ci, _ci, _vp],
+    "gvd_tr_att_scores_mul_bwd": [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _ci, _ci, _ci, _vp],
     "gvd_tr_gather_rows": [_vp, _vp, _vp, _ll, _ci, _vp],
     "gvd_tr_index_add_rows": [_vp, _vp, _vp, _ci, _ci, _ci, _vp],
     "gvd_tr_bn_normalize": [_vp, _vp, _vp, _vp, _ll, _ci, _vp],
@@ -313,6 +315,24 @@ class NativeOps:
         dq = self._new(B, A)
         capi.check(self.L.gvd_tr_colsum(_p(dpre), _p(dq), B, N, A, self._st()))            # per clip: sum over the N rows
         return dpre, dq, self.colsum(dst.reshape(B * N, A)), self.sum_all(ds)
+
+    # ---- multiplicative attention scores (region_attn_mode 'mix_mul')  s[b,n] = w . tanh(p[b,n,:] * q[b,:]) + b
+    def att_scores_mul(self, p, q, w, b):
+        p, q = _f(p), _f(q)
+        B, N, A = p.shape
+        s = self._new(B, N)
+        capi.check(self.L.gvd_tr_att_scores_mul_fwd(_p(p), _p(q), _p(_f(w).reshape(-1)), _p(_f(b).reshape(-1)), _p(s), B, N, A, self._st()))
+        return s
+
+    def att_scores_mul_bwd(self, ds, p, q, w):
+        """(dp, dq, dw, db): the per-element terms come from one kernel, their sums from the deterministic colsum kernel (no atomics)."""
+        ds, p, q = _f(ds), _f(p), _f(q)
+        B, N, A = p.shape
+        dp, dqt, dst = torch.empty_like(p), torch.empty_like(p), torch.empty_like(p)
+        capi.check(self.L.gvd_tr_att_scores_mul_bwd(_p(ds), _p(p), _p(q), _p(_f(w).reshape(-1)), _p(dp), _p(dqt), _p(dst), B, N, A, self._st()))
+        dq = self._new(B, A)
+        capi.check(self.L.gvd_tr_colsum(_p(dqt), _p(dq), B, N, A, self._st()))             # per clip: sum over the N rows
+        return dp, dq, self.colsum(dst.reshape(B * N, A)), self.sum_all(ds)
 
     # ---- embeddings
     def gather_rows(self, table, idx):

@@ -60,11 +60,23 @@ GVD_API int gvd_model_create(const gvd_dims_t* dims, gvd_model_t** out);   /* at
  *               masks, read in one pass; the returned logits are the first one's.  No temporal attention: the prologue skips the frame
  *               branch (att_embed, BatchNorm, bi-GRU, ctx2att).  The parameter list gains core.attention2_dual.{h2att,alpha_net}.* and
  *               core.dual_pointer.0.* (after core.attention2.*, before core.i2h_2.*).
- * 'region' is not implemented: gvd_model_create_mode rejects it. */
+ * 'region' is not implemented: gvd_model_create_mode and gvd_model_create_modes reject it. */
 #define GVD_ATT_INPUT_BOTH 0
 #define GVD_ATT_INPUT_FEATMAP 1
 #define GVD_ATT_INPUT_DUAL_REGION 2
-GVD_API int gvd_model_create_mode(const gvd_dims_t* dims, int att_input_mode, gvd_model_t** out);
+GVD_API int gvd_model_create_mode(const gvd_dims_t* dims, int att_input_mode, gvd_model_t** out);   /* region_attn_mode 'mix' */
+/* opt.region_attn_mode (opts.py:63-64, AttModel.py:56-108): how the region attention Attention2 (and attention2_dual in DUAL_REGION)
+ * scores proposal r against the query q = h2att(h_att).  The temporal attention is additive in every mode; the grounding is unchanged.
+ *   MIX     (0) z_r = w . tanh(p_r + q) + b   (the default);
+ *   MIX_MUL (1) z_r = w . tanh(p_r * q) + b   (element-wise product; same parameters as MIX);
+ *   DP      (2) z_r = p_r . q                 (no tanh, weight or bias: the parameter list has no core.attention2.alpha_net.* nor, in
+ *               DUAL_REGION, core.attention2_dual.alpha_net.*).
+ * 'add' (a model-level alpha_net the grounding applies to 2048-wide vectors, model.py:55-56,256-261) and 'cat' (Attention2.forward reads an
+ * undefined `xt`, AttModel.py:87) cannot run in the reference and are rejected. */
+#define GVD_REGION_ATTN_MIX 0
+#define GVD_REGION_ATTN_MIX_MUL 1
+#define GVD_REGION_ATTN_DP 2
+GVD_API int gvd_model_create_modes(const gvd_dims_t* dims, int att_input_mode, int region_attn_mode, gvd_model_t** out);
 GVD_API void gvd_model_destroy(gvd_model_t* m);
 /* Copy one state_dict entry (by its reference key, e.g. "core.att_lstm.weight_ih") from a
  * DEVICE fp32 buffer of `numel` elements into the model's packed weight arena. */
@@ -275,6 +287,14 @@ GVD_API int gvd_op_attention_mode(const float* p_pool, const float* pool, const 
                   int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld, int B, int R, int T, int A, int H, int RC, int TC,
                   int feat_div, int att_input_mode, const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld,
                   void* stream);
+/* gvd_op_attention_form: gvd_op_attention_mode with the region score form GVD_REGION_ATTN_* (gvd_op_attention_mode = MIX).  In DP the region
+ *   alpha_net pointers (w2 / b2, and w1 / b1 in DUAL_REGION) are not read and may be NULL. */
+GVD_API int gvd_op_attention_form(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                  const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2, const float* b2,
+                  const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out, int64_t z_stride_b, float* partial,
+                  int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld, int B, int R, int T, int A, int H, int RC, int TC,
+                  int feat_div, int att_input_mode, const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld,
+                  int region_attn_mode, void* stream);
 /* beam_topk: per row of logits [rows, V] (pitch ld) the K <= 8 (K <= V) best words, value descending, ties to the lower index:
  *   topv [rows, K] = their log_softmax, topi [rows, K].  NaN words are skipped; a pick that finds only NaN left takes the lowest untaken
  *   index, so an all-NaN row gives 0 .. K-1 (as a stable torch.sort(descending=True) does).  Rows only partly NaN differ from torch,
@@ -342,6 +362,12 @@ GVD_API int gvd_tr_gru_cell_bwd(const float* dh, const float* r, const float* z,
                   float* dgh, float* dh_keep, int B, int G, void* stream);
 GVD_API int gvd_tr_att_scores_fwd(const float* p, const float* q, const float* w, const float* bias, float* s, int B, int N, int A, void* stream);
 GVD_API int gvd_tr_att_scores_bwd(const float* ds, const float* p, const float* q, const float* w, float* dpre, float* ds_t, int B, int N, int A, void* stream);
+/* multiplicative scores (region_attn_mode 'mix_mul'): s[b,n] = w . tanh(p[b,n,:] * q[b,:]) + bias; the backward writes, per [b,n,a] with
+ * t = tanh(p q) and dpre = ds[b,n] w[a] (1 - t^2):  dp = dpre q[b,a],  dq_t = dpre p[b,n,a] (dq = its sum over n),  ds_t = ds[b,n] t (dw = its
+ * sum over b, n) */
+GVD_API int gvd_tr_att_scores_mul_fwd(const float* p, const float* q, const float* w, const float* bias, float* s, int B, int N, int A, void* stream);
+GVD_API int gvd_tr_att_scores_mul_bwd(const float* ds, const float* p, const float* q, const float* w, float* dp, float* dq_t, float* ds_t, int B,
+                  int N, int A, void* stream);
 GVD_API int gvd_tr_gather_rows(const float* table, const int64_t* idx, float* out, long long M, int D, void* stream);
 GVD_API int gvd_tr_index_add_rows(const int64_t* idx, const float* rows, float* out, int n_rows, int M, int D, void* stream);
 GVD_API int gvd_tr_bn_normalize(const float* e, const float* mu, const float* var, float* out, long long M, int N, void* stream);
