@@ -20,7 +20,7 @@ EXPORTS = [
     "gvd_decode_reset_state", "gvd_sample_greedy_host", "gvd_op_linear", "gvd_op_tanh", "gvd_op_kernel_launches",
     "gvd_profile_enable", "gvd_profile_reset", "gvd_profile_count", "gvd_profile_entry",
     "gvd_op_linear_tc", "gvd_op_linear_f16ss", "gvd_op_skinny_partials", "gvd_op_reduce_lstm", "gvd_op_reduce_bias", "gvd_op_reduce_pick",
-    "gvd_op_reduce_sample", "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_attention", "gvd_op_attention_mode", "gvd_op_attention_form", "gvd_op_beam_topk",
+    "gvd_op_reduce_sample", "gvd_op_reduce_pick_split", "gvd_op_greedy_pick", "gvd_op_logit_pick_tc", "gvd_op_gru_layer", "gvd_op_attention", "gvd_op_attention_mode", "gvd_op_attention_form", "gvd_op_beam_topk",
     "gvd_op_row_argmax", "gvd_op_beam_search_scripted", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_self_attention_fused", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
     "gvd_tfm_workspace_bytes", "gvd_tfm_decode_greedy", "gvd_tfm_teacher_fwd",
     "gvd_grounding_extract", "gvd_grounding_eval", "gvd_plan_skinny_splits", "gvd_plan_h2d_chunks", "gvd_workspace_bytes_beam", "gvd_beam_decode", "gvd_workspace_bytes_teacher", "gvd_teacher_fwd",
@@ -98,6 +98,8 @@ def lib():
     L.gvd_op_reduce_pick.argtypes = [vp, ci, ci, vp, ci, ci, ci, vp, vp, vp, i64, vp, vp, i64, ci, vp, i64, vp, i64, vp]
     L.gvd_op_greedy_pick.argtypes = [vp, i64, ci, ci, ci, vp, vp, vp, i64, vp, vp, i64, ci, vp]
     L.gvd_op_reduce_sample.argtypes = [vp, ci, ci, vp, ci, ci, ctypes.c_float, ctypes.c_uint64, ci, vp, vp, vp, i64, vp, vp, i64, ci, vp, i64, vp]
+    L.gvd_op_reduce_pick_split.argtypes = [vp, ci, ci, vp, ci, ci, ci, ci, ctypes.c_float, ctypes.c_uint64, ci, vp, vp, vp, i64, vp, vp, i64, ci, vp,
+                                           i64, vp, i64, vp]
     L.gvd_op_logit_pick_tc.argtypes = [vp, i64, vp, i64, vp, ci, ci, ci, ci, vp, ci, vp, vp, vp, i64, vp, vp]
     L.gvd_op_gru_layer.argtypes = [ci, vp, vp, vp, vp, ci, ci, ci, vp, vp]
     L.gvd_op_attention.argtypes = [vp, vp, vp, vp, vp, vp, ci, vp, vp, vp, vp, vp, vp, vp, i64, vp, i64, vp, vp, vp, i64, vp, i64,
@@ -632,6 +634,21 @@ def op_reduce_sample(part, bias, V, temperature, seed, step, it, seq=None, logp=
     check(lib().gvd_op_reduce_sample(_ptr(part), S, ldp, _ptr(bias), B, V, float(temperature), int(seed) & 0xFFFFFFFFFFFFFFFF, int(step), _ptr(it),
                                      _ptr(seq), _ptr(logp), _strided_outputs(seq, logp), _ptr(embed), _ptr(xt), _pitch(xt), E, _ptr(xt_pk),
                                      _pitch(xt_pk), _stream()))
+
+
+VOCAB_GREEDY, VOCAB_SAMPLE, VOCAB_ARGMAX = 0, 1, 2
+
+
+def op_reduce_pick_split(part, bias, V, mode, it, unk=-1, temperature=1.0, seed=0, step=0, seq=None, logp=None, embed=None, xt=None,
+                         logits_out=None, xt_pk=None):
+    """The vocabulary tail for any V on partial planes part [S, B, ldp] (+ bias or None): mode VOCAB_GREEDY (top-2 + UNK rule),
+    VOCAB_SAMPLE (the multinomial draw at (temperature, seed, step)) or VOCAB_ARGMAX (first maximum)."""
+    S, B, ldp = part.shape
+    E = embed.shape[1] if embed is not None else 0
+    check(lib().gvd_op_reduce_pick_split(_ptr(part), S, ldp, _ptr(bias), B, V, int(mode), int(unk), float(temperature),
+                                         int(seed) & 0xFFFFFFFFFFFFFFFF, int(step), _ptr(it), _ptr(seq), _ptr(logp), _strided_outputs(seq, logp),
+                                         _ptr(embed), _ptr(xt), _pitch(xt), E, _ptr(logits_out), _pitch(logits_out), _ptr(xt_pk), _pitch(xt_pk),
+                                         _stream()))
 
 
 def op_greedy_pick(logits, unk, it, seq=None, logp=None, embed=None, xt=None):

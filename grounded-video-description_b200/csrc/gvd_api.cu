@@ -566,6 +566,7 @@ struct WS {
     int* ticket;                       // [rows] last-CTA tickets of the fused attention combine
     float* pk_part; int* pk_ticket;    // fused vocabulary head + greedy pick: per-CTA partials, one ticket
     GvdSampleParams* sample_par;       // seed + temperature of the multinomial sampler, copied in before each decode
+    float* vt_rec; int* vt_ticket;     // vocabularies above 6144 words: per-(row, slice) records and per-row tickets of gvd_vocab_tail
     // beam search (rows = B * beam)
     BeamBufs bb;
     int* bos_att;
@@ -688,6 +689,11 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     w.pk_ticket = (int*)take(256);
     // the sampler's parameter block shares the ticket's slot: the workspace keeps the size and layout it has without sampling
     w.sample_par = (GvdSampleParams*)((char*)w.pk_ticket + 128);
+    w.vt_rec = nullptr; w.vt_ticket = nullptr;
+    if (d.vocab_size > 6144) {
+        w.vt_rec = (float*)take(gvd_vocab_rec_floats((int)BD, d.vocab_size) * 4);
+        w.vt_ticket = (int*)take(BD * 4);
+    }
     if (beam > 1) {
         const size_t L = d.seq_length, K = beam;
         w.bb.seq = (int*)take((size_t)B * L * K * 4);
@@ -1107,6 +1113,7 @@ extern "C" GVD_API int gvd_decode_reset_state(gvd_model_t* m, int B, int T, void
     GVD_CHECK_CUDA(cudaMemsetAsync(w.c_lang, 0, n, st));
     GVD_CHECK_CUDA(cudaMemsetAsync(w.ticket, 0, (size_t)B * w.beam * sizeof(int), st));
     GVD_CHECK_CUDA(cudaMemsetAsync(w.pk_ticket, 0, sizeof(int), st));
+    if (w.vt_ticket) GVD_CHECK_CUDA(cudaMemsetAsync(w.vt_ticket, 0, (size_t)B * w.beam * sizeof(int), st));
     if (w.xcat_att) {      // split-K path: the recurrent states also live inside the concatenated LSTM inputs
         GVD_CHECK_CUDA(cudaMemsetAsync(w.xcat_att, 0, (size_t)B * w.beam * (m->d.input_encoding_size + m->d.rnn_size) * sizeof(float), st));
         GVD_CHECK_CUDA(cudaMemsetAsync(w.xcat_lang, 0, (size_t)B * w.beam * 3 * m->d.rnn_size * sizeof(float), st));
@@ -1289,11 +1296,21 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
                                                              m->P("embed.0.weight"), w.xt, d.input_encoding_size, st));
         } else {
             const int E = d.input_encoding_size;
-            const int S = (tc && (gvd_backend() & 8) != 0 && w.sk_part && V <= 6144) ? gvd_skinny_splits(V, H, B) : 0;
+            const int S = (tc && (gvd_backend() & 8) != 0 && w.sk_part) ? gvd_skinny_splits(V, H, B) : 0;
             const bool sk_core = core_skinny(m, w, B, 1);                       // then xt goes into the core step's concatenated input
+            const bool sk16 = sk_core && core_skinny_f16(m);                    // ... and its fp16x3 image into xp_att
+            // above 6144 words (reduce_pick / reduce_sample hold a row in one CTA's registers): the sliced tail, one CTA per (row, 1024 words)
+            auto vocab_tail = [&](const float* part, int nplanes, const float* bias, float* xt, float* xt_pk) {
+                VocabTailArgs a{};
+                a.part = part; a.S = nplanes; a.plane = (long long)B * m->Vp; a.ldp = m->Vp; a.bias = bias; a.B = B; a.V = V;
+                a.mode = sample ? VOCAB_SAMPLE : VOCAB_GREEDY; a.unk_idx = d.unk_idx; a.par = sample; a.step = t;
+                a.it_out = w.it; a.seq_out = (long long*)seq_out + t; a.logp_out = logprobs_out ? logprobs_out + t : nullptr; a.out_stride = L;
+                a.embed = xt ? m->P("embed.0.weight") : nullptr; a.xt = xt; a.ld_xt = sk_core ? E + H : E; a.E = E; a.xt_pk = xt_pk; a.ld_xt_pk = E + H;
+                a.rec = w.vt_rec; a.ticket = w.vt_ticket;
+                return gvd_vocab_tail(a, st);
+            };
             if (S > 0) {
                 // vocabulary head: split-K partials, then ONE kernel sums them, adds the bias and samples (no [B,V] logits round trip)
-                const bool sk16 = sk_core && core_skinny_f16(m);
                 const float* Wp; long long ldwp;
                 if (sk16 && gvd_packed_lookup(m->P("logit.weight"), H, V, H, &Wp, &ldwp)) {
                     GVD_STAGE("decode.logit", gvd_skinny_f16(Wp, ldwp, V, w.xp_lang + 2 * H, 3 * H, B, H, S, w.sk_part, m->Vp, st));     // X = h_lang(t) inside xp_lang
@@ -1301,7 +1318,10 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
                     GVD_REQUIRE(!sk16, "decode: packed vocabulary-head weights missing");
                     GVD_STAGE("decode.logit", gvd_skinny_splitk(m->P("logit.weight"), V, H, h, H, B, S, w.sk_part, m->Vp, st));
                 }
-                if (sample) {
+                if (V > 6144) {
+                    GVD_STAGE(sample ? "decode.sample" : "decode.pick", vocab_tail(w.sk_part, S, m->P("logit.bias"), sk_core ? w.xcat_att : w.xt,
+                                                                                   sk16 ? w.xp_att : nullptr));
+                } else if (sample) {
                     GVD_STAGE("decode.sample", gvd_reduce_sample(w.sk_part, S, m->Vp, m->P("logit.bias"), B, V, sample, t, w.it, (long long*)seq_out + t,
                                                                  logprobs_out ? logprobs_out + t : nullptr, L, m->P("embed.0.weight"),
                                                                  sk_core ? w.xcat_att : w.xt, sk_core ? E + H : E, E, st, sk16 ? w.xp_att : nullptr, E + H));
@@ -1312,7 +1332,10 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
                 }
             } else {
                 GVD_STAGE("decode.logit", gvd_linear(h, H, m->P("logit.weight"), H, m->P("logit.bias"), w.logits, m->Vp, B, V, H, GVD_ACT_NONE, st));
-                if (sample) {   // the logits already hold the bias: one plane, no bias
+                if (V > 6144) {   // (the sliced tail also writes the image of xt, which the next step's products read)
+                    GVD_STAGE(sample ? "decode.sample" : "decode.pick", vocab_tail(w.logits, 1, nullptr, tc ? (sk_core ? w.xcat_att : w.xt) : nullptr,
+                                                                                   tc && sk16 ? w.xp_att : nullptr));
+                } else if (sample) {   // the logits already hold the bias: one plane, no bias
                     GVD_STAGE("decode.sample", gvd_reduce_sample(w.logits, 1, m->Vp, nullptr, B, V, sample, t, w.it, (long long*)seq_out + t,
                                                                  logprobs_out ? logprobs_out + t : nullptr, L, tc ? m->P("embed.0.weight") : nullptr,
                                                                  tc ? (sk_core ? w.xcat_att : w.xt) : nullptr, sk_core ? E + H : E, E, st));
@@ -1379,7 +1402,6 @@ extern "C" GVD_API int gvd_decode_sample(gvd_model_t* m, int B, int T, void* wor
     GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
     GVD_REQUIRE(pnt_mask && seq_out && att2_logits_out, "decode_sample: null argument");
     GVD_REQUIRE(std::isfinite(temperature) && temperature > 0.f, "decode_sample: temperature must be finite and > 0 (got %g)", (double)temperature);
-    GVD_REQUIRE(m->d.vocab_size <= 6144, "decode_sample: the sampler holds a vocabulary of at most 6144 words (got %d)", m->d.vocab_size);
     cudaStream_t st = (cudaStream_t)stream;
     // the parameter block is copied in on the caller's stream ahead of the loop (pageable source: staged before this call returns)
     const GvdSampleParams par{(uint32_t)(seed & 0xffffffffull), (uint32_t)(seed >> 32), temperature, 0u};
@@ -1830,6 +1852,36 @@ extern "C" GVD_API int gvd_op_reduce_sample(const float* part, int S, int ldp, c
     if (!rc) rc = gvd_reduce_sample(part, S, ldp, bias, B, V, dpar, step, (long long*)it_out, (long long*)seq_out, logp_out, out_stride, embed, xt, ld_xt,
                                     E, st, xt_pk, ld_xt_pk);
     cudaFreeAsync(dpar, st);
+    return rc;
+}
+static_assert(VOCAB_GREEDY == GVD_VOCAB_GREEDY && VOCAB_SAMPLE == GVD_VOCAB_SAMPLE && VOCAB_ARGMAX == GVD_VOCAB_ARGMAX, "vocabulary tail modes");
+extern "C" GVD_API int gvd_op_reduce_pick_split(const float* part, int S, int ldp, const float* bias, int B, int V, int mode, int unk_idx,
+                                                float temperature, uint64_t seed, int step, int64_t* it_out, int64_t* seq_out, float* logp_out,
+                                                int64_t out_stride, const float* embed, float* xt, int64_t ld_xt, int E, float* logits_out,
+                                                int64_t ld_logits, float* xt_pk, int64_t ld_xt_pk, void* stream) {
+    GVD_REQUIRE(part && S >= 1 && B >= 1 && V >= 2 && it_out && (!xt || embed), "op_reduce_pick_split: bad arguments");
+    GVD_REQUIRE(mode != GVD_VOCAB_SAMPLE || (std::isfinite(temperature) && temperature > 0.f),
+                "op_reduce_pick_split: temperature must be finite and > 0 (got %g)", (double)temperature);
+    cudaStream_t st = (cudaStream_t)stream;
+    // records | tickets | sampler parameter block, in one allocation
+    const size_t rec_bytes = gvd_vocab_rec_floats(B, V) * 4, tk_bytes = ((size_t)B * 4 + 15) / 16 * 16;
+    char* buf = nullptr;
+    GVD_CHECK_CUDA(cudaMallocAsync((void**)&buf, rec_bytes + tk_bytes + sizeof(GvdSampleParams), st));
+    const GvdSampleParams par{(uint32_t)(seed & 0xffffffffull), (uint32_t)(seed >> 32), temperature, 0u};
+    VocabTailArgs a{};
+    a.part = part; a.S = S; a.plane = (long long)B * ldp; a.ldp = ldp; a.bias = bias; a.B = B; a.V = V;
+    a.mode = mode; a.unk_idx = unk_idx; a.par = reinterpret_cast<GvdSampleParams*>(buf + rec_bytes + tk_bytes); a.step = step;
+    a.it_out = (long long*)it_out; a.seq_out = (long long*)seq_out; a.logp_out = logp_out; a.out_stride = out_stride;
+    a.embed = embed; a.xt = xt; a.ld_xt = ld_xt; a.E = E; a.xt_pk = xt_pk; a.ld_xt_pk = ld_xt_pk; a.logits_out = logits_out; a.ld_logits = ld_logits;
+    a.rec = reinterpret_cast<float*>(buf); a.ticket = reinterpret_cast<int*>(buf + rec_bytes);
+    int rc = 0;
+    if (cudaMemsetAsync(a.ticket, 0, tk_bytes, st) != cudaSuccess ||
+        cudaMemcpyAsync(buf + rec_bytes + tk_bytes, &par, sizeof(par), cudaMemcpyHostToDevice, st) != cudaSuccess) {
+        gvd_set_error("op_reduce_pick_split: staging failed");
+        rc = 2;
+    }
+    if (!rc) rc = gvd_vocab_tail(a, st);
+    cudaFreeAsync(buf, st);
     return rc;
 }
 extern "C" GVD_API int gvd_op_greedy_pick(const float* logits, int64_t ld, int B, int V, int unk_idx, int64_t* it_out, int64_t* seq_out,

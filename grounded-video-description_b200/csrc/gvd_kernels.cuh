@@ -113,6 +113,26 @@ struct GvdSampleParams { uint32_t seed_lo, seed_hi; float temperature; uint32_t 
 int gvd_reduce_sample(const float* part, int S, int ldp, const float* bias, int B, int V, const GvdSampleParams* params, int step,
                       long long* it_out, long long* seq_out, float* logp_out, long long out_stride, const float* embed, float* xt,
                       long long ld_xt, int E, cudaStream_t st, float* xt_pk = nullptr, long long ld_xt_pk = 0);
+// Vocabulary head tail for any V (gvd_skinny.cu): one CTA per (row, slice of VOCAB_SLICE words) writes a record of its slice, the last CTA
+// of the row merges the records in a fixed order and writes the outputs.  Same destinations as reduce_pick / reduce_sample, plus the
+// transformer head's logits copy and teacher-forced nll.
+enum { VOCAB_GREEDY = 0, VOCAB_SAMPLE = 1, VOCAB_ARGMAX = 2 };
+constexpr int VOCAB_SLICE = 1024;
+struct VocabTailArgs {
+    const float* part; int S; long long plane; int ldp;      // S planes [B][ldp], plane stride in floats
+    const float* bias; int B, V;                             // bias [V] or NULL
+    int mode, unk_idx;                                       // VOCAB_GREEDY: top-2 + UNK rule; VOCAB_ARGMAX: first maximum
+    const GvdSampleParams* par; int step;                    // VOCAB_SAMPLE: seed, temperature and decode step of the noise
+    long long *it_out, *seq_out; float* logp_out; long long out_stride;
+    const float* embed; float* xt; long long ld_xt; int E; float* xt_pk; long long ld_xt_pk;
+    float* logits_out; long long ld_logits;                  // row b's logits at logits_out + b * ld_logits
+    const long long* target; long long target_stride;        // nll[b] = lse - logit[target[b]] (0 unless 0 < target < V)
+    float* nll; long long nll_stride;
+    float* rec; int* ticket;                                 // [B][gvd_vocab_slices(V)] records; [B] tickets, zero before the first launch
+};
+inline int gvd_vocab_slices(int V) { return (V + VOCAB_SLICE - 1) / VOCAB_SLICE; }
+inline size_t gvd_vocab_rec_floats(int B, int V) { return (size_t)B * gvd_vocab_slices(V) * 8; }
+int gvd_vocab_tail(const VocabTailArgs& a, cudaStream_t st);
 int gvd_gemm_nt_tc(const GemmArgs& g, int batch, cudaStream_t stream);
 int gvd_gemm_nt_astat(const GemmArgs& g, int batch, cudaStream_t stream);   // short-K (<= 192), one K pass
 // self-attention pair (W operands pre-split into tf32 hi / lo planes): softmax-numerator scores + group factors F, then (F (.) E) V

@@ -267,6 +267,174 @@ __global__ void __launch_bounds__(PICK_NT) reduce_sample_kernel(const float* __r
     }
 }
 
+// Vocabulary head tail for any V (the two kernels above hold a whole row in one CTA's registers: at most 6 x 1024 words).
+// Grid (row b, slice j): slice j covers the words [j * VOCAB_SLICE, (j + 1) * VOCAB_SLICE), thread x the four consecutive words from
+// 4x on (one float4 per plane: ldp % 4 == 0 keeps the last group inside the row).  For sampling those four words are exactly the four
+// outputs of Philox counter (i >> 2, b, step, 0), the noise of reduce_sample_kernel.  Each CTA writes one record of its slice:
+//   m  = slice max (greedy / argmax: its top-1 value, as reduce_pick_kernel),  s = sum exp(x - m) over the slice (0 when m = -inf),
+//   greedy / argmax: v1 i1 v2 i2 = the slice's top-2;  sampling: v1 i1 = its best key and that word, v2 = the word's raw logit.
+// The last CTA of the row (ticket) merges the records in a fixed order — lane l of warp 0 takes slices l, l + 32, ... ascending, then a
+// butterfly — so the result does not depend on which CTA finishes last, and writes the token, its log-prob and the next input.
+constexpr int VT_NT = VOCAB_SLICE / 4;
+struct VocabRec { float m, s, v1, v2; int i1, i2, pad0, pad1; };
+__device__ __forceinline__ void top2_butterfly(Top2& t) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ov1 = __shfl_xor_sync(0xffffffffu, t.v1, o), ov2 = __shfl_xor_sync(0xffffffffu, t.v2, o);
+        const int oi1 = __shfl_xor_sync(0xffffffffu, t.i1, o), oi2 = __shfl_xor_sync(0xffffffffu, t.i2, o);
+        top2_insert(t, ov1, oi1);
+        top2_insert(t, ov2, oi2);
+    }
+}
+__device__ __forceinline__ void argkey_butterfly(ArgKey& a) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+        const float ok = __shfl_xor_sync(0xffffffffu, a.key, o), ol = __shfl_xor_sync(0xffffffffu, a.logit, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, a.i, o);
+        argkey_merge(a, ok, ol, oi);
+    }
+}
+template <int MODE>
+__global__ void __launch_bounds__(VT_NT) vocab_tail_kernel(const VocabTailArgs a) {
+    __shared__ float red[32];
+    __shared__ Top2 wtop[VT_NT / 32];
+    __shared__ ArgKey wbest[VT_NT / 32];
+    __shared__ int last_s, tok_s;
+    const int b = blockIdx.x, slice = blockIdx.y, nsl = gridDim.y, lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    const int i0 = slice * VOCAB_SLICE + 4 * threadIdx.x;
+    const int V = a.V;
+    pdl_trigger();
+    float g[4] = {0.f, 0.f, 0.f, 0.f};
+    float temperature = 1.f;
+    if (MODE == VOCAB_SAMPLE) {     // the noise depends on nothing the decode loop writes: drawn before waiting for the previous kernel
+        temperature = a.par->temperature;
+        if (i0 < V) {
+            uint32_t r[4];
+            philox4x32_10((uint32_t)(i0 >> 2), (uint32_t)b, (uint32_t)a.step, 0u, a.par->seed_lo, a.par->seed_hi, r);
+#pragma unroll
+            for (int j = 0; j < 4; ++j) g[j] = gumbel_from_word(r[j]);
+        }
+    }
+    pdl_wait();
+    const float* p = a.part + (long long)b * a.ldp;
+    float x[4] = {-INFINITY, -INFINITY, -INFINITY, -INFINITY};
+    if (i0 < V) {
+        float4 v = *reinterpret_cast<const float4*>(p + i0);
+        for (int s = 1; s < a.S; ++s) {                                  // ascending split order, as the other tails
+            const float4 t = *reinterpret_cast<const float4*>(p + i0 + s * a.plane);
+            v.x += t.x; v.y += t.y; v.z += t.z; v.w += t.w;
+        }
+        const float vv[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            if (i0 + j < V) {
+                x[j] = a.bias ? vv[j] + __ldg(a.bias + i0 + j) : vv[j];
+                if (a.logits_out) a.logits_out[(long long)b * a.ld_logits + i0 + j] = x[j];
+            }
+        }
+    }
+    float m;
+    Top2 t{-INFINITY, -INFINITY, 0x7fffffff, 0x7fffffff};
+    ArgKey k{-INFINITY, -INFINITY, 0x7fffffff};
+    if (MODE == VOCAB_SAMPLE) {
+        m = -INFINITY;
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (i0 + j < V) { m = fmaxf(m, x[j]); argkey_merge(k, x[j] / temperature + g[j], x[j], i0 + j); }
+        argkey_butterfly(k);
+        if (lane == 0) wbest[warp] = k;
+        m = block_max(m, red);                                           // (its barriers publish wbest)
+        k = lane < VT_NT / 32 ? wbest[lane] : ArgKey{-INFINITY, -INFINITY, 0x7fffffff};
+        argkey_butterfly(k);
+    } else {
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+            if (i0 + j < V) top2_insert(t, x[j], i0 + j);
+        top2_butterfly(t);
+        if (lane == 0) wtop[warp] = t;
+        __syncthreads();
+        t = lane < VT_NT / 32 ? wtop[lane] : Top2{-INFINITY, -INFINITY, 0x7fffffff, 0x7fffffff};
+        top2_butterfly(t);
+        m = t.v1;
+    }
+    float s = 0.f;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) s += (i0 + j < V) ? expf(x[j] - m) : 0.f;
+    s = block_sum(s, red);
+    VocabRec* rec = reinterpret_cast<VocabRec*>(a.rec) + (long long)b * nsl;
+    if (threadIdx.x == 0) {
+        if (m == -INFINITY) s = 0.f;
+        rec[slice] = MODE == VOCAB_SAMPLE ? VocabRec{m, s, k.key, k.logit, k.i, 0, 0, 0} : VocabRec{m, s, t.v1, t.v2, t.i1, t.i2, 0, 0};
+        __threadfence();                                                 // publish the record before taking a ticket
+        last_s = atomicAdd(a.ticket + b, 1) == nsl - 1;
+    }
+    __syncthreads();
+    if (!last_s) return;
+    __threadfence();
+    if (warp == 0) {
+        float M = -INFINITY;
+        t = Top2{-INFINITY, -INFINITY, 0x7fffffff, 0x7fffffff};
+        k = ArgKey{-INFINITY, -INFINITY, 0x7fffffff};
+        for (int j = lane; j < nsl; j += 32) {
+            const float4 r = __ldcg(reinterpret_cast<const float4*>(rec + j));
+            const int2 ri = __ldcg(reinterpret_cast<const int2*>(rec + j) + 2);
+            M = fmaxf(M, r.x);
+            if (MODE == VOCAB_SAMPLE) argkey_merge(k, r.z, r.w, ri.x);
+            else { top2_insert(t, r.z, ri.x); top2_insert(t, r.w, ri.y); }
+        }
+        M = warp_max(M);
+        if (MODE == VOCAB_SAMPLE) argkey_butterfly(k); else top2_butterfly(t);
+        float sum = 0.f;
+        for (int j = lane; j < nsl; j += 32) {
+            const float2 r = __ldcg(reinterpret_cast<const float2*>(rec + j));
+            if (r.x != -INFINITY) sum += r.y * expf(r.x - M);
+        }
+        sum = warp_sum(sum);
+        if (lane == 0) {
+            const float lse = M + logf(sum);
+            int it;
+            float lv;
+            if (MODE == VOCAB_SAMPLE) { it = k.i; lv = k.logit; }                 // no UNK rule when sampling (model.py:595-603)
+            else {
+                const bool keep = MODE == VOCAB_ARGMAX || t.i1 != a.unk_idx;     // misc/model.py:590-594
+                it = keep ? t.i1 : t.i2;
+                lv = keep ? t.v1 : t.v2;
+            }
+            if ((unsigned)it >= (unsigned)V) it = 0;                             // no finite comparison: stay inside the embedding table
+            if (a.it_out) a.it_out[b] = it;
+            if (a.seq_out) a.seq_out[(long long)b * a.out_stride] = it;
+            if (a.logp_out) a.logp_out[(long long)b * a.out_stride] = lv - lse;
+            if (a.nll) {                                                         // teacher forcing (transformer.py:51-54)
+                const long long tgt = a.target[(long long)b * a.target_stride];
+                float y = 0.f;
+                if (tgt > 0 && tgt < V) {                                        // the target's logit, summed in the order of the slice pass
+                    y = p[tgt];
+                    for (int s2 = 1; s2 < a.S; ++s2) y += p[tgt + s2 * a.plane];
+                    if (a.bias) y += __ldg(a.bias + tgt);
+                    y = lse - y;
+                }
+                a.nll[(long long)b * a.nll_stride] = y;
+            }
+            tok_s = it;
+            a.ticket[b] = 0;                                                     // ready for the next launch
+        }
+    }
+    if (a.xt) {                                                  // next step's input xt = ReLU(embed[token]) (model.py:79-82,605)
+        __syncthreads();
+        const float* row = a.embed + (long long)tok_s * a.E;
+        for (int e = threadIdx.x; e < a.E; e += blockDim.x) a.xt[(long long)b * a.ld_xt + e] = fmaxf(row[e], 0.f);
+        if (a.xt_pk) {                                           // and its fp16x3 operand image (E is even)
+            uint32_t* d = reinterpret_cast<uint32_t*>(a.xt_pk) + (long long)b * a.ld_xt_pk;
+            for (int e2 = threadIdx.x; 2 * e2 < a.E; e2 += blockDim.x) {
+                uint32_t hi, lo;
+                f16x3_split_pair(fmaxf(row[2 * e2], 0.f), fmaxf(row[2 * e2 + 1], 0.f), GVD_F16_SA, hi, lo);
+                const long long w = f16x3_word(2 * e2);
+                d[w] = hi; d[w + 16] = lo;
+            }
+        }
+    }
+}
+
 }  // namespace
 
 // Number of K splits for a skinny product with Nw weight rows and Ktot columns (0 = shape not supported by this path):
@@ -339,6 +507,23 @@ int gvd_reduce_sample(const float* part, int S, int ldp, const float* bias, int 
     if (V <= PICK_NT * 2) GVD_CHECK_CUDA(gvd_launch(reduce_sample_kernel<2>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, params, step, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, xt_pk, ld_xt_pk, GVD_F16_SA));
     else if (V <= PICK_NT * 5) GVD_CHECK_CUDA(gvd_launch(reduce_sample_kernel<5>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, params, step, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, xt_pk, ld_xt_pk, GVD_F16_SA));
     else GVD_CHECK_CUDA(gvd_launch(reduce_sample_kernel<6>, dim3(B), dim3(PICK_NT), 0, st, part, S, plane, ldp, bias, V, params, step, it_out, seq_out, logp_out, out_stride, embed, xt, ld_xt, E, xt_pk, ld_xt_pk, GVD_F16_SA));
+    GVD_CHECK_LAUNCH();
+    return 0;
+}
+
+int gvd_vocab_tail(const VocabTailArgs& a, cudaStream_t st) {
+    GVD_REQUIRE(a.part && a.S >= 1 && a.B >= 1 && a.V >= 2 && a.ldp >= a.V && a.ldp % 4 == 0 && a.plane % 4 == 0 && ((uintptr_t)a.part & 15) == 0,
+                "vocab_tail: partial planes need V >= 2, a 4-multiple pitch >= V and 16-byte alignment (V=%d ldp=%d)", a.V, a.ldp);
+    GVD_REQUIRE(gvd_vocab_slices(a.V) <= 65535, "vocab_tail: vocabulary of at most %d words (got %d)", 65535 * VOCAB_SLICE, a.V);
+    GVD_REQUIRE(a.rec && ((uintptr_t)a.rec & 15) == 0 && a.ticket, "vocab_tail: records and tickets needed");
+    GVD_REQUIRE(a.mode == VOCAB_GREEDY || a.mode == VOCAB_ARGMAX || (a.mode == VOCAB_SAMPLE && a.par && a.step >= 0), "vocab_tail: bad mode %d", a.mode);
+    GVD_REQUIRE((!a.xt || a.embed) && (!a.nll || a.target), "vocab_tail: xt needs the embedding, nll the targets");
+    GVD_REQUIRE(!a.xt_pk || (a.xt && a.E % 2 == 0 && a.ld_xt_pk % 32 == 0 && a.ld_xt_pk >= (a.E + 31) / 32 * 32),
+                "vocab_tail: the packed xt needs an even E and a 32-multiple pitch covering E");
+    const dim3 grid(a.B, gvd_vocab_slices(a.V));
+    if (a.mode == VOCAB_GREEDY) GVD_CHECK_CUDA(gvd_launch(vocab_tail_kernel<VOCAB_GREEDY>, grid, dim3(VT_NT), 0, st, a));
+    else if (a.mode == VOCAB_SAMPLE) GVD_CHECK_CUDA(gvd_launch(vocab_tail_kernel<VOCAB_SAMPLE>, grid, dim3(VT_NT), 0, st, a));
+    else GVD_CHECK_CUDA(gvd_launch(vocab_tail_kernel<VOCAB_ARGMAX>, grid, dim3(VT_NT), 0, st, a));
     GVD_CHECK_LAUNCH();
     return 0;
 }

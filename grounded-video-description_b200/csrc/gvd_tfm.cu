@@ -27,6 +27,7 @@ namespace {
 constexpr int TFM_MAX_HEADS = 8;
 constexpr int TFM_MAX_L = 64;          // self-attention positions held in shared memory
 constexpr int TFM_RC = 64;             // encoder rows per CTA of the attention stream (upper bound)
+constexpr int TFM_HEAD_MAXV = 12000;   // tfm_head_kernel holds a logit row in shared memory; above this the sliced tail runs
 
 // x0[b, :] = pe[t, :] + out_w[tok, :] * sqrt(d_model)       (transformer.py:222-231; two roundings as in the reference: fp32 product, then sum)
 // tok[b] = tok_src[b * tok_stride + tok_off], or 0 (<bos>) when tok_src is null
@@ -355,6 +356,7 @@ struct TfmWs {
     float *wqkv[2];                       // [Wq; Wk; Wv] of the self-attention, one product per layer and step
     float *Kc[2], *Vc[2], *Ke[2], *Ve[2];
     float *part_acc, *part_ml, *nll;
+    float* vt_rec; int* vt_ticket;        // vocabularies above 12000 words: records and tickets of the sliced head tail (gvd_vocab_tail)
     long long* out_seq;                   // graph replay: the prediction lands here (fixed address), then is copied to the caller's tensor
     // conversion-free products (backend bit 4): fp16x3 operand images of the 13 weight matrices (packed once per batch by tfm_run) and of the
     // current product's activation rows; null when a contraction length is not a multiple of 32
@@ -408,6 +410,10 @@ TfmWs tfm_layout(const gvd_tfm_weights_t* w, int B, int L, const int n[2], void*
     s.part_ml = take((size_t)B * cmax * 2 * TFM_MAX_HEADS);
     s.nll = take((size_t)B * L);
     s.out_seq = reinterpret_cast<long long*>(take((size_t)B * L * 2));
+    if (V > TFM_HEAD_MAXV) {
+        s.vt_rec = take(gvd_vocab_rec_floats(B, V));
+        s.vt_ticket = reinterpret_cast<int*>(take((size_t)B));
+    }
     if (H % 32 == 0 && DH % 32 == 0 && B <= 128) {
         const size_t HH = (size_t)H * H;
         for (int l = 0; l < 2; ++l) {
@@ -429,7 +435,8 @@ int tfm_check(const gvd_tfm_weights_t* w, int B, int L, int n0, int n1) {
     GVD_REQUIRE(w->d_hidden >= 4 && w->d_hidden % 4 == 0, "tfm: d_hidden must be a multiple of 4 (got %d)", w->d_hidden);
     GVD_REQUIRE(w->n_heads >= 1 && w->n_heads <= TFM_MAX_HEADS, "tfm: 1..%d heads (got %d)", TFM_MAX_HEADS, w->n_heads);
     GVD_REQUIRE((H + w->n_heads - 1) / w->n_heads >= 4, "tfm: heads narrower than 4 columns are not supported (d_model %d, %d heads)", H, w->n_heads);
-    GVD_REQUIRE(w->vocab_size >= 2 && w->vocab_size <= 12000, "tfm: vocab_size must be in [2, 12000] (got %d)", w->vocab_size);
+    GVD_REQUIRE(w->vocab_size >= 2 && w->vocab_size <= 65535 * VOCAB_SLICE, "tfm: vocab_size must be in [2, %d] (got %d)", 65535 * VOCAB_SLICE,
+                w->vocab_size);
     GVD_REQUIRE(B >= 1 && L >= 1 && L <= TFM_MAX_L && n0 >= 1 && n1 >= 1, "tfm: bad sizes B=%d L=%d n0=%d n1=%d (L <= %d)", B, L, n0, n1, TFM_MAX_L);
     return 0;
 }
@@ -556,6 +563,7 @@ static int tfm_run(const gvd_tfm_weights_t* w, int B, int L, const float* enc0, 
         }
     }
     if (s.ximg && tfm_f16()) GVD_TRY(gvd_pack_f16x3(w->out_w, H, w->vocab_size, H, s.wi_out, H, st, GVD_F16_SW));
+    if (s.vt_ticket) GVD_CHECK_CUDA(cudaMemsetAsync(s.vt_ticket, 0, (size_t)B * sizeof(int), st));    // the tail resets them after each use
     if (!teacher && !logits_out && tfm_graph_ok()) return tfm_loop_graph(w, s, B, L, n0, n1, pe, workspace, seq_out, st);
     return tfm_loop(w, s, B, L, n0, n1, pe, seq_out, logits_out, teacher, loss_out, st);
 }
@@ -611,9 +619,20 @@ static int tfm_loop(const gvd_tfm_weights_t* w, const TfmWs& s, int B, int L, in
         }
         const int ldv = rup4i(V);
         GVD_TRY(tfm_product(w->out_w, V, H, s.x, H, B, s.part, ldv, &S, st, s.wi_out, s.ximg, ix));
-        tfm_head_kernel<256><<<B, 256, (size_t)V * sizeof(float), st>>>(s.part, S, (long long)B * ldv, ldv, w->out_b, V, (long long*)seq_out, L, t, logits_out,
-                                                                      (const long long*)teacher, s.nll);
-        GVD_CHECK_LAUNCH();
+        if (V <= TFM_HEAD_MAXV) {
+            tfm_head_kernel<256><<<B, 256, (size_t)V * sizeof(float), st>>>(s.part, S, (long long)B * ldv, ldv, w->out_b, V, (long long*)seq_out, L, t,
+                                                                          logits_out, (const long long*)teacher, s.nll);
+            GVD_CHECK_LAUNCH();
+        } else {                  // one CTA per (clip, 1024 words), the last CTA of each clip merges
+            VocabTailArgs a{};
+            a.part = s.part; a.S = S; a.plane = (long long)B * ldv; a.ldp = ldv; a.bias = w->out_b; a.B = B; a.V = V; a.mode = VOCAB_ARGMAX;
+            a.seq_out = seq_out ? (long long*)seq_out + t : nullptr; a.out_stride = L;
+            a.logits_out = logits_out ? logits_out + (size_t)t * V : nullptr; a.ld_logits = (long long)L * V;
+            a.target = teacher ? (const long long*)teacher + t + 1 : nullptr; a.target_stride = L + 1;
+            a.nll = teacher ? s.nll + t : nullptr; a.nll_stride = L;
+            a.rec = s.vt_rec; a.ticket = s.vt_ticket;
+            GVD_TRY(gvd_vocab_tail(a, st));
+        }
     }
     if (teacher) {
         tfm_loss_kernel<256><<<1, 256, 0, st>>>(s.nll, (const long long*)teacher, B, L, loss_out);

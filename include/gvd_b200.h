@@ -121,7 +121,7 @@ GVD_API int gvd_decode_greedy(gvd_model_t* m, int B, int T, void* workspace, siz
  * key = seed) — the token follows softmax(logit / temperature), the distribution torch.multinomial draws from.  logprobs_out holds the
  * UNTEMPERED log-softmax of the drawn word (model.py:602); there is no UNK rule.  The 23-bit uniforms bound g to [-2.82, 16.64]: a word
  * whose key is more than ~19.5 below the best is never drawn (probability < 1e-8).  b is the row's index in this call, so splitting a batch
- * changes the draws.  A row whose keys are all -inf or all NaN yields token 0.  temperature: finite and > 0; vocab_size <= 6144.
+ * changes the draws.  A row whose keys are all -inf or all NaN yields token 0.  temperature: finite and > 0.
  * The seed and temperature travel in a workspace-resident parameter block, so the captured loop is replayed, not re-captured, for new ones. */
 GVD_API int gvd_decode_sample(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes,
                       const uint8_t* pnt_mask,      /* [B,R+1]                     */
@@ -254,6 +254,16 @@ GVD_API int gvd_op_greedy_pick(const float* logits, int64_t ld, int B, int V, in
 GVD_API int gvd_op_reduce_sample(const float* part, int S, int ldp, const float* bias, int B, int V, float temperature, uint64_t seed, int step,
                   int64_t* it_out, int64_t* seq_out, float* logp_out, int64_t out_stride, const float* embed, float* xt, int64_t ld_xt, int E,
                   float* xt_pk, int64_t ld_xt_pk, void* stream);
+/* the vocabulary tail for any V (2 <= V <= 65535 * 1024), the one the decode loops run above 6144 words: one CTA per (row, 1024 words) writes
+ * a record of its slice, the last CTA of the row merges the records in a fixed order.  mode GVD_VOCAB_GREEDY: top-2 + UNK rule as
+ * reduce_pick; GVD_VOCAB_SAMPLE: the draw of reduce_sample at (temperature, seed, step); GVD_VOCAB_ARGMAX: the first maximum (transformer
+ * head).  ldp % 4 == 0, part 16-byte aligned; logits_out (or NULL) receives the summed logits at pitch ld_logits. */
+#define GVD_VOCAB_GREEDY 0
+#define GVD_VOCAB_SAMPLE 1
+#define GVD_VOCAB_ARGMAX 2
+GVD_API int gvd_op_reduce_pick_split(const float* part, int S, int ldp, const float* bias, int B, int V, int mode, int unk_idx, float temperature,
+                  uint64_t seed, int step, int64_t* it_out, int64_t* seq_out, float* logp_out, int64_t out_stride, const float* embed, float* xt,
+                  int64_t ld_xt, int E, float* logits_out, int64_t ld_logits, float* xt_pk, int64_t ld_xt_pk, void* stream);
 /* vocabulary head h [B,K] . W [V,K]^T + bias with the sampler in the GEMM epilogue; B <= 128, E % 4 == 0, xt [B,E] */
 GVD_API int gvd_op_logit_pick_tc(const float* h, int64_t ldh, const float* W, int64_t ldw, const float* bias, int B, int V, int K, int unk_idx,
                   const float* embed, int E, int64_t* it_out, int64_t* seq_out, float* logp_out, int64_t out_stride, float* xt, void* stream);
