@@ -483,6 +483,61 @@ __global__ void __launch_bounds__(256) adam_flat_kernel(float* __restrict__ w, f
         w[i] = ww - (lr / bc1) * (mm / denom);
     }
 }
+// torch.optim.SGD (momentum mu, dampening 0, nesterov off) over the flat buffers, same segment layout / lr rule / in-place clipping as
+// adam_flat_kernel.  torch keeps the momentum buffer per parameter and creates it on the tensor's first step (buf = d); seg_step[s] = the
+// steps segment s has taken before this one (advanced by seg_step_advance_kernel after this launch).
+__global__ void __launch_bounds__(256) sgd_flat_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ buf, long long n,
+                                                       const long long* __restrict__ seg_end, const float* __restrict__ seg_lr,
+                                                       const int* __restrict__ seg_step, int nseg, const float* __restrict__ norm, float mu,
+                                                       float wd) {
+    const float coef = norm ? norm[1] : 1.f;
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        int lo = 0, hi = nseg - 1;
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (seg_end[mid] > i) hi = mid; else lo = mid + 1; }
+        const float lr = seg_lr[lo];
+        float d = g[i] * coef;
+        g[i] = d;
+        if (lr <= 0.f) continue;
+        const float ww = w[i];
+        if (wd != 0.f) d = fmaf(wd, ww, d);
+        const float b = seg_step[lo] == 0 ? d : fmaf(mu, buf[i], d);
+        buf[i] = b;
+        w[i] = ww - lr * b;
+    }
+}
+// torch.optim.Adamax (single-tensor arithmetic): exp_avg m = b1 m + (1 - b1) d, exp_inf u = max(b2 u, |d| + eps),
+// w -= lr / (1 - b1^t) * m / u with t the segment's own step count (seg_step[s] + 1).  Layout and idle rule as adam_flat_kernel.
+__global__ void __launch_bounds__(256) adamax_flat_kernel(float* __restrict__ w, float* __restrict__ g, float* __restrict__ m, float* __restrict__ u,
+                                                          long long n, const long long* __restrict__ seg_end, const float* __restrict__ seg_lr,
+                                                          const int* __restrict__ seg_step, int nseg, const float* __restrict__ norm, float b1,
+                                                          float b2, float eps, float wd) {
+    const float coef = norm ? norm[1] : 1.f;
+    int cur = -1;
+    float clr = 0.f;                                     // lr / (1 - b1^t) of segment `cur`
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        int lo = 0, hi = nseg - 1;
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (seg_end[mid] > i) hi = mid; else lo = mid + 1; }
+        const float lr = seg_lr[lo];
+        float d = g[i] * coef;
+        g[i] = d;
+        if (lr <= 0.f) continue;
+        if (lo != cur) {                                 // torch: bias_correction = 1 - beta1 ** step in double
+            cur = lo;
+            clr = (float)((double)lr / (1.0 - pow((double)b1, (double)(seg_step[lo] + 1))));
+        }
+        const float ww = w[i];
+        if (wd != 0.f) d = fmaf(wd, ww, d);
+        const float mm = b1 * m[i] + (1.f - b1) * d;
+        const float uu = fmaxf(b2 * u[i], fabsf(d) + eps);
+        m[i] = mm; u[i] = uu;
+        w[i] = ww - clr * (mm / uu);
+    }
+}
+// seg_step[s] += 1 for every segment that stepped (lr > 0): after the update launch, so that all of it read the old count
+__global__ void seg_step_advance_kernel(int* __restrict__ seg_step, const float* __restrict__ seg_lr, int nseg) {
+    const int s = blockIdx.x * blockDim.x + threadIdx.x;
+    if (s < nseg && seg_lr[s] > 0.f) seg_step[s] += 1;
+}
 
 // ---------------------------------------------------------------- dropout: counter-based masks (Philox4x32-10), nothing stored
 // Element i of a tensor at dropout site `site` in optimisation step `step` draws word (i & 3) of Philox(counter = (i >> 2, site, step_lo,
@@ -711,6 +766,24 @@ GVD_API int gvd_tr_adam_flat(float* w, float* g, float* m, float* v, long long n
     GVD_REQUIRE(w && g && m && v && seg_end && seg_lr && nseg >= 1 && n > 0 && t >= 1, "tr_adam_flat: bad arguments");
     const float bc1 = (float)(1.0 - pow((double)b1, (double)t)), bc2s = (float)sqrt(1.0 - pow((double)b2, (double)t));
     adam_flat_kernel<<<132 * 8, 256, 0, ST(st)>>>(w, g, m, v, n, (const long long*)seg_end, seg_lr, nseg, norm, b1, b2, eps, weight_decay, bc1, bc2s);
+    LAUNCH_OK();
+}
+// One SGD-with-momentum step on the flat buffers (see sgd_flat_kernel), then seg_step[s] += 1 for the segments with lr > 0.
+GVD_API int gvd_tr_sgd_flat(float* w, float* g, float* buf, long long n, const int64_t* seg_end, const float* seg_lr, int* seg_step, int nseg,
+                            const float* norm, float momentum, float weight_decay, void* st) {
+    GVD_REQUIRE(w && g && buf && seg_end && seg_lr && seg_step && nseg >= 1 && n > 0, "tr_sgd_flat: bad arguments");
+    sgd_flat_kernel<<<132 * 8, 256, 0, ST(st)>>>(w, g, buf, n, (const long long*)seg_end, seg_lr, seg_step, nseg, norm, momentum, weight_decay);
+    GVD_CHECK_LAUNCH();
+    seg_step_advance_kernel<<<gvd_cdiv(nseg, TB), TB, 0, ST(st)>>>(seg_step, seg_lr, nseg);
+    LAUNCH_OK();
+}
+// One Adamax step on the flat buffers (see adamax_flat_kernel), then seg_step[s] += 1 for the segments with lr > 0.
+GVD_API int gvd_tr_adamax_flat(float* w, float* g, float* m, float* u, long long n, const int64_t* seg_end, const float* seg_lr, int* seg_step,
+                               int nseg, const float* norm, float b1, float b2, float eps, float weight_decay, void* st) {
+    GVD_REQUIRE(w && g && m && u && seg_end && seg_lr && seg_step && nseg >= 1 && n > 0, "tr_adamax_flat: bad arguments");
+    adamax_flat_kernel<<<132 * 8, 256, 0, ST(st)>>>(w, g, m, u, n, (const long long*)seg_end, seg_lr, seg_step, nseg, norm, b1, b2, eps, weight_decay);
+    GVD_CHECK_LAUNCH();
+    seg_step_advance_kernel<<<gvd_cdiv(nseg, TB), TB, 0, ST(st)>>>(seg_step, seg_lr, nseg);
     LAUNCH_OK();
 }
 // C[z] = A[z] W[z]^T  (A [batch, M, K], W [batch, N, K], C [batch, M, N]; row pitches lda / ldw / ldc, batch strides in elements)

@@ -59,6 +59,19 @@ TFM_DROP_SITES = {n: len(DROP_SITES) + i for i, n in enumerate(("tfm_embed", "tf
 _SITE_IDS = dict(DROP_SITES, **TFM_DROP_SITES)
 
 
+def check_disable_caption(opt):
+    """True when the language loss is part of the objective.  opt.disable_caption (main.py:243-246) drops it; the reference cannot step
+    when nothing is left: with w_att2 = w_grd = w_cls = 0 its loss stays the Python int 0 (no .backward()), and the transformer captioner's
+    other three losses are constants without a graph (model.py:418-419)."""
+    if not getattr(opt, "disable_caption", False):
+        return True
+    if getattr(opt, "att_model", "topdown") == "transformer":
+        raise ValueError("disable_caption with att_model='transformer': the captioner's only loss with a gradient is the language loss")
+    if not (opt.w_att2 or opt.w_grd or opt.w_cls):
+        raise ValueError("disable_caption with w_att2 = w_grd = w_cls = 0: the training objective is empty")
+    return False
+
+
 class TrainStep:
     """forward_backward(W, opt, inp) -> (losses[4], loss, grads{key});  step(...) adds clip + Adam (first step, main.py:660-677).
 
@@ -483,7 +496,10 @@ class TrainStep:
             # gradient at all (None in the reference: Adam skips it)
             region_grad = not featmap or bool(w_att2) or bool(w_grd)
             # ========================================================== backward, loss heads
-            douts = self._lin_bwd(ops.scale(dlogits, w_lm), outs_t, W, "logit", grads)
+            # w_lm = 0 (disable_caption, main.py:243-246): the logit head gets no gradient (None in the reference).  Everything else still
+            # gets one, exact zeros where only the language loss reached it: the reference's decode state is torch.stack([h_att, h_lang])
+            # (AttModel.py:163), so the next step's h_att = state[0][0] carries a zero gradient into h_lang, the language LSTM and its inputs.
+            douts = self._lin_bwd(ops.scale(dlogits, w_lm), outs_t, W, "logit", grads) if w_lm else ops.zeros(tuple(outs_t.shape))
             dz_all = ops.zeros(tuple(z_all.shape))
             dg_pool = ops.zeros(tuple(g_pool.shape))
             if w_att2:
@@ -662,20 +678,22 @@ class TrainStep:
         return [lm, zero, zero, zero], backward
 
     def forward_backward(self, W, opt, inp, n_replicas=1, host=None):
-        """loss = (lm + w_att2 att2 + w_grd grd + w_cls cls) / n_replicas with the zero-weight terms dropped (main.py:238-255)."""
+        """loss = (lm + w_att2 att2 + w_grd grd + w_cls cls) / n_replicas with the zero-weight terms dropped (main.py:238-255).
+        opt.disable_caption (main.py:243-246): the language loss leaves the objective and the returned lm is 0; the logit head gets no
+        gradient (absent from `grads`), the tensors only the language loss reached get exact zeros, as in the reference."""
         ops = self.ops
+        caption = check_disable_caption(opt)
         losses, backward = self.forward(W, opt, inp, host)
         lm, att2_loss, grd_loss, cls_loss = losses
-        loss = lm
-        if opt.w_att2:
-            loss = ops.add(loss, ops.scale(att2_loss, opt.w_att2))
-        if opt.w_grd:
-            loss = ops.add(loss, ops.scale(grd_loss, opt.w_grd))
-        if opt.w_cls:
-            loss = ops.add(loss, ops.scale(cls_loss, opt.w_cls))
+        loss = lm if caption else None
+        for w, l in ((opt.w_att2, att2_loss), (opt.w_grd, grd_loss), (opt.w_cls, cls_loss)):
+            if w:
+                loss = ops.scale(l, w) if loss is None else ops.add(loss, ops.scale(l, w))
         loss = ops.scale(loss, 1.0 / n_replicas)
         c0 = 1.0 / n_replicas
-        grads = backward(c0, opt.w_att2 * c0, opt.w_grd * c0, opt.w_cls * c0)
+        grads = backward(c0 if caption else 0.0, opt.w_att2 * c0, opt.w_grd * c0, opt.w_cls * c0)
+        if not caption:
+            losses = [ops.zeros((1,)), att2_loss, grd_loss, cls_loss]          # lm_loss.fill_(0), main.py:246
         return losses, loss, grads
 
     def step(self, W, opt, inp, lr=5e-4, betas=(0.9, 0.999), eps=1e-8, grad_clip=0.1, n_replicas=1, host=None, all_reduce=None):
@@ -717,15 +735,29 @@ class Trainer:
                      count like main.py:255, so the sum is nn.DataParallel's averaged gradient)
         gvd_tr_grad_norm  (global norm + clip coefficient, stays on the device)   -> clip_grad_norm_(grad_clip)   main.py:265
         gvd_tr_adam_flat  (torch.optim.Adam arithmetic, per-tensor lr table, step t) -> optimizer.step()          main.py:266
+          (optim = 'sgd' / 'adamax': gvd_tr_sgd_flat / gvd_tr_adamax_flat, torch.optim.SGD(momentum=0.9) / Adamax, main.py:671-677)
         BatchNorm running statistics (train-mode side effect of model.py:114; rank-local like DataParallel's replica 0)
 
     `W` (the dict handed out by `.weights`) holds VIEWS into `flat_w`, so a module whose parameters are re-pointed at them
     (`adopt_module`) trains in place.  Tensors that receive no gradient keep lr 0 in the table and come out of a step unchanged, as
     torch.optim.Adam skips them: core.i2h_2 / h2h_2 (quirk Q10) from the start, and whatever else the last backward left out (with
-    att_model = 'transformer': the top-down core, its embedding and heads, and the branch att_input_mode does not read)."""
+    att_model = 'transformer': the top-down core, its embedding and heads, and the branch att_input_mode does not read; with
+    opt.disable_caption: the logit head).
+
+    optim: 'adam' (default), 'sgd' or 'adamax' — the three optimisers of main.py:671-677, with the same param groups, lr, weight_decay and betas
+    (main.py:660-669; SGD ignores betas, as torch does).  The optimiser state lives in `flat_m` (Adam exp_avg, SGD momentum_buffer, Adamax
+    exp_avg) and `flat_v` (Adam exp_avg_sq, Adamax exp_inf).  SGD and Adamax keep torch's per-tensor step count in `seg_step` (device int32,
+    one entry per tensor), so a tensor's momentum buffer / bias correction starts with its own first gradient."""
+
+    OPTIMS = ("adam", "sgd", "adamax")
+    SGD_MOMENTUM = 0.9                                             # optim.SGD(params, momentum=0.9), main.py:673
 
     def __init__(self, ops, state_dict, opt, lr=5e-4, betas=(0.9, 0.999), eps=1e-8, weight_decay=0.0, grad_clip=0.1, all_reduce=None,
-                 n_replicas=1):
+                 n_replicas=1, optim="adam"):
+        if optim not in self.OPTIMS:
+            raise ValueError("optim must be one of %s (main.py:671-677), got %r" % (", ".join(repr(o) for o in self.OPTIMS), optim))
+        check_disable_caption(opt)
+        self.optim = optim
         self.ops, self.opt = ops, opt
         self.step_fn = TrainStep(ops)
         self.lr, self.betas, self.eps, self.weight_decay, self.grad_clip = lr, betas, eps, weight_decay, grad_clip
@@ -755,6 +787,7 @@ class Trainer:
         self.buffers = {k: state_dict[k].detach().clone().to(dev) for k in state_dict if k not in self.weights}
         ends = [offs[k] + (state_dict[k].numel() + 3) // 4 * 4 for k in self.keys]
         self.seg_end = torch.tensor(ends, dtype=torch.int64, device=dev)
+        self.seg_step = torch.zeros(len(self.keys), dtype=torch.int32, device=dev)
         self.set_lr(lr)
 
     def set_lr(self, lr):
@@ -807,13 +840,20 @@ class Trainer:
         return losses, loss
 
     def apply(self):
-        """clip_grad_norm_ + Adam on the flat buffers + the BatchNorm running statistics of the last forward."""
+        """clip_grad_norm_ + the optimiser step on the flat buffers + the BatchNorm running statistics of the last forward."""
         ops = self.ops
         self.t += 1
         ops.grad_norm_(self.flat_g, self.grad_clip, self.norm)
-        ops.adam_flat_(self.flat_w, self.flat_g, self.flat_m, self.flat_v, self.seg_end, self.seg_lr, self.norm, self.betas[0], self.betas[1],
-                       self.eps, self.weight_decay, self.t)
-        # the Adam kernel writes the weights behind torch's back: bump the version counters of adopted modules' parameters, so that
+        if self.optim == "adam":
+            ops.adam_flat_(self.flat_w, self.flat_g, self.flat_m, self.flat_v, self.seg_end, self.seg_lr, self.norm, self.betas[0], self.betas[1],
+                           self.eps, self.weight_decay, self.t)
+        elif self.optim == "sgd":
+            ops.sgd_flat_(self.flat_w, self.flat_g, self.flat_m, self.seg_end, self.seg_lr, self.seg_step, self.norm, self.SGD_MOMENTUM,
+                          self.weight_decay)
+        else:
+            ops.adamax_flat_(self.flat_w, self.flat_g, self.flat_m, self.flat_v, self.seg_end, self.seg_lr, self.seg_step, self.norm, self.betas[0],
+                             self.betas[1], self.eps, self.weight_decay)
+        # the optimiser kernel writes the weights behind torch's back: bump the version counters of adopted modules' parameters, so that
         # code keyed on them (the module's cached native weights, AttModel._native_model) sees the new values
         for m in self._adopted:
             for k, p in m.named_parameters():

@@ -6,6 +6,10 @@
 four losses, its backward receives their four upstream gradients — the weights of the caller's combination — and runs the
 hand-written backward ONCE with those weights (it is linear in them), handing every parameter its gradient.
 
+A loss without `lm` (--disable_caption, main.py:243-246) reaches backward with g_lm = 0: the logit head's .grad stays None, and the tensors
+only the language loss reached get exact-zero gradients rather than None, as in the reference, whose decode state torch.stack([h_att, h_lang])
+(AttModel.py:163) carries a zero gradient into the language LSTM.
+
 Verified on the CPU with the torch mock of the primitives (tests/test_train_host_logic.py) and on the device (tests/test_gpu_zz_train.py)."""
 import torch
 

@@ -51,6 +51,8 @@ _SIGS = {
     "gvd_tr_dropout": [_vp, _vp, _ll, _cf, _ll, _ci, _ll, _vp],
     "gvd_tr_grad_norm": [_vp, _ll, _cf, _vp, _vp, _vp],
     "gvd_tr_adam_flat": [_vp, _vp, _vp, _vp, _ll, _vp, _vp, _ci, _vp, _cf, _cf, _cf, _cf, _ci, _vp],
+    "gvd_tr_sgd_flat": [_vp, _vp, _vp, _ll, _vp, _vp, _vp, _ci, _vp, _cf, _cf, _vp],
+    "gvd_tr_adamax_flat": [_vp, _vp, _vp, _vp, _ll, _vp, _vp, _vp, _ci, _vp, _cf, _cf, _cf, _cf, _vp],
     "gvd_tr_gemm_nt_batched": [_vp, _ll, _ll, _vp, _ll, _ll, _vp, _ll, _ll, _ci, _ci, _ci, _ci, _vp],
     "gvd_tr_transpose": [_vp, _vp, _ci, _ci, _ci, _vp],
     "gvd_tr_mha_fwd": [_vp, _vp, _vp, _vp, _vp, _ci, _ci, _ci, _ci, _ci, _cf, _cf, _ll, _ci, _ll, _vp],
@@ -433,6 +435,17 @@ class NativeOps:
         capi.check(self.L.gvd_tr_adam_flat(_p(w), _p(g), _p(m), _p(v), w.numel(), _p(seg_end), _p(seg_lr), seg_end.numel(),
                                            _p(norm) if norm is not None else None, float(b1), float(b2), float(eps), float(weight_decay), int(t),
                                            self._st()))
+
+    def sgd_flat_(self, w, g, buf, seg_end, seg_lr, seg_step, norm, momentum, weight_decay):
+        """One torch.optim.SGD(momentum) step on flat buffers, in place (w, buf, seg_step updated; g clipped by norm[1])."""
+        capi.check(self.L.gvd_tr_sgd_flat(_p(w), _p(g), _p(buf), w.numel(), _p(seg_end), _p(seg_lr), _p(seg_step), seg_end.numel(),
+                                          _p(norm) if norm is not None else None, float(momentum), float(weight_decay), self._st()))
+
+    def adamax_flat_(self, w, g, m, u, seg_end, seg_lr, seg_step, norm, b1, b2, eps, weight_decay):
+        """One torch.optim.Adamax step on flat buffers, in place (w, m, u, seg_step updated; g clipped by norm[1])."""
+        capi.check(self.L.gvd_tr_adamax_flat(_p(w), _p(g), _p(m), _p(u), w.numel(), _p(seg_end), _p(seg_lr), _p(seg_step), seg_end.numel(),
+                                             _p(norm) if norm is not None else None, float(b1), float(b2), float(eps), float(weight_decay),
+                                             self._st()))
 
     # ---- integer / mask targets of the teacher forcing, on the device (gvd_losses.cu kernels)
     def host_targets(self, step, opt, inp, host):

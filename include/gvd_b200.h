@@ -395,6 +395,19 @@ GVD_API size_t gvd_tr_sumsq_scratch_bytes(void);
 GVD_API int gvd_tr_grad_norm(const float* g, long long n, float max_norm, void* scratch, float* norm_out /* [2]: norm, clip coef */, void* stream);
 GVD_API int gvd_tr_adam_flat(float* w, float* g, float* m, float* v, long long n, const int64_t* seg_end, const float* seg_lr, int nseg,
                              const float* norm, float b1, float b2, float eps, float weight_decay, int t, void* stream);
+/* The other two optimisers main.py:671-677 builds (--optim sgd | adamax), on the same flat layout as gvd_tr_adam_flat: segment s covers
+   [seg_end[s-1], seg_end[s]) with learning rate seg_lr[s] (lr <= 0: the tensor got no gradient and is left bit-identical, state included), g
+   is scaled in place by the clip coefficient norm[1] (null: 1).  torch keeps optimiser state per parameter, so seg_step[s] (int32, device) is
+   the number of steps segment s has taken; each call advances it for the segments with lr > 0, after the update.
+   gvd_tr_sgd_flat:    torch.optim.SGD(momentum, dampening=0, nesterov=False, weight_decay):  d = g coef + wd w;  buf = d on the segment's
+                       first step, else buf = momentum buf + d;  w -= lr buf.  (main.py:673 builds it with momentum = 0.9.)
+   gvd_tr_adamax_flat: torch.optim.Adamax(betas=(b1, b2), eps, weight_decay):  d = g coef + wd w;  m = b1 m + (1 - b1) d;
+                       u = max(b2 u, |d| + eps);  w -= lr / (1 - b1^t) m / u,  t = seg_step[s] + 1.  (main.py:677, betas = optim_alpha /
+                       optim_beta of main.py:666-669.) */
+GVD_API int gvd_tr_sgd_flat(float* w, float* g, float* buf, long long n, const int64_t* seg_end, const float* seg_lr, int* seg_step, int nseg,
+                            const float* norm, float momentum, float weight_decay, void* stream);
+GVD_API int gvd_tr_adamax_flat(float* w, float* g, float* m, float* u, long long n, const int64_t* seg_end, const float* seg_lr, int* seg_step,
+                               int nseg, const float* norm, float b1, float b2, float eps, float weight_decay, void* stream);
 GVD_API int gvd_tr_count_inv(const void* data, long long n, int elem_bytes /* 1: bytes != 0, 4: int32 > 0 */, float* inv_out, void* stream);   /* 1 / count on the device */
 GVD_API int gvd_tr_scalar_mul(const float* a, const float* b, float* out, void* stream);
 GVD_API int gvd_tr_outer_rows_acc(const float* a, const float* v, float* acc, int B, int N, int H, void* stream);   /* acc[b,n,:] += a[b,n] v[b,:] */
