@@ -24,6 +24,7 @@ EXPORTS = [
     "gvd_op_row_argmax", "gvd_op_beam_search_scripted", "gvd_op_scores_tc", "gvd_op_self_attention_tc", "gvd_op_self_attention_fused", "gvd_op_lstm_step", "gvd_set_backend", "gvd_get_backend",
     "gvd_tfm_workspace_bytes", "gvd_tfm_decode_greedy", "gvd_tfm_teacher_fwd",
     "gvd_grounding_extract", "gvd_grounding_eval", "gvd_plan_skinny_splits", "gvd_plan_h2d_chunks", "gvd_workspace_bytes_beam", "gvd_beam_decode", "gvd_workspace_bytes_teacher", "gvd_teacher_fwd",
+    "gvd_workspace_bytes_video", "gvd_prologue_fwd_video", "gvd_sample_greedy_host_video", "gvd_op_attention_video",
     # training-step primitives (csrc/gvd_train.cu; bound in train_ops.py)
     "gvd_tr_adam_first_step", "gvd_tr_adam_flat", "gvd_tr_sgd_flat", "gvd_tr_adamax_flat", "gvd_tr_grad_norm", "gvd_tr_sumsq_scratch_bytes", "gvd_tr_att_scores_bwd", "gvd_tr_att_scores_fwd", "gvd_tr_att_scores_mul_bwd", "gvd_tr_att_scores_mul_fwd", "gvd_tr_bn_bwd", "gvd_tr_bn_normalize", "gvd_tr_cls_nll", "gvd_tr_colsum", "gvd_tr_count_inv", "gvd_tr_scalar_mul", "gvd_tr_dropout", "gvd_tr_ew", "gvd_tr_gather_rows", "gvd_tr_gemm_nt_batched", "gvd_tr_gru_cell_bwd", "gvd_tr_gru_cell_fwd", "gvd_tr_index_add_rows", "gvd_tr_lm_nll", "gvd_tr_ln_bwd", "gvd_tr_ln_fwd", "gvd_tr_ln_star_bwd", "gvd_tr_ln_star_fwd", "gvd_tr_lstm_cell_bwd", "gvd_tr_lstm_cell_fwd", "gvd_tr_mean_dim1", "gvd_tr_mha_bwd", "gvd_tr_mha_fwd", "gvd_tr_outer_rows", "gvd_tr_outer_rows_acc", "gvd_tr_pos_nll", "gvd_tr_rowsum", "gvd_tr_softmax_bwd", "gvd_tr_softmax_fwd", "gvd_tr_sum_all", "gvd_tr_targets", "gvd_tr_transpose",
 ]
@@ -75,6 +76,10 @@ def lib():
     L.gvd_workspace_tensor.argtypes = [vp, vp, ci, ci, ctypes.c_char_p]
     L.gvd_workspace_tensor.restype = vp
     L.gvd_prologue_fwd.argtypes = [vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, sz, vp, vp]
+    L.gvd_workspace_bytes_video.argtypes = [vp, ci, ci, ci, ci, ci]
+    L.gvd_workspace_bytes_video.restype = sz
+    L.gvd_prologue_fwd_video.argtypes = [vp, ci, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp, vp]
+    L.gvd_sample_greedy_host_video.argtypes = [vp, ci, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp]
     L.gvd_decode_greedy.argtypes = [vp, ci, ci, vp, sz, vp, vp, vp, vp, vp]
     L.gvd_decode_sample.argtypes = [vp, ci, ci, vp, sz, vp, ctypes.c_uint64, ctypes.c_float, vp, vp, vp, vp]
     L.gvd_decode_step_fwd.argtypes = [vp, ci, ci, vp, sz, ci, vp, vp, vp, vp, i64, vp, vp]
@@ -106,6 +111,7 @@ def lib():
                                    ci, ci, ci, ci, ci, ci, ci, ci, vp]
     L.gvd_op_attention_mode.argtypes = L.gvd_op_attention.argtypes[:-1] + [ci, vp, vp, vp, i64, vp]
     L.gvd_op_attention_form.argtypes = L.gvd_op_attention_mode.argtypes[:-1] + [ci, vp]
+    L.gvd_op_attention_video.argtypes = L.gvd_op_attention_form.argtypes[:-1] + [vp, vp, vp, vp]
     L.gvd_op_beam_topk.argtypes = [vp, i64, ci, ci, ci, vp, vp, vp]
     L.gvd_op_row_argmax.argtypes = [vp, i64, ci, ci, vp, vp]
     L.gvd_op_beam_search_scripted.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
@@ -234,6 +240,7 @@ class NativeModel:
         self.device = torch.cuda.current_device()      # the weight arena and every workspace live on this device
         check(self._L.gvd_model_create_modes(ctypes.byref(self.dims), self.att_input_mode, self.region_attn_mode, ctypes.byref(self._h)))
         self._live = None                              # (B, T, beam, nbox) of the prologue whose outputs sit in the workspace
+        self._live_V = 0                               # ... and its video count (0: a per-clip prologue)
         self.R = self.dims.num_sampled_frm * self.dims.num_prop_per_frm
         self._ws = {}
         n = self._L.gvd_model_num_params(self._h)
@@ -285,16 +292,22 @@ class NativeModel:
         del keep
 
     # ---- workspace
-    def workspace(self, B, T, beam=1, nbox=0):
+    def workspace(self, B, T, beam=1, nbox=0, V=None):
         """The (single) live workspace, sized for a decode with `beam` rows per clip and `nbox` GT boxes.  The prologue's outputs
         live INSIDE it, so a decode entry point that would need a larger allocation than the one the prologue ran in raises instead
-        of silently reallocating (and then decoding from uninitialised memory): size it up front with prologue(..., beam=, nbox=)."""
+        of silently reallocating (and then decoding from uninitialised memory): size it up front with prologue(..., beam=, nbox=).
+        V: the layout of a video-indexed batch of V videos (0: per clip); None: the layout of the live prologue's batch."""
         self._check_device()
         key = (B, T, self.device)
         ws = self._ws.get(key)
-        need = int(self._L.gvd_workspace_bytes_beam(self._h, B, T, beam))
-        if nbox:
-            need = max(need, int(self._L.gvd_workspace_bytes_teacher(self._h, B, T, nbox)))
+        if V is None:
+            V = self._live_V if self._live is not None and self._live[:2] == (B, T) else 0
+        if V:                                      # a video-indexed prologue's layout (gvd_prologue_fwd_video)
+            need = int(self._L.gvd_workspace_bytes_video(self._h, B, V, T, beam, nbox))
+        else:
+            need = int(self._L.gvd_workspace_bytes_beam(self._h, B, T, beam))
+            if nbox:
+                need = max(need, int(self._L.gvd_workspace_bytes_teacher(self._h, B, T, nbox)))
         if ws is not None and ws.numel() < need:
             if self._live is not None and self._live[:2] == (B, T) and (beam > 1 or nbox > 0):
                 raise GvdError("the workspace holding this batch's prologue outputs (sized for beam=%d, nbox=%d) is too small for the requested "
@@ -302,7 +315,7 @@ class NativeModel:
                                (self._live[2], self._live[3], beam, nbox, beam, nbox))
             ws = None                              # a larger layout was requested before any prologue ran in it: reallocate
         if ws is None:
-            self._live = None
+            self._live, self._live_V = None, 0
             nbytes = need
             if nbytes == 0:
                 raise GvdError("bad workspace request B=%d T=%d" % (B, T))
@@ -323,18 +336,26 @@ class NativeModel:
         return ws[off:off + 4 * n].view(torch.float32).view(*shape)
 
     # ---- hot path
-    def prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, want_sim=True, beam=1, nbox=0):
-        B, T = segs_feat.shape[0], segs_feat.shape[1]
-        self._check_device(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask)
-        self._live = None
-        ws = self.workspace(B, T, beam, nbox)
+    def prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, want_sim=True, beam=1, nbox=0, video_idx=None):
+        """video_idx (int64 [B], CUDA): a video-indexed batch.  segs_feat then holds the frame features of V videos [V,T,F] and clip b is
+        event b of video video_idx[b] with its window sample_idx[b]; every result equals the per-clip prologue on segs_feat[video_idx]."""
+        self._check_device(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, video_idx)
+        T = segs_feat.shape[1]
+        B = check_video_batch(segs_feat, video_idx, ppls, num, ppls_feat, sample_idx, pnt_mask) if video_idx is not None else segs_feat.shape[0]
+        V = segs_feat.shape[0] if video_idx is not None else 0
+        self._live, self._live_V = None, 0
+        ws = self.workspace(B, T, beam, nbox, V)
         sim = torch.empty(B, self.dims.detect_size + 1, self.R, dtype=torch.float32, device="cuda") if want_sim else None
-        check(self._L.gvd_prologue_fwd(
-            self._h, B, T, _dev(segs_feat, torch.float32, "segs_feat"), _dev(ppls, torch.float32, "ppls"),
-            _dev(num, torch.int64, "num"), _dev(ppls_feat, torch.float32, "ppls_feat"),
-            _dev(sample_idx, torch.int64, "sample_idx"), _dev(pnt_mask, torch.uint8, "pnt_mask"),
-            ctypes.c_void_p(ws.data_ptr()), ws.numel(), ctypes.c_void_p(sim.data_ptr()) if want_sim else None, _stream()))
-        self._live = (B, T, beam, nbox)
+        common = (_dev(ppls, torch.float32, "ppls"), _dev(num, torch.int64, "num"), _dev(ppls_feat, torch.float32, "ppls_feat"),
+                  _dev(sample_idx, torch.int64, "sample_idx"))
+        tail = (_dev(pnt_mask, torch.uint8, "pnt_mask"), ctypes.c_void_p(ws.data_ptr()), ws.numel(),
+                ctypes.c_void_p(sim.data_ptr()) if want_sim else None, _stream())
+        if V:
+            check(self._L.gvd_prologue_fwd_video(self._h, B, V, T, _dev(segs_feat, torch.float32, "segs_feat"), *common,
+                                                 _dev(video_idx, torch.int64, "video_idx"), *tail))
+        else:
+            check(self._L.gvd_prologue_fwd(self._h, B, T, _dev(segs_feat, torch.float32, "segs_feat"), *common, *tail))
+        self._live, self._live_V = (B, T, beam, nbox), V
         return sim
 
     def decode_greedy(self, B, T, pnt_mask):
@@ -406,14 +427,18 @@ class NativeModel:
             ctypes.c_void_p(att2_out.data_ptr()), int(att2_stride_b),
             ctypes.c_void_p(h_lang_out.data_ptr()) if h_lang_out is not None else None, _stream()))
 
-    def sample_greedy_host(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, out=None):
-        """End-to-end with HOST tensors (pinned recommended): H2D + prologue + loop + D2H inside."""
+    def sample_greedy_host(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, out=None, video_idx=None):
+        """End-to-end with HOST tensors (pinned recommended): H2D + prologue + loop + D2H inside.  video_idx (int64 [B], host): a
+        video-indexed batch as in prologue(); segs_feat [V,T,F] then crosses PCIe once per video."""
         for n, t in (("segs_feat", segs_feat), ("ppls", ppls), ("num", num), ("ppls_feat", ppls_feat),
-                     ("sample_idx", sample_idx), ("pnt_mask", pnt_mask)):
-            if t.is_cuda or not t.is_contiguous():
+                     ("sample_idx", sample_idx), ("pnt_mask", pnt_mask), ("video_idx", video_idx)):
+            if t is not None and (t.is_cuda or not t.is_contiguous()):
                 raise GvdError("%s must be a contiguous host tensor" % n)
-        B, T = segs_feat.shape[0], segs_feat.shape[1]
-        ws = self.workspace(B, T)
+        T = segs_feat.shape[1]
+        B = check_video_batch(segs_feat, video_idx, ppls, num, ppls_feat, sample_idx, pnt_mask) if video_idx is not None else segs_feat.shape[0]
+        V = segs_feat.shape[0] if video_idx is not None else 0
+        self._live, self._live_V = None, 0
+        ws = self.workspace(B, T, 1, 0, V)
         L, R, NC = self.dims.seq_length, self.R, self.dims.detect_size + 1
         if out is None:
             out = dict(seq=torch.empty(B, L, dtype=torch.int64).pin_memory(),
@@ -421,11 +446,33 @@ class NativeModel:
                        att2=torch.empty(B, L, R, dtype=torch.float32).pin_memory(),
                        sim=torch.empty(B, NC, R, dtype=torch.float32).pin_memory())
         hp = lambda t: ctypes.c_void_p(t.data_ptr())
-        check(self._L.gvd_sample_greedy_host(
-            self._h, B, T, hp(segs_feat), hp(ppls), hp(num), hp(ppls_feat), hp(sample_idx), hp(pnt_mask),
-            ctypes.c_void_p(ws.data_ptr()), ws.numel(), hp(out["seq"]), hp(out["logp"]), hp(out["att2"]),
-            hp(out["sim"]) if out.get("sim") is not None else None, _stream()))
+        outs = (ctypes.c_void_p(ws.data_ptr()), ws.numel(), hp(out["seq"]), hp(out["logp"]), hp(out["att2"]),
+                hp(out["sim"]) if out.get("sim") is not None else None, _stream())
+        if V:
+            check(self._L.gvd_sample_greedy_host_video(self._h, B, V, T, hp(segs_feat), hp(ppls), hp(num), hp(ppls_feat), hp(sample_idx),
+                                                       hp(video_idx), hp(pnt_mask), *outs))
+        else:
+            check(self._L.gvd_sample_greedy_host(self._h, B, T, hp(segs_feat), hp(ppls), hp(num), hp(ppls_feat), hp(sample_idx), hp(pnt_mask),
+                                                 *outs))
+        self._live, self._live_V = (B, T, 1, 0), V
         return out
+
+
+def check_video_batch(segs_feat, video_idx, ppls, num, ppls_feat, sample_idx, pnt_mask):
+    """Validate a video-indexed batch: segs_feat [V,T,F] holds V videos, video_idx int64 [B] maps each of the B events to one of them, and
+    the per-event tensors have B rows.  Returns B; raises ValueError."""
+    if not torch.is_tensor(video_idx) or video_idx.dtype != torch.int64:
+        raise ValueError("video_idx must be an int64 tensor, got %s" % (video_idx.dtype if torch.is_tensor(video_idx) else type(video_idx).__name__))
+    if video_idx.dim() != 1 or video_idx.numel() < 1:
+        raise ValueError("video_idx must be a non-empty 1-D tensor [B], got shape %s" % (tuple(video_idx.shape),))
+    B, V = video_idx.numel(), segs_feat.shape[0]
+    for n, t in (("ppls", ppls), ("num", num), ("ppls_feat", ppls_feat), ("sample_idx", sample_idx), ("pnt_mask", pnt_mask)):
+        if t.shape[0] != B:
+            raise ValueError("video_idx has %d events but %s has %d rows" % (B, n, t.shape[0]))
+    lo, hi = int(video_idx.min()), int(video_idx.max())
+    if lo < 0 or hi >= V:
+        raise ValueError("video_idx values must lie in [0, %d) (segs_feat holds %d videos), got [%d, %d]" % (V, V, lo, hi))
+    return B
 
 
 class TfmLayer(ctypes.Structure):
@@ -681,7 +728,7 @@ def op_gru_layer(path, gi, Whh, bhh, sample_idx=None):
 
 def op_attention(p_pool, pool, p_conv, conv, w1, b1, w2, b2, att_mask, out_mask, z_out, partial, x_out, RC, TC, q=None, q_part=None,
                  q_bias=None, ticket=None, x_pk=None, feat_div=1, att_input_mode=None, gate_w=None, gate_b=None, gate_h=None,
-                 region_attn_mode=None):
+                 region_attn_mode=None, _video=None):
     """The decode attention of B query rows through gvd_op_attention.  Features [B / feat_div, N, A | H]; q [B, 2A] or its split-K planes
     q_part [q_S, B, 2A] + q_bias [2A]; att_mask [B / feat_div, R+1]; out_mask [B / feat_div, R+1] or a [B / feat_div, R+1] column window
     of a wider mask (its row pitch is passed); z_out [B, R] and x_out [B, H] (x_pk [B, rup32(H)] int32 words) may be column windows of
@@ -700,7 +747,12 @@ def op_attention(p_pool, pool, p_conv, conv, w1, b1, w2, b2, att_mask, out_mask,
             _dev(p_conv, torch.float32, "p_conv") if p_conv is not None else None, _dev(conv, torch.float32, "conv") if conv is not None else None, _ptr(q), _ptr(q_part), q_S, _ptr(q_bias), _ptr(w1), _ptr(b1),
             _ptr(w2), _ptr(b2), _ptr(att_mask), _ptr(out_mask), out_mask.stride(0), _ptr(z_out), _pitch(z_out), _ptr(partial), _ptr(ticket),
             _ptr(x_out), _pitch(x_out), _ptr(x_pk), _pitch(x_pk), B, R, T, A, H, int(RC), int(TC), int(feat_div))
-    if region_attn_mode is not None:
+    if _video is not None:
+        vid, win, cb = _video
+        check(lib().gvd_op_attention_video(*args, ATT_INPUT_MODES[att_input_mode or "both"], _ptr(gate_w), _ptr(gate_b), _ptr(gate_h),
+                                           _pitch(gate_h), REGION_ATTN_MODES[region_attn_mode or "mix"], _dev(vid, torch.int64, "video_idx"),
+                                           _dev(win, torch.int64, "sample_idx"), _dev(cb, torch.float32, "ctx_bias"), _stream()))
+    elif region_attn_mode is not None:
         check(lib().gvd_op_attention_form(*args, ATT_INPUT_MODES[att_input_mode or "both"], _ptr(gate_w), _ptr(gate_b), _ptr(gate_h),
                                           _pitch(gate_h), REGION_ATTN_MODES[region_attn_mode], _stream()))
     elif att_input_mode is None:
@@ -708,6 +760,14 @@ def op_attention(p_pool, pool, p_conv, conv, w1, b1, w2, b2, att_mask, out_mask,
     else:
         check(lib().gvd_op_attention_mode(*args, ATT_INPUT_MODES[att_input_mode], _ptr(gate_w), _ptr(gate_b), _ptr(gate_h), _pitch(gate_h),
                                           _stream()))
+
+
+def op_attention_video(video_idx, sample_idx, ctx_bias, *args, **kw):
+    """op_attention over video-level frame features (gvd_op_attention_video): p_conv / conv [V, T, A | H] unmasked, video_idx [B / feat_div]
+    int64, sample_idx [B / feat_div, 2] the windows, ctx_bias [A].  Equals op_attention on p_conv / conv gathered by video_idx with the rows
+    outside each window set to (ctx_bias, 0)."""
+    kw = dict(kw, _video=(video_idx, sample_idx, ctx_bias))
+    op_attention(*args, **kw)
 
 
 def op_beam_topk(logits, K):

@@ -182,7 +182,9 @@ __global__ void bn_affine_kernel(const float* w, const float* b, const float* me
 
 // ------------------------------------------------------------------------------------ model
 struct Param { std::string key; size_t numel; size_t off; bool set; };
-struct LoopKey { int B, T, backend; void* ws; size_t ws_bytes; };   // what a captured decode loop depends on
+struct LoopKey { int B, T, backend; void* ws; size_t ws_bytes; int V; };   // what a captured decode loop depends on
+// a workspace whose prologue ran on a video-indexed batch (gvd_prologue_fwd_video): the decode entries lay it out for V videos
+struct VideoWs { void* ws; int B, T, V; };
 
 struct gvd_model {
     gvd_dims_t d;
@@ -215,13 +217,14 @@ struct gvd_model {
     // cudaGraphLaunch (no per-launch host cost, back-to-back scheduling on the device)
     cudaStream_t capture_stream = nullptr;
     cudaGraphExec_t greedy_exec = nullptr;
-    LoopKey greedy_key{0, 0, 0, nullptr, 0};
+    LoopKey greedy_key{0, 0, 0, nullptr, 0, 0};
     long long greedy_nodes = 0;      // kernel launches inside one replay (counted while capturing)
     // the multinomial-sampling loop has a graph of its own (alternating greedy and sampling calls re-capture neither); its seed and
     // temperature are read from the workspace, so a new draw replays the same graph
     cudaGraphExec_t sample_exec = nullptr;
-    LoopKey sample_key{0, 0, 0, nullptr, 0};
+    LoopKey sample_key{0, 0, 0, nullptr, 0, 0};
     long long sample_nodes = 0;
+    std::vector<VideoWs> video_ws;   // set by the video prologues, cleared by a per-clip prologue on the same workspace
 
     float* P(const std::string& k) const {
         auto it = index.find(k);
@@ -577,6 +580,8 @@ struct WS {
     int *target, *pred_cls, *cls_idx, *part_cnt;
     long long* tok_col;
     int RC, TC, nch_r, nch_t, clip_chunk, beam, nbox;
+    int V;                             // > 0: video-indexed batch, the frame tensors hold V videos' rows (V = 0: one copy per clip)
+    long long* in_vid;                 // [B] video of each clip (V > 0); the windows stay in in_sidx
     size_t bytes;
 };
 
@@ -594,16 +599,18 @@ static void attn_chunking(int B, int R, int T, int* RC, int* TC) {
     if (const char* e = getenv("GVD_ATTN_TC")) { const int v = atoi(e); if (v >= 16 && v <= 128) *TC = (v + 7) / 8 * 8; }
 }
 
-static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, int nbox = 0) {
+static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, int nbox = 0, int V = 0) {
     const gvd_dims_t& d = m->d;
     const int H = d.rnn_size, A = d.att_hid_size, R = m->R, G = m->G;
     WS w{};
     size_t off = 0;
     char* b0 = (char*)base;
     auto take = [&](size_t bytes) { size_t o = off; off += rup(bytes, 256); return (void*)(b0 ? b0 + o : (char*)0 + o); };
-    const size_t BR = (size_t)B * R, BT = (size_t)B * T;
+    const size_t NV = V > 0 ? V : B;          // rows of the frame branch: the clips, or the videos of a video-indexed batch
+    const size_t BR = (size_t)B * R, BT = NV * T;
     const size_t BD = (size_t)B * beam;       // decode rows (beam rows of one clip share its features)
     w.beam = beam;
+    w.V = V;
     attn_chunking((int)BD, R, T, &w.RC, &w.TC);
     gvd_attn_chunks(R, T, w.RC, w.TC, &w.nch_r, &w.nch_t);
     w.clip_chunk = std::max(1, std::min(B, (int)(100000000ll / ((long long)m->nheads * R * R * 4 + 1))));   // S chunk ~<= 100 MB (L2)
@@ -619,12 +626,15 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     w.in_feat = (float*)take(BR * d.att_feat_size * 4);
     w.in_num = (long long*)take((size_t)B * 7 * 8);
     w.in_sidx = (long long*)take((size_t)B * 2 * 8);
+    // (ahead of every slot sized by beam / nbox: the prologue lays the workspace out for one row per clip, the beam and teacher-forced
+    // decodes for theirs, and both must find the video indices at the same place)
+    w.in_vid = V > 0 ? (long long*)take((size_t)B * 8) : nullptr;
     w.in_mask = (unsigned char*)take((size_t)B * (R + 1));
     w.out_seq = (long long*)take((size_t)B * d.seq_length * 8);
     w.out_logp = (float*)take((size_t)B * d.seq_length * 4);
     w.out_att2 = (float*)take((size_t)B * d.seq_length * R * 4);
     w.out_sim = (float*)take((size_t)B * m->NC * R * 4);
-    w.fc_mean = (float*)take((size_t)B * d.fc_feat_size * 4);
+    w.fc_mean = (float*)take(NV * d.fc_feat_size * 4);
     w.xcat = (float*)take((size_t)B * m->FCXp * 4);
     w.fc_feats = (float*)take((size_t)B * H * 4);
     w.g_pool = (float*)take(BR * 2048 * 4);
@@ -658,10 +668,10 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     w.gru_out0 = (float*)take(BT * 2 * G * 4);
     w.conv = (float*)take(BT * H * 4);
     w.p_conv = (float*)take(BT * A * 4);
-    w.gh = (float*)take((size_t)2 * B * 3 * G * 4);
-    w.hstate = (float*)take((size_t)2 * 2 * B * G * 4);
+    w.gh = (float*)take((size_t)2 * NV * 3 * G * 4);
+    w.hstate = (float*)take((size_t)2 * 2 * NV * G * 4);
     w.gru_bar = (unsigned int*)take(256);
-    w.h_img = (float*)take((size_t)2 * 2 * B * G * 4);
+    w.h_img = (float*)take((size_t)2 * 2 * NV * G * 4);
     w.a_pk_frame = (float*)take(BT * (size_t)((std::max(H, 2 * G) + 31) / 32 * 32 + 32) * 4);   // the frame branch's own pack buffer (it runs concurrently with the region stages)
     w.pre_att = (float*)take((size_t)B * 4 * H * 4);
     w.h_att = (float*)take(2 * BD * H * 4);
@@ -748,9 +758,27 @@ extern "C" GVD_API size_t gvd_workspace_bytes_beam(const gvd_model_t* m, int B, 
     return ws_layout(m, B, T, nullptr, beam_size).bytes;
 }
 
+extern "C" GVD_API size_t gvd_workspace_bytes_video(const gvd_model_t* m, int B, int V, int T, int beam_size, int nbox) {
+    if (!m || B < 1 || V < 1 || T < 1 || beam_size < 1 || nbox < 0) return 0;
+    return ws_layout(m, B, T, nullptr, beam_size, nbox, V).bytes;
+}
+
+// V of the video prologue whose outputs sit in `workspace` for (B, T), 0 if a per-clip prologue (or none) filled it
+static int video_of(const gvd_model* m, const void* workspace, int B, int T) {
+    for (const VideoWs& v : m->video_ws)
+        if (v.ws == workspace) return v.B == B && v.T == T ? v.V : 0;
+    return 0;
+}
+static void set_video(gvd_model* m, void* workspace, int B, int T, int V) {
+    auto& vs = m->video_ws;
+    for (size_t i = 0; i < vs.size(); ++i)
+        if (vs[i].ws == workspace) { vs.erase(vs.begin() + i); break; }
+    if (V > 0) vs.push_back(VideoWs{workspace, B, T, V});
+}
+
 extern "C" GVD_API float* gvd_workspace_tensor(const gvd_model_t* m, void* workspace, int B, int T, const char* name) {
     if (!m || !workspace || !name) return nullptr;
-    WS w = ws_layout(m, B, T, workspace);
+    WS w = ws_layout(m, B, T, workspace, 1, 0, video_of(m, workspace, B, T));
     const std::string n(name);
     if (n == "fc_feats") return w.fc_feats;
     if (n == "g_pool") return w.g_pool;
@@ -766,11 +794,12 @@ extern "C" GVD_API float* gvd_workspace_tensor(const gvd_model_t* m, void* works
     return nullptr;
 }
 
-static int check_ws(const gvd_model* m, int B, int T, void* workspace, size_t bytes, WS* w, int beam = 1, int nbox = 0) {
+// V < 0: the layout the last prologue on this workspace left (video_of); V >= 0: that layout explicitly (a prologue about to run)
+static int check_ws(const gvd_model* m, int B, int T, void* workspace, size_t bytes, WS* w, int beam = 1, int nbox = 0, int V = -1) {
     GVD_REQUIRE(m && m->finalized, "model not finalized (call gvd_model_finalize after setting every parameter)");
     GVD_REQUIRE(B >= 1 && T >= 1, "bad batch/frames B=%d T=%d", B, T);
     GVD_REQUIRE(workspace && ((uintptr_t)workspace & 255) == 0, "workspace must be a 256-byte aligned device pointer");
-    *w = ws_layout(m, B, T, workspace, beam, nbox);
+    *w = ws_layout(m, B, T, workspace, beam, nbox, V < 0 ? video_of(m, workspace, B, T) : V);
     GVD_REQUIRE(bytes >= w->bytes, "workspace too small: %zu < %zu bytes", bytes, w->bytes);
     return 0;
 }
@@ -1019,16 +1048,21 @@ static int region_prologue(const gvd_model* m, const WS& w0, int c0, int cb, con
     return 0;
 }
 
-// P1 + P7 + the constant part of the attention-LSTM gates: everything that only needs the frame features
-static int frame_stages(const gvd_model* m, const WS& w, int B, int T, const float* segs_feat, const long long* num, const long long* sample_idx, cudaStream_t st) {
+// P1 + P7 + the constant part of the attention-LSTM gates: everything that only needs the frame features.
+// Video-indexed batch (w.V > 0, vid = the workspace's copy of video_idx): segs_feat holds V videos; the frame mean and the frame branch run
+// once per video, the latter unmasked (the decode attention applies each clip's window), and clip b's vector reads video vid[b]'s mean.
+static int frame_stages(const gvd_model* m, const WS& w, int B, int T, const float* segs_feat, const long long* num, const long long* sample_idx,
+                        cudaStream_t st, const long long* vid = nullptr) {
     const gvd_dims_t& d = m->d;
     const int H = d.rnn_size, E = d.input_encoding_size, FC = d.fc_feat_size;
+    const int NV = vid ? w.V : B;
     // P1 clip vector (model.py:508-510,548)
-    GVD_STAGE("clip.frame_mean", gvd_frame_mean(segs_feat, w.fc_mean, B, T, FC, st));
-    GVD_STAGE("clip.vector", gvd_clip_vector(w.fc_mean, num, m->P("seg_info_embed.0.weight"), m->P("seg_info_embed.0.bias"), w.xcat, B, FC, 50, m->FCXp, st));
+    GVD_STAGE("clip.frame_mean", gvd_frame_mean(segs_feat, w.fc_mean, NV, T, FC, st));
+    GVD_STAGE("clip.vector", gvd_clip_vector(w.fc_mean, num, m->P("seg_info_embed.0.weight"), m->P("seg_info_embed.0.bias"), w.xcat, B, FC, 50, m->FCXp, st,
+                                             vid));
     GVD_STAGE("clip.fc_embed", gvd_linear(w.xcat, m->FCXp, m->fc_embed_w, m->FCXp, m->P("fc_embed.0.bias"), w.fc_feats, H, B, H, m->FCXp, GVD_ACT_RELU, st));
     // P7 frame branch (model.py:556-565); dual_region reads no frame features (model.py:393: dummies)
-    if (m->att_mode != GVD_ATT_INPUT_DUAL_REGION) GVD_TRY(frame_branch_fwd(m, w, B, T, segs_feat, sample_idx, st));
+    if (m->att_mode != GVD_ATT_INPUT_DUAL_REGION) GVD_TRY(frame_branch_fwd(m, w, NV, T, segs_feat, vid ? nullptr : sample_idx, st));
     // constant part of the attention-LSTM gates: W_ih[:, :H] fc_feats + b_ih + b_hh (fc_feats is the same at every step)
     GVD_STAGE("decode.pre_att", gvd_linear(w.fc_feats, H, m->P("core.att_lstm.weight_ih"), H + E, m->att_bias_sum, w.pre_att, 4 * H, B, 4 * H, H, GVD_ACT_NONE, st));
     return 0;
@@ -1056,13 +1090,19 @@ static int frame_join(gvd_model* m, cudaStream_t st) {
     GVD_CHECK_CUDA(cudaStreamWaitEvent(st, m->ev_join, 0));
     return 0;
 }
-extern "C" GVD_API int gvd_prologue_fwd(gvd_model_t* m, int B, int T, const float* segs_feat, const float* ppls, const int64_t* num,
-                                const float* ppls_feat, const int64_t* sample_idx, const uint8_t* pnt_mask, void* workspace,
-                                size_t workspace_bytes, float* sim_mat_out, void* stream) {
+// V = 0: per-clip batch; V > 0: video-indexed batch (segs_feat [V,T,F], video_idx [B])
+static int prologue_run(gvd_model_t* m, int B, int V, int T, const float* segs_feat, const float* ppls, const int64_t* num,
+                        const float* ppls_feat, const int64_t* sample_idx, const int64_t* video_idx, const uint8_t* pnt_mask, void* workspace,
+                        size_t workspace_bytes, float* sim_mat_out, void* stream) {
     WS w;
-    GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
-    GVD_REQUIRE(segs_feat && ppls && num && ppls_feat && sample_idx && pnt_mask, "prologue: null input");
+    GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w, 1, 0, V));
+    GVD_REQUIRE(segs_feat && ppls && num && ppls_feat && sample_idx && pnt_mask && (V == 0 || video_idx), "prologue: null input");
     cudaStream_t st = (cudaStream_t)stream;
+    set_video(m, workspace, B, T, V);
+    if (V > 0) {       // the decode entries read each clip's video and window from the workspace
+        GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_vid, video_idx, (size_t)B * 8, cudaMemcpyDeviceToDevice, st));
+        GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_sidx, sample_idx, (size_t)B * 2 * 8, cudaMemcpyDeviceToDevice, st));
+    }
     const gvd_dims_t& d = m->d;
     const int R = m->R;
     const bool overlap = frame_overlap_on();
@@ -1073,7 +1113,7 @@ extern "C" GVD_API int gvd_prologue_fwd(gvd_model_t* m, int B, int T, const floa
     if (otrace) for (auto& e : te) GVD_CHECK_CUDA(cudaEventCreate(&e));
     if (overlap) { GVD_TRY(frame_fork(m, st)); fst = m->frame_stream; }
     if (otrace) GVD_CHECK_CUDA(cudaEventRecord(te[0], st));
-    const int rc_frame = frame_stages(m, w, B, T, segs_feat, (const long long*)num, (const long long*)sample_idx, fst);
+    const int rc_frame = frame_stages(m, w, B, T, segs_feat, (const long long*)num, (const long long*)sample_idx, fst, V > 0 ? w.in_vid : nullptr);
     if (otrace) GVD_CHECK_CUDA(cudaEventRecord(te[1], fst));
     if (overlap && rc_frame != 0) frame_join(m, st);            // never leave the second stream dangling behind an error return
     if (rc_frame != 0) return rc_frame;
@@ -1099,6 +1139,17 @@ extern "C" GVD_API int gvd_prologue_fwd(gvd_model_t* m, int B, int T, const floa
         for (auto& e : te) cudaEventDestroy(e);
     }
     return rc;
+}
+extern "C" GVD_API int gvd_prologue_fwd(gvd_model_t* m, int B, int T, const float* segs_feat, const float* ppls, const int64_t* num,
+                                const float* ppls_feat, const int64_t* sample_idx, const uint8_t* pnt_mask, void* workspace,
+                                size_t workspace_bytes, float* sim_mat_out, void* stream) {
+    return prologue_run(m, B, 0, T, segs_feat, ppls, num, ppls_feat, sample_idx, nullptr, pnt_mask, workspace, workspace_bytes, sim_mat_out, stream);
+}
+extern "C" GVD_API int gvd_prologue_fwd_video(gvd_model_t* m, int B, int V, int T, const float* segs_feat, const float* ppls, const int64_t* num,
+                                              const float* ppls_feat, const int64_t* sample_idx, const int64_t* video_idx, const uint8_t* pnt_mask,
+                                              void* workspace, size_t workspace_bytes, float* sim_mat_out, void* stream) {
+    GVD_REQUIRE(V >= 1, "prologue_video: V=%d must be >= 1", V);
+    return prologue_run(m, B, V, T, segs_feat, ppls, num, ppls_feat, sample_idx, video_idx, pnt_mask, workspace, workspace_bytes, sim_mat_out, stream);
 }
 
 // ------------------------------------------------------------------------------------ decode
@@ -1223,6 +1274,7 @@ static int core_step(const gvd_model* m, const WS& w, int B, int T, int step, co
         a.att_mask = att_mask; a.out_mask = out_mask; a.z_out = z_out; a.z_stride_b = z_stride_b;
         a.partial = w.partial; a.B = B; a.R = R; a.T = T; a.A = A; a.H = H; a.RC = w.RC; a.TC = w.TC; a.feat_div = div;
         a.out_mask_stride = out_mask_stride; a.mode = m->att_mode; a.form = m->region_form;   // (dp: P() of the absent alpha_net keys is NULL)
+        if (w.V > 0) { a.vid = w.in_vid; a.win = w.in_sidx; a.ctx_bias = m->P("ctx2att.bias"); }   // video-level p_conv / conv
         a.ticket = w.ticket; a.x_out = w.x_lang;         // chunk partials are merged by the last CTA of each row (no combine launch)
         if (skinny) { a.x_out = w.xcat_lang; a.x_ld = 3 * H; }   // ... straight into the language LSTM's concatenated input
         if (sk16) { a.x_pk = w.xp_lang; a.x_pk_ld = 3 * H; }
@@ -1360,7 +1412,7 @@ static int decode_loop_run(gvd_model_t* m, const WS& w, int B, int T, void* work
         return decode_greedy_enqueue(m, w, B, T, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_logits_out, st, sample);
     // Graph path: the loop reads the mask from / writes its results to workspace-resident buffers (fixed addresses), the caller's
     // tensors are copied in / out around the replay.
-    if (!exec || key.B != B || key.T != T || key.backend != gvd_backend() || key.ws != workspace || key.ws_bytes != workspace_bytes) {
+    if (!exec || key.B != B || key.T != T || key.backend != gvd_backend() || key.ws != workspace || key.ws_bytes != workspace_bytes || key.V != w.V) {
         if (exec) { cudaGraphExecDestroy(exec); exec = nullptr; }
         if (!m->capture_stream) GVD_CHECK_CUDA(cudaStreamCreateWithFlags(&m->capture_stream, cudaStreamNonBlocking));
         cudaGraph_t graph = nullptr;
@@ -1376,7 +1428,7 @@ static int decode_loop_run(gvd_model_t* m, const WS& w, int B, int T, void* work
         const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
         cudaGraphDestroy(graph);
         GVD_CHECK_CUDA(ie);
-        key = {B, T, gvd_backend(), workspace, workspace_bytes};
+        key = {B, T, gvd_backend(), workspace, workspace_bytes, w.V};
     }
     if (pnt_mask != w.in_mask) GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_mask, pnt_mask, (size_t)B * (R + 1), cudaMemcpyDeviceToDevice, st));
     GVD_CHECK_CUDA(cudaGraphLaunch(exec, st));
@@ -1603,17 +1655,21 @@ extern "C" GVD_API int gvd_plan_h2d_chunks(int batch_clips, int unit, int* chunk
     return (int)s.size();
 }
 
-extern "C" GVD_API int gvd_sample_greedy_host(gvd_model_t* m, int B, int T, const float* h_segs_feat, const float* h_ppls, const int64_t* h_num,
-                                      const float* h_ppls_feat, const int64_t* h_sample_idx, const uint8_t* h_pnt_mask, void* workspace,
-                                      size_t workspace_bytes, int64_t* h_seq_out, float* h_logprobs_out, float* h_att2_out,
-                                      float* h_sim_mat_out, void* stream) {
+// V = 0: per-clip batch; V > 0: video-indexed batch, h_segs_feat [V,T,F] (V videos' frames cross PCIe instead of B copies)
+static int sample_greedy_host_run(gvd_model_t* m, int B, int V, int T, const float* h_segs_feat, const float* h_ppls, const int64_t* h_num,
+                                  const float* h_ppls_feat, const int64_t* h_sample_idx, const int64_t* h_video_idx, const uint8_t* h_pnt_mask,
+                                  void* workspace, size_t workspace_bytes, int64_t* h_seq_out, float* h_logprobs_out, float* h_att2_out,
+                                  float* h_sim_mat_out, void* stream) {
     WS w;
-    GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
-    GVD_REQUIRE(h_segs_feat && h_ppls && h_num && h_ppls_feat && h_sample_idx && h_pnt_mask && h_seq_out, "sample_greedy_host: null argument");
+    GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w, 1, 0, V));
+    GVD_REQUIRE(h_segs_feat && h_ppls && h_num && h_ppls_feat && h_sample_idx && h_pnt_mask && h_seq_out && (V == 0 || h_video_idx),
+                "sample_greedy_host: null argument");
+    for (int b = 0; b < (V > 0 ? B : 0); ++b)
+        GVD_REQUIRE(h_video_idx[b] >= 0 && h_video_idx[b] < V, "sample_greedy_host: video_idx[%d] = %lld outside [0, %d)", b, (long long)h_video_idx[b], V);
     cudaStream_t st = (cudaStream_t)stream;
     const gvd_dims_t& d = m->d;
     const int R = m->R, L = d.seq_length, FC = d.fc_feat_size;
-    const size_t BR = (size_t)B * R, BT = (size_t)B * T;
+    const size_t BR = (size_t)B * R, BT = (size_t)(V > 0 ? V : B) * T;     // BT: frame rows that cross PCIe
     // The fc6 region features are ~98 % of the input bytes (819 MB at B=100) and every region stage is per-clip independent,
     // so they cross PCIe in clip chunks on a second stream while the previous chunk runs P2-P6 on the compute stream.
     const std::vector<int> sched = h2d_schedule(B, w.clip_chunk);
@@ -1651,6 +1707,8 @@ extern "C" GVD_API int gvd_sample_greedy_host(gvd_model_t* m, int B, int T, cons
     GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_num, h_num, (size_t)B * 7 * 8, cudaMemcpyHostToDevice, st));
     GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_sidx, h_sample_idx, (size_t)B * 2 * 8, cudaMemcpyHostToDevice, st));
     GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_mask, h_pnt_mask, (size_t)B * (R + 1), cudaMemcpyHostToDevice, st));
+    if (V > 0) GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_vid, h_video_idx, (size_t)B * 8, cudaMemcpyHostToDevice, st));
+    set_video(m, workspace, B, T, V);
     cudaStream_t fst = st;
     if (overlap) { GVD_TRY(frame_fork(m, st)); fst = m->frame_stream; }          // (forked behind the small copies: the frame stages read num / sample_idx)
     // the big chunk copies are enqueued AFTER the small ones: the H2D copy engine is one FIFO across streams, and the first
@@ -1678,7 +1736,7 @@ extern "C" GVD_API int gvd_sample_greedy_host(gvd_model_t* m, int B, int T, cons
     auto run_frame = [&]() -> int {
         frame_done = true;
         if (big_segs) GVD_CHECK_CUDA(cudaStreamWaitEvent(fst, ev_segs, 0));
-        return frame_stages(m, w, B, T, w.in_segs, w.in_num, w.in_sidx, fst);
+        return frame_stages(m, w, B, T, w.in_segs, w.in_num, w.in_sidx, fst, V > 0 ? w.in_vid : nullptr);
     };
     if (!big_segs) rc = run_frame();
     {
@@ -1712,6 +1770,21 @@ extern "C" GVD_API int gvd_sample_greedy_host(gvd_model_t* m, int B, int T, cons
     GVD_CHECK_CUDA(cudaStreamSynchronize(m->copy_stream));
     if (trace) fprintf(stderr, "[gvd] %.2f ms: copy stream drained\n", ms_since());
     return 0;
+}
+extern "C" GVD_API int gvd_sample_greedy_host(gvd_model_t* m, int B, int T, const float* h_segs_feat, const float* h_ppls, const int64_t* h_num,
+                                      const float* h_ppls_feat, const int64_t* h_sample_idx, const uint8_t* h_pnt_mask, void* workspace,
+                                      size_t workspace_bytes, int64_t* h_seq_out, float* h_logprobs_out, float* h_att2_out,
+                                      float* h_sim_mat_out, void* stream) {
+    return sample_greedy_host_run(m, B, 0, T, h_segs_feat, h_ppls, h_num, h_ppls_feat, h_sample_idx, nullptr, h_pnt_mask, workspace, workspace_bytes,
+                                  h_seq_out, h_logprobs_out, h_att2_out, h_sim_mat_out, stream);
+}
+extern "C" GVD_API int gvd_sample_greedy_host_video(gvd_model_t* m, int B, int V, int T, const float* h_segs_feat, const float* h_ppls,
+                                                    const int64_t* h_num, const float* h_ppls_feat, const int64_t* h_sample_idx,
+                                                    const int64_t* h_video_idx, const uint8_t* h_pnt_mask, void* workspace, size_t workspace_bytes,
+                                                    int64_t* h_seq_out, float* h_logprobs_out, float* h_att2_out, float* h_sim_mat_out, void* stream) {
+    GVD_REQUIRE(V >= 1, "sample_greedy_host_video: V=%d must be >= 1", V);
+    return sample_greedy_host_run(m, B, V, T, h_segs_feat, h_ppls, h_num, h_ppls_feat, h_sample_idx, h_video_idx, h_pnt_mask, workspace,
+                                  workspace_bytes, h_seq_out, h_logprobs_out, h_att2_out, h_sim_mat_out, stream);
 }
 
 // Post-decode grounding extraction (main.py:364-370, SURVEY 8(f) rank 2): for every generated word and every sampled frame the
@@ -1934,13 +2007,13 @@ extern "C" GVD_API int gvd_op_gru_layer(int path, const float* gi, const float* 
 // The decode attention (attn_partial_kernel) with every AttnArgs field the decode step sets.  ticket != NULL: the last chunk CTA of each row
 // merges the partials (the decode step's fused path; the caller zeroes the tickets once); ticket == NULL: attn_combine_kernel merges them
 // after the partial launch, into x_out at pitch H.  Test hook.
-extern "C" GVD_API int gvd_op_attention_form(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
-                                             const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
-                                             const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
-                                             int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
-                                             int B, int R, int T, int A, int H, int RC, int TC, int feat_div, int att_input_mode,
-                                             const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld, int region_attn_mode,
-                                             void* stream) {
+static int op_attention(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                        const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
+                        const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
+                        int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
+                        int B, int R, int T, int A, int H, int RC, int TC, int feat_div, int att_input_mode,
+                        const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld, int region_attn_mode,
+                        const int64_t* video_idx, const int64_t* sample_idx, const float* ctx_bias, void* stream) {
     GVD_REQUIRE(att_input_mode == GVD_ATT_INPUT_BOTH || att_input_mode == GVD_ATT_INPUT_FEATMAP || att_input_mode == GVD_ATT_INPUT_DUAL_REGION,
                 "op_attention: unknown att_input_mode %d", att_input_mode);
     GVD_REQUIRE(region_attn_mode == GVD_REGION_ATTN_MIX || region_attn_mode == GVD_REGION_ATTN_MIX_MUL || region_attn_mode == GVD_REGION_ATTN_DP,
@@ -1963,12 +2036,36 @@ extern "C" GVD_API int gvd_op_attention_form(const float* p_pool, const float* p
     a.B = B; a.R = R; a.T = T; a.A = A; a.H = H; a.RC = RC; a.TC = TC; a.feat_div = feat_div; a.mode = att_input_mode;
     a.gate_w = gate_w; a.gate_b = gate_b; a.gate_h = gate_h; a.gate_ld = gate_ld; a.form = region_attn_mode;
     if (dp) { a.w2 = a.b2 = nullptr; if (dual) a.w1 = a.b1 = nullptr; }          // the kernel must not need them
+    a.vid = (const long long*)video_idx; a.win = (const long long*)sample_idx; a.ctx_bias = ctx_bias;
     cudaStream_t st = (cudaStream_t)stream;
     GVD_TRY(gvd_attn_partial(a, st));
     if (ticket) return 0;
     int nch_r, nch_t;
     gvd_attn_chunks(R, T, RC, TC, &nch_r, &nch_t);
     return gvd_attn_combine(partial, x_out, B, H, nch_r, nch_t, att_input_mode, st);
+}
+extern "C" GVD_API int gvd_op_attention_form(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                                             const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
+                                             const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
+                                             int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
+                                             int B, int R, int T, int A, int H, int RC, int TC, int feat_div, int att_input_mode,
+                                             const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld, int region_attn_mode,
+                                             void* stream) {
+    return op_attention(p_pool, pool, p_conv, conv, q, q_part, q_S, q_bias, w1, b1, w2, b2, att_mask, out_mask, out_mask_stride, z_out,
+                        z_stride_b, partial, ticket, x_out, x_ld, x_pk, x_pk_ld, B, R, T, A, H, RC, TC, feat_div, att_input_mode, gate_w,
+                        gate_b, gate_h, gate_ld, region_attn_mode, nullptr, nullptr, nullptr, stream);
+}
+extern "C" GVD_API int gvd_op_attention_video(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                                              const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
+                                              const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
+                                              int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
+                                              int B, int R, int T, int A, int H, int RC, int TC, int feat_div, int att_input_mode,
+                                              const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld, int region_attn_mode,
+                                              const int64_t* video_idx, const int64_t* sample_idx, const float* ctx_bias, void* stream) {
+    GVD_REQUIRE(video_idx && sample_idx && ctx_bias, "op_attention_video: video_idx, sample_idx and ctx_bias are required");
+    return op_attention(p_pool, pool, p_conv, conv, q, q_part, q_S, q_bias, w1, b1, w2, b2, att_mask, out_mask, out_mask_stride, z_out,
+                        z_stride_b, partial, ticket, x_out, x_ld, x_pk, x_pk_ld, B, R, T, A, H, RC, TC, feat_div, att_input_mode, gate_w,
+                        gate_b, gate_h, gate_ld, region_attn_mode, video_idx, sample_idx, ctx_bias, stream);
 }
 extern "C" GVD_API int gvd_op_attention_mode(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
                                              const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,

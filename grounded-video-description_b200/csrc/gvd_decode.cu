@@ -19,6 +19,8 @@
 //                          region chunks' score: ADD w.tanh(p+q)+b ('mix'), MUL w.tanh(p*q)+b
 //                          ('mix_mul') or DOT p.q ('dp': no alpha_net, w / b never read).  The
 //                          temporal chunks are additive in every mode.
+//                          Video-indexed batches (AttnArgs::vid): a clip's temporal chunks stream only its window's rows of
+//                          the video's unmasked features; the first one adds the closed-form out-of-window softmax term.
 //   attn_combine_kernel  : merges the chunk partials (flash-decoding style) into att + att2.
 //   greedy_pick_kernel   : log_softmax + top-2 + UNK rule (misc/model.py:590-594,615).
 #include "../../include/gvd_b200.h"
@@ -391,11 +393,22 @@ __global__ void __launch_bounds__(ATT_THREADS, FORM == GVD_REGION_ATTN_MIX ? 0 :
     const bool region = c < nch_r;
     const int N = region ? a.R : a.T;
     const int chunk = region ? a.RC : a.TC;
-    const int r0 = region ? c * chunk : (c - nch_r) * chunk;
-    const int nrows = min(chunk, N - r0);
+    int r0 = region ? c * chunk : (c - nch_r) * chunk;
+    int nrows = min(chunk, N - r0);
+    long long frow = fb;                                       // feature row block: the clip, or its video
+    int n_out = 0;                                             // out-of-window rows this chunk's record stands for (video rows only)
+    if (a.vid && !region) {
+        const long long lo = max(a.win[2 * fb], 0ll), hi = min(a.win[2 * fb + 1], (long long)N);
+        const int wlo = (int)min(lo, (long long)N), whi = (int)max(hi, (long long)wlo);     // window ∩ [0,T), empty -> wlo == whi
+        const int c0 = max(r0, wlo), c1 = min(r0 + nrows, whi);
+        frow = a.vid[fb];
+        if (c == nch_r) n_out = N - (whi - wlo);
+        r0 = c0;
+        nrows = max(c1 - c0, 0);
+    }
     const int A = a.A, H = a.H;
-    const float* p_rows = (region ? a.p_pool : a.p_conv) + ((long long)fb * N + r0) * A;
-    const float* f_rows = (region ? a.pool : a.conv) + ((long long)fb * N + r0) * H;
+    const float* p_rows = (region ? a.p_pool : a.p_conv) + (frow * N + r0) * A;
+    const float* f_rows = (region ? a.pool : a.conv) + (frow * N + r0) * H;
     const int rows_pa = ATT_STAGE_BYTES / (A * 4), rows_pb = ATT_STAGE_BYTES / (H * 4);
     const bool featmap = a.mode == GVD_ATT_INPUT_FEATMAP, dual = a.mode == GVD_ATT_INPUT_DUAL_REGION;
     // featmap: a region chunk's weighted sum never reaches the language LSTM, so its feature rows are not streamed (phase B is empty)
@@ -505,9 +518,10 @@ __global__ void __launch_bounds__(ATT_THREADS, FORM == GVD_REGION_ATTN_MIX ? 0 :
     else phase_a(FormTag<GVD_REGION_ATTN_MIX>{});
     consumer_bar();
     if (warp == 0) {
-        float m = -INFINITY;
+        float m = -INFINITY, s0 = -INFINITY;
+        if (n_out > 0) s0 = warp_sum(att_row_sum<AJ, GVD_REGION_ATTN_MIX>(a.ctx_bias, q4, w4, qs, ws, A, lane)) + bias;   // p_conv row = ctx_bias
         for (int r = lane; r < nrows; r += 32) m = fmaxf(m, z_s[r]);
-        m = warp_max(m);
+        m = fmaxf(warp_max(m), s0);
         float l = 0.f;
         for (int r = lane; r < nrows; r += 32) {
             const float e = expf(z_s[r] - m);
@@ -515,6 +529,7 @@ __global__ void __launch_bounds__(ATT_THREADS, FORM == GVD_REGION_ATTN_MIX ? 0 :
             l += e;
         }
         l = warp_sum(l);
+        if (n_out > 0) l = fmaf((float)n_out, expf(s0 - m), l);
         if (lane == 0) { ml[0] = m; ml[1] = l; }
     }
     consumer_bar();
@@ -544,7 +559,8 @@ __global__ void __launch_bounds__(ATT_THREADS, FORM == GVD_REGION_ATTN_MIX ? 0 :
     }
     float* out = a.partial + ((long long)b * nch + c) * (H + 4);
     if (tid == 0) { out[0] = ml[0]; out[1] = ml[1]; }
-    if (active && n_pb > 0) *reinterpret_cast<float4*>(out + 4 + h0) = acc;     // (featmap region chunks: no weighted sum to store)
+    // (featmap region chunks: no weighted sum to store; a video row's temporal chunk outside its window stores its zero sum)
+    if (active && !(featmap && region)) *reinterpret_cast<float4*>(out + 4 + h0) = acc;
     if (a.ticket == nullptr) return;
     // ---- fused combine: the last CTA of this row to finish merges all chunk partials (flash-decoding style).
     // Fixed merge order (chunk index), so the result does not depend on which CTA happens to be last.
@@ -711,6 +727,8 @@ int gvd_attn_partial(const AttnArgs& a, cudaStream_t st) {
     GVD_REQUIRE(a.A * 4 <= ATT_STAGE_BYTES && a.H * 4 <= ATT_STAGE_BYTES, "attn: row larger than a pipeline stage");
     GVD_REQUIRE(a.H <= ATT_CWARPS * 32 * 4, "attn: H=%d > %d not supported", a.H, ATT_CWARPS * 32 * 4);
     GVD_REQUIRE(a.RC >= 1 && a.RC <= ATT_MAXC && a.TC >= 1 && a.TC <= ATT_MAXC, "attn: chunk rows must be in [1,%d]", ATT_MAXC);
+    GVD_REQUIRE(!a.vid || (a.win && a.ctx_bias && ((uintptr_t)a.ctx_bias & 15) == 0),
+                "attn: video rows need the windows and a 16-byte aligned ctx2att bias");
     int nch_r, nch_t;
     gvd_attn_chunks(a.R, a.T, a.RC, a.TC, &nch_r, &nch_t);
     if (dual) nch_t = 0;                         // no temporal attention (AttModel.py:126-128: the frame features are dummies)

@@ -6,7 +6,7 @@
 // ---- row-wise prologue kernels (gvd_rowops.cu)
 int gvd_frame_mean(const float* segs, float* out, int B, int T, int C, cudaStream_t st);
 int gvd_clip_vector(const float* fc_mean, const long long* num, const float* Wseg, const float* bseg, float* xcat, int B,
-                    int C, int S, int ld, cudaStream_t st);
+                    int C, int S, int ld, cudaStream_t st, const long long* rows = nullptr);
 int gvd_sim_softmax(float* simT, const unsigned char* pnt_mask, int B, int R, int NC, int ld, cudaStream_t st);
 int gvd_transpose(const float* in, float* out, int B, int R, int C, int ld_in, cudaStream_t st);
 int gvd_transpose_split(const float* in, float* hi, float* lo, int B, int R, int C, int ld_in, cudaStream_t st);          // + tf32 hi/lo planes
@@ -72,6 +72,13 @@ struct AttnArgs {
     const float* gate_h; long long gate_ld;     //   h_att rows (pitch gate_ld)
     int form;                                   // GVD_REGION_ATTN_* (include/gvd_b200.h): the region attentions' score (the temporal one is
                                                 //   additive in every mode); DP reads no region alpha_net (w2 / b2, and w1 / b1 in DUAL_REGION)
+    // Video-indexed frame features (NULL vid: p_conv / conv are per clip).  Clip k attends over video vid[k]'s rows of the UNMASKED
+    // p_conv / conv [V,T,A|H], only inside its window [win[2k], win[2k+1]) ∩ [0,T).  The T - n_in rows outside hold zero features and
+    // p_conv = ctx_bias in the per-clip path, so they share one score s0 = w1 . tanh(ctx_bias + q) + b1 and add nothing to the weighted
+    // sum: the first temporal chunk folds (s0, T - n_in, 0) into its (max, sum, acc) record and no chunk streams an out-of-window row.
+    const long long* vid;                       // [B / feat_div] video of each clip
+    const long long* win;                       // [B / feat_div, 2] sample_idx
+    const float* ctx_bias;                      // [A] ctx2att.bias
 };
 int gvd_attn_chunks(int R, int T, int RC, int TC, int* nch_r, int* nch_t);
 int gvd_attn_partial(const AttnArgs& a, cudaStream_t st);

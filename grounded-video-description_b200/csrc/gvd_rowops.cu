@@ -26,13 +26,14 @@ __global__ void frame_mean_kernel(const float* __restrict__ segs, float* __restr
 
 // ---------------------------------------------------------------- clip vector assembly
 // xcat[b] = [ LN_C(fc) | LN_50(ReLU(W_seg . float(num[b,3:7]) + b_seg)) | 0-pad ]   (model.py:509-510)
+// rows (optional): clip b's mean is fc_mean row rows[b] (video-indexed batches: one mean per video)
 __global__ void clip_vector_kernel(const float* __restrict__ fc_mean, const long long* __restrict__ num,
                                    const float* __restrict__ Wseg, const float* __restrict__ bseg,
-                                   float* __restrict__ xcat, int C, int S, int ld) {
+                                   float* __restrict__ xcat, int C, int S, int ld, const long long* __restrict__ rows) {
     __shared__ float red[32];
     __shared__ float seg[64];
     const int b = blockIdx.x;
-    const float* x = fc_mean + (long long)b * C;
+    const float* x = fc_mean + (rows ? rows[b] : (long long)b) * C;
     float s = 0.f;
     for (int c = threadIdx.x; c < C; c += blockDim.x) s += x[c];
     const float mu = block_sum(s, red) / (float)C;
@@ -369,9 +370,9 @@ int gvd_frame_mean(const float* segs, float* out, int B, int T, int C, cudaStrea
     return 0;
 }
 int gvd_clip_vector(const float* fc_mean, const long long* num, const float* Wseg, const float* bseg, float* xcat, int B,
-                    int C, int S, int ld, cudaStream_t st) {
+                    int C, int S, int ld, cudaStream_t st, const long long* rows) {
     GVD_REQUIRE(S <= 64 && S <= 256, "clip_vector: seg_info_size %d too large", S);
-    clip_vector_kernel<<<B, 256, 0, st>>>(fc_mean, num, Wseg, bseg, xcat, C, S, ld);
+    clip_vector_kernel<<<B, 256, 0, st>>>(fc_mean, num, Wseg, bseg, xcat, C, S, ld, rows);
     GVD_CHECK_LAUNCH();
     return 0;
 }

@@ -163,10 +163,25 @@ class AttModel(CaptionModel):
     # ------------------------------------------------------------------ the reference's entry point
     def forward(self, segs_feat, seq, gt_seq, num, ppls, gt_boxes, mask_boxes, ppls_feat, frm_mask, sample_idx, pnt_mask, opt,
                 eval_opt={}):
+        """eval_opt['video_idx'] (int64 [B]): a video-indexed batch of B events.  segs_feat then holds the frame features of V videos
+        [V,T,F], passed once per video, and event b is the window sample_idx[b] of video video_idx[b]; every other tensor is per event.
+        The result equals the same call on segs_feat[video_idx] without the key.  Top-down captioner in eval mode only."""
+        video_idx = eval_opt.get("video_idx") if eval_opt else None
+        if video_idx is not None:
+            if self.att_model == "transformer":
+                raise NotImplementedError("video_idx: the transformer captioner's cross-attention reads per-clip frame encodings; pass "
+                                          "segs_feat[video_idx] without the key")
+            if self.training:
+                raise NotImplementedError("video_idx is an inference batch layout; training batches are random events: pass "
+                                          "segs_feat[video_idx] without the key")
+            if not torch.is_tensor(video_idx) or video_idx.device != segs_feat.device:
+                raise ValueError("video_idx must be a tensor on the device of segs_feat (%s)" % segs_feat.device)
         if opt == "MLE":
-            return self._forward(segs_feat, seq, gt_seq, ppls, gt_boxes, mask_boxes, num, ppls_feat, frm_mask, sample_idx, pnt_mask)
+            return self._forward(segs_feat, seq, gt_seq, ppls, gt_boxes, mask_boxes, num, ppls_feat, frm_mask, sample_idx, pnt_mask,
+                                 video_idx=video_idx)
         elif opt == "GRD":
-            return self._forward(segs_feat, seq, gt_seq, ppls, gt_boxes, mask_boxes, num, ppls_feat, frm_mask, sample_idx, pnt_mask, True)
+            return self._forward(segs_feat, seq, gt_seq, ppls, gt_boxes, mask_boxes, num, ppls_feat, frm_mask, sample_idx, pnt_mask, True,
+                                 video_idx=video_idx)
         elif opt == "sample":
             if self.att_model == "transformer":
                 # the reference cannot return here: it unpacks four values from the three its _sample returns in this mode (model.py:233,578);
@@ -176,11 +191,12 @@ class AttModel(CaptionModel):
             return seq, att2, sim_mat
         raise ValueError("unknown forward mode %r (expected 'MLE', 'GRD' or 'sample')" % (opt,))
 
-    def _prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, beam=1, nbox=0):
+    def _prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, beam=1, nbox=0, video_idx=None):
         nm = self._native_model()
         sim = nm.prologue(segs_feat.float().contiguous(), ppls.float().contiguous(), num.long().contiguous(),
                           ppls_feat.float().contiguous(), sample_idx.long().contiguous(), self._u8(pnt_mask).contiguous(),
-                          beam=beam, nbox=nbox)     # the workspace is sized for the decode that follows
+                          beam=beam, nbox=nbox,     # the workspace is sized for the decode that follows
+                          video_idx=video_idx.contiguous() if video_idx is not None else None)
         return nm, sim
 
     def _sample(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, opt={}):
@@ -194,6 +210,7 @@ class AttModel(CaptionModel):
         sample_max = opt.get("sample_max", 1)
         beam_size = opt.get("beam_size", 1)
         temperature = opt.get("temperature", 1.0)
+        video_idx = opt.get("video_idx")
         if beam_size > 1:
             if self.att_model == "transformer":
                 raise NotImplementedError("the transformer captioner decodes greedily (Decoder.greedy, transformer.py:214); the reference has no "
@@ -201,7 +218,7 @@ class AttModel(CaptionModel):
             return self._sample_beam(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, opt)
         if self.training:
             raise capi.GvdError("'sample' runs in eval mode (main.py:315); call model.eval()")
-        B, T = segs_feat.size(0), segs_feat.size(1)
+        B, T = ppls.size(0), segs_feat.size(1)
         if self.att_model == "transformer":
             nm, _ = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask)
             seq = self._tfm.decode_greedy(*self._tfm_encodings(nm, B, T))
@@ -212,7 +229,7 @@ class AttModel(CaptionModel):
             if not (math.isfinite(temperature) and temperature > 0):
                 raise ValueError("temperature must be finite and > 0 (got %r)" % (temperature,))
             seed = int(torch.randint(0, 2 ** 62, (1,)))
-        nm, sim = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask)
+        nm, sim = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, video_idx=video_idx)
         mask = self._u8(pnt_mask).contiguous()
         if sample_max:
             seq, logp, att2 = nm.decode_greedy(B, T, mask)
@@ -250,8 +267,8 @@ class AttModel(CaptionModel):
         beam_size = opt.get("beam_size", 10)
         if self.training:
             raise capi.GvdError("'sample' runs in eval mode (main.py:315); call model.eval()")
-        B, T = segs_feat.size(0), segs_feat.size(1)
-        nm, sim = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, beam=beam_size)
+        B, T = ppls.size(0), segs_feat.size(1)
+        nm, sim = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, beam=beam_size, video_idx=opt.get("video_idx"))
         seq, logp, att = nm.beam_decode(B, T, beam_size, self._u8(pnt_mask).contiguous())
         return seq, logp, att, sim
 
@@ -323,7 +340,7 @@ class AttModel(CaptionModel):
             raise IndexError("input_seq word/class id outside [0, %d]" % (V + D))
 
     def _forward(self, segs_feat, input_seq, gt_seq, ppls, gt_boxes, mask_boxes, num, ppls_feat, frm_mask, sample_idx, pnt_mask,
-                 eval_obj_ground=False):
+                 eval_obj_ground=False, video_idx=None):
         """Teacher-forced pass (model.py:283-489): 'MLE' -> (lm, att2, ground, cls) losses each of shape (1,)
         (model.py:483); 'GRD' -> (cls_pred [N,2] or 0 in test_mode, att2 idx [B,S,10], grounding idx [B,S,10]).
         model.eval(): eval-mode arithmetic through gvd_teacher_fwd; model.train() + 'MLE': the training forward with its explicit backward
@@ -334,7 +351,7 @@ class AttModel(CaptionModel):
             if eval_obj_ground:
                 raise capi.GvdError("'GRD' runs in eval mode (main.py:90); call model.eval()")
             return self._forward_train(segs_feat, input_seq, gt_seq, ppls, gt_boxes, mask_boxes, num, ppls_feat, frm_mask, sample_idx, pnt_mask)
-        B, T, L = segs_feat.size(0), segs_feat.size(1), self.seq_length
+        B, T, L = ppls.size(0), segs_feat.size(1), self.seq_length
         seq = torch.cat((gt_seq.new_zeros(B, 1), gt_seq[:, 0, :]), dim=1).long().contiguous()          # model.py:285-286
         col_any = (seq[:, 1:L] != 0).any(dim=0)                                                          # model.py:425 early exit
         dead = (~col_any).nonzero()
@@ -343,7 +360,7 @@ class AttModel(CaptionModel):
         self._check_ids(seq, input_cls)
         nbox = gt_boxes.size(1)
         pm = self._u8(pnt_mask).contiguous()
-        nm, _ = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, nbox=nbox)
+        nm, _ = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, nbox=nbox, video_idx=video_idx)
         fmask = self._u8(frm_mask).contiguous()
         if not eval_obj_ground:
             mb = self._u8(mask_boxes)[:, 0].contiguous()                                                 # seq_per_img == 1

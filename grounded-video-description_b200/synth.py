@@ -261,3 +261,30 @@ def make_inputs(opt, B, seed=1234, masked=True, train=False, nbox=3, cap_len=8):
     out["gt_seq"] = torch.from_numpy(gt_seq)
     out["mask_boxes"] = torch.from_numpy(box_mask)
     return out
+
+
+def make_video_inputs(opt, B, V, seed=1234, masked=True, train=False, nbox=3, cap_len=8):
+    """A video-indexed batch: B events of V videos (``TopDownModel.forward(..., eval_opt={'video_idx': ...})``).
+
+    Returns ``make_inputs(opt, B, ...)`` with ``segs_feat`` replaced by V videos' frame features [V, T, F] and a ``video_idx`` [B] (int64;
+    every video has an event when B >= V).  The windows ``sample_idx`` cycle through the cases the decode attention treats differently:
+    the whole clip, an empty window, one row, a window ending at T, one straddling a temporal chunk boundary, one reaching past T, and
+    seeded random windows."""
+    T = opt.t_attn_size
+    out = make_inputs(opt, B, seed=seed, masked=masked, train=train, nbox=nbox, cap_len=cap_len)
+    rs = _rs(seed, "video")
+    out["segs_feat"] = torch.from_numpy(rs.standard_normal((V, T, opt.fc_feat_size)).astype(np.float32))
+    vid = np.arange(B) % V
+    rs.shuffle(vid)
+    out["video_idx"] = torch.from_numpy(vid.astype(np.int64))
+    mid = max(1, T // 2)
+    fixed = [(0, T), (mid, mid), (mid, mid + 1), (max(0, T - 3), T), (max(0, mid - 2), min(T, mid + 2)), (max(0, T - 2), T + 5)]
+    sidx = np.zeros((B, 2), dtype=np.int64)
+    for b in range(B):
+        if b < len(fixed):
+            sidx[b] = fixed[b]
+        else:
+            lo = int(rs.randint(0, T))
+            sidx[b] = (lo, int(rs.randint(lo + 1, T + 1)))
+    out["sample_idx"] = torch.from_numpy(sidx)
+    return out

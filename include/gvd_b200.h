@@ -92,7 +92,7 @@ GVD_API size_t gvd_workspace_bytes(const gvd_model_t* m, int B, int T);
 GVD_API size_t gvd_workspace_bytes_beam(const gvd_model_t* m, int B, int T, int beam_size);   /* for gvd_beam_decode */
 /* Address of a named activation inside a workspace laid out for (B,T): "fc_feats" [B,H],
  * "g_pool" [B,R,2048], "pool_embed"/"pool_feats" [B,R,H], "p_pool_feats" [B,R,A],
- * "conv_feats" [B,T,H], "p_conv_feats" [B,T,A].  NULL if unknown. */
+ * "conv_feats" [B,T,H], "p_conv_feats" [B,T,A] ([V,T,H] / [V,T,A], unmasked, after gvd_prologue_fwd_video).  NULL if unknown. */
 GVD_API float* gvd_workspace_tensor(const gvd_model_t* m, void* workspace, int B, int T, const char* name);
 
 /* ---- P1-P7: everything _sample computes before the loop (misc/model.py:504-568) */
@@ -103,6 +103,30 @@ GVD_API int gvd_prologue_fwd(gvd_model_t* m, int B, int T,
                      const float* ppls_feat,        /* [B,R,att_feat_size]         */
                      const int64_t* sample_idx,     /* [B,2]                       */
                      const uint8_t* pnt_mask,       /* [B,R+1], leading 0 column   */
+                     void* workspace, size_t workspace_bytes,
+                     float* sim_mat_out,            /* [B,D+1,R] or NULL           */
+                     void* stream);
+
+/* ---- video-indexed batch: B events (clips) of V videos, the frame features passed once per video.  The result equals gvd_prologue_fwd
+ * on segs_feat[video_idx] (and every decode entry point after it equals the per-clip decode), with less traffic and work:
+ *   - the frame mean and the frame branch (att_embed, BatchNorm, bi-GRU, ctx2att) run on the V videos, UNMASKED: the workspace holds
+ *     conv_feats [V,T,H] / p_conv_feats [V,T,A] instead of B masked copies; clip b's clip vector reads video video_idx[b]'s mean;
+ *   - the region stages are per clip as in gvd_prologue_fwd;
+ *   - the decode attention of clip b reads only the rows of video video_idx[b] inside its window sample_idx[b] = [lo, hi) ∩ [0,T) and adds
+ *     the closed form of the T - n_in rows outside it (in the per-clip path: zero features, p_conv = ctx2att.bias, one shared score).
+ * Workspace: gvd_workspace_bytes_video(B, V, T, beam_size, nbox) (beam_size 1 / nbox 0 for the greedy and sampling loops).  The prologue
+ * copies video_idx and sample_idx into it and records the workspace as video-indexed: gvd_decode_greedy / _sample / gvd_beam_decode /
+ * gvd_teacher_fwd / gvd_decode_step_fwd / gvd_workspace_tensor with the same (B,T) then use that layout, until gvd_prologue_fwd runs on
+ * the same workspace.  video_idx must lie in [0,V) (not checked on the device). */
+GVD_API size_t gvd_workspace_bytes_video(const gvd_model_t* m, int B, int V, int T, int beam_size, int nbox);
+GVD_API int gvd_prologue_fwd_video(gvd_model_t* m, int B, int V, int T,
+                     const float* segs_feat,        /* [V,T,fc_feat_size]          */
+                     const float* ppls,             /* [B,R,7]                     */
+                     const int64_t* num,            /* [B,7]                       */
+                     const float* ppls_feat,        /* [B,R,att_feat_size]         */
+                     const int64_t* sample_idx,     /* [B,2] each clip's window    */
+                     const int64_t* video_idx,      /* [B] in [0,V)                */
+                     const uint8_t* pnt_mask,       /* [B,R+1]                     */
                      void* workspace, size_t workspace_bytes,
                      float* sim_mat_out,            /* [B,D+1,R] or NULL           */
                      void* stream);
@@ -174,6 +198,14 @@ GVD_API int gvd_teacher_fwd(gvd_model_t* m, int B, int T, int nbox, int S, int m
 GVD_API int gvd_sample_greedy_host(gvd_model_t* m, int B, int T,
                            const float* h_segs_feat, const float* h_ppls, const int64_t* h_num,
                            const float* h_ppls_feat, const int64_t* h_sample_idx, const uint8_t* h_pnt_mask,
+                           void* workspace, size_t workspace_bytes,
+                           int64_t* h_seq_out, float* h_logprobs_out, float* h_att2_out, float* h_sim_mat_out,
+                           void* stream);
+/* the same for a video-indexed batch (see gvd_prologue_fwd_video): h_segs_feat [V,T,F], so V videos' frames cross PCIe instead of B
+ * copies; h_video_idx [B] is checked on the host.  Workspace: gvd_workspace_bytes_video(B, V, T, 1, 0). */
+GVD_API int gvd_sample_greedy_host_video(gvd_model_t* m, int B, int V, int T,
+                           const float* h_segs_feat, const float* h_ppls, const int64_t* h_num,
+                           const float* h_ppls_feat, const int64_t* h_sample_idx, const int64_t* h_video_idx, const uint8_t* h_pnt_mask,
                            void* workspace, size_t workspace_bytes,
                            int64_t* h_seq_out, float* h_logprobs_out, float* h_att2_out, float* h_sim_mat_out,
                            void* stream);
@@ -305,6 +337,15 @@ GVD_API int gvd_op_attention_form(const float* p_pool, const float* pool, const 
                   int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld, int B, int R, int T, int A, int H, int RC, int TC,
                   int feat_div, int att_input_mode, const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld,
                   int region_attn_mode, void* stream);
+/* gvd_op_attention_video: gvd_op_attention_form over video-level frame features: p_conv / conv [V,T,A|H] unmasked, video_idx [B / feat_div]
+ *   int64 in [0,V), sample_idx [B / feat_div, 2] the windows, ctx_bias [A] (ctx2att.bias, 16-byte aligned): the temporal attention of row b
+ *   equals gvd_op_attention_form on conv[video] with the rows outside the window zeroed and p_conv there = ctx_bias. */
+GVD_API int gvd_op_attention_video(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                  const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2, const float* b2,
+                  const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out, int64_t z_stride_b, float* partial,
+                  int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld, int B, int R, int T, int A, int H, int RC, int TC,
+                  int feat_div, int att_input_mode, const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld,
+                  int region_attn_mode, const int64_t* video_idx, const int64_t* sample_idx, const float* ctx_bias, void* stream);
 /* beam_topk: per row of logits [rows, V] (pitch ld) the K <= 8 (K <= V) best words, value descending, ties to the lower index:
  *   topv [rows, K] = their log_softmax, topi [rows, K].  NaN words are skipped; a pick that finds only NaN left takes the lowest untaken
  *   index, so an all-NaN row gives 0 .. K-1 (as a stable torch.sort(descending=True) does).  Rows only partly NaN differ from torch,
