@@ -2,7 +2,6 @@
 // decode orchestration.  Host code only launches kernels; there is no CPU compute path.
 #include <atomic>
 #include <mutex>
-#include <chrono>
 #include <cmath>
 #include <cstdarg>
 #include <cstdlib>
@@ -31,13 +30,13 @@ extern "C" GVD_API const char* gvd_version(void) { return "gvd-b200 0.1.0 (sm_90
 extern "C" GVD_API int gvd_op_kernel_launches(void) { return (int)g_launches.load(); }
 // backend switches (gvd_set_backend): bit 0 wgmma tensor cores for every GEMM-shaped stage (0 = fp32 CUDA cores); bit 1 fused self-attention
 // pair; bit 2 (4) inert (it selected 256-column tiles of a kernel that needed tensor memory); bit 3 (8) operand-swapped split-K decode products
-// with fused reduce + sampler; bit 4 (16) fp16x3 instead of 3xTF32 in the forward GEMMs (pre-split constant weights); bit 5 (32) cooperative
-// GRU layer kernel (off); bit 6 (64) programmatic dependent launch in the decode loop (off); bit 7 (128) conversion-free GEMMs for the
-// prologue (activations packed into the fp16x3 image, both operands straight from TMA); bit 8 (256)
+// with fused reduce + sampler; bit 4 (16) fp16x3 instead of 3xTF32 in the forward GEMMs (pre-split constant weights); bit 5 (32) inert (it
+// selected a cooperative GRU layer kernel); bit 6 (64) programmatic dependent launch in the decode loop (off); bit 7 (128) conversion-free
+// GEMMs for the prologue (activations packed into the fp16x3 image, both operands straight from TMA); bit 8 (256)
 // fp16x3 images instead of tf32 planes in the fused self-attention pair; bit 9 (512) pack fusion: the producer of a prologue activation (GEMM
 // epilogue / row kernel) stores the fp16x3 operand image the next GEMM streams, instead of a separate pack pass; bit 10 (1024) inert (it
-// selected CTA pairs).  Bits 2 and 10 are accepted so that stored flag values keep working; nothing reads them.
-// Default 923 = 1 + 2 + 8 + 16 + 128 + 256 + 512.
+// selected CTA pairs).  Bits 2, 5 and 10 are accepted so that stored flag values keep working; nothing reads them.  Names: GvdBackendBit
+// (gvd_common.cuh).  Default 923 = 1 + 2 + 8 + 16 + 128 + 256 + 512.
 static std::atomic<int> g_backend{923};
 int gvd_backend() { return g_backend.load(std::memory_order_relaxed); }
 // registry of pre-split constant weights (fp16x3 variant): fp32 weight pointer -> packed image
@@ -54,10 +53,10 @@ bool gvd_packed_lookup(const float* W, long long ldw, int N, int K, const float*
     *ld_packed = it->second.ld;
     return true;
 }
-bool gvd_pdl() { return (g_backend.load(std::memory_order_relaxed) & 64) != 0; }
+bool gvd_pdl() { return gvd_backend_on(BK_PDL); }
 static thread_local int g_f16_depth = 0;
 void gvd_f16_scope(int delta) { g_f16_depth += delta; }
-bool gvd_gemm_f16() { return g_f16_depth > 0 && (g_backend.load(std::memory_order_relaxed) & 16) != 0; }
+bool gvd_gemm_f16() { return g_f16_depth > 0 && gvd_backend_on(BK_F16X3); }
 extern "C" GVD_API int gvd_set_backend(int flags) { g_backend.store(flags); return 0; }
 extern "C" GVD_API int gvd_get_backend(void) { return g_backend.load(); }
 
@@ -564,7 +563,6 @@ struct WS {
                                              // a pack pass: [BR, H] (region embedding / encoder state), [BR, H/2] (FFN hidden), [BR, 2048] (fc7)
     int sk_ldp;
     long long* it;
-    unsigned int* gru_bar;             // [2] arrival counters of the persistent GRU layer kernel
     float* h_img;                      // [2 parity][2 dir][B][G] words: fp16x3 images of the GRU state (tensor-core step kernel)
     int* ticket;                       // [rows] last-CTA tickets of the fused attention combine
     float* pk_part; int* pk_ticket;    // fused vocabulary head + greedy pick: per-CTA partials, one ticket
@@ -594,9 +592,6 @@ static void attn_chunking(int B, int R, int T, int* RC, int* TC) {
     };
     *RC = pick(R);
     *TC = pick(T);
-    // measurement aid: rows per region chunk (the CTA count of the decode attention: B * (ceil(R / RC) + ceil(T / TC)) on 2 CTAs per SM)
-    if (const char* e = getenv("GVD_ATTN_RC")) { const int v = atoi(e); if (v >= 16 && v <= 128) *RC = (v + 7) / 8 * 8; }
-    if (const char* e = getenv("GVD_ATTN_TC")) { const int v = atoi(e); if (v >= 16 && v <= 128) *TC = (v + 7) / 8 * 8; }
 }
 
 static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, int nbox = 0, int V = 0) {
@@ -617,10 +612,6 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     // the attention kernels run one CTA per (clip, head, 128 query rows) and one CTA per SM: a chunk that is one full wave
     // (132 SMs -> 2 clips x 6 heads x 8 row blocks = 96 CTAs at R = 1000) has no partial second wave
     w.clip_chunk = std::max(1, std::min(w.clip_chunk, 132 / std::max(1, m->nheads * ((R + 127) / 128))));
-    {
-        static const int env_chunk = getenv("GVD_CLIP_CHUNK") ? atoi(getenv("GVD_CLIP_CHUNK")) : 0;
-        if (env_chunk > 0) w.clip_chunk = std::min(B, env_chunk);
-    }
     w.in_segs = (float*)take(BT * d.fc_feat_size * 4);
     w.in_ppls = (float*)take(BR * 7 * 4);
     w.in_feat = (float*)take(BR * d.att_feat_size * 4);
@@ -670,7 +661,6 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     w.p_conv = (float*)take(BT * A * 4);
     w.gh = (float*)take((size_t)2 * NV * 3 * G * 4);
     w.hstate = (float*)take((size_t)2 * 2 * NV * G * 4);
-    w.gru_bar = (unsigned int*)take(256);
     w.h_img = (float*)take((size_t)2 * 2 * NV * G * 4);
     w.a_pk_frame = (float*)take(BT * (size_t)((std::max(H, 2 * G) + 31) / 32 * 32 + 32) * 4);   // the frame branch's own pack buffer (it runs concurrently with the region stages)
     w.pre_att = (float*)take((size_t)B * 4 * H * 4);
@@ -686,7 +676,7 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     w.xt = (float*)take(BD * d.input_encoding_size * 4);
     w.sk_ldp = (int)rup(BD, 4);
     w.xcat_att = w.xcat_lang = w.sk_part = w.xp_att = w.xp_lang = nullptr;
-    if (BD <= 128) {    // operand-swapped split-K path (experimental, backend bit 3): at most 132 (weight-row tile, K split) pairs per product
+    if (BD <= 128) {    // operand-swapped split-K path (BK_SPLITK): at most 132 (weight-row tile, K split) pairs per product
         w.xcat_att = (float*)take(BD * (size_t)(d.input_encoding_size + H) * 4);
         w.xcat_lang = (float*)take(BD * (size_t)3 * H * 4);
         w.sk_part = (float*)take((size_t)132 * 128 * w.sk_ldp * 4 + (size_t)BD * 64);      // [S][B][ldp], S * ceil(Nw/128) <= 132, ldp <= Nw + 3
@@ -814,12 +804,12 @@ static int check_ws(const gvd_model* m, int B, int T, void* workspace, size_t by
 static bool linear_w_f16ss(const WS& w, const float* W, long long ldw, int M, int N, int K, const float** Wp = nullptr, long long* ldwp = nullptr) {
     const float* p = nullptr;
     long long l = 0;
-    const bool ok = (gvd_backend() & 128) != 0 && gvd_gemm_f16() && M >= 1024 && w.a_pk && gvd_packed_lookup(W, ldw, N, K, &p, &l);
+    const bool ok = gvd_backend_on(BK_SS_GEMM) && gvd_gemm_f16() && M >= 1024 && w.a_pk && gvd_packed_lookup(W, ldw, N, K, &p, &l);
     if (Wp) *Wp = p;
     if (ldwp) *ldwp = l;
     return ok;
 }
-static bool pack_fusion() { return (gvd_backend() & 512) != 0; }      // backend bit 9
+static bool pack_fusion() { return gvd_backend_on(BK_PACK_FUSION); }
 static int linear_w(const WS& w, const float* A, long long lda, const float* W, long long ldw, const float* bias, float* C, long long ldc, int M, int N,
                     int K, int act, cudaStream_t st, const float* scale2 = nullptr, const float* shift2 = nullptr, const float* A_img = nullptr,
                     float* C_img = nullptr) {
@@ -859,14 +849,13 @@ static int obj_interact_fwd(const gvd_model* m, const WS& w0, int c0, int B, cud
     for (int l = 0; l < 2; ++l) {
         const std::string p = "obj_interact.encoder.layers." + std::to_string(l) + ".";
         // Q|K|V projections for every region in one GEMM (bias-free, transformer.py:111-114,119)
-        const bool fused = (gvd_backend() & 3) == 3 && HS <= 192;
-        const bool att16 = fused && (gvd_backend() & 256) != 0 && w.k_img != nullptr;      // fp16x3 images instead of tf32 planes (bit 8)
+        const bool fused = gvd_backend_on(BK_TC | BK_FUSED_ATTN) && HS <= 192;
+        const bool att16 = fused && gvd_backend_on(BK_ATT_F16) && w.k_img != nullptr;      // fp16x3 images instead of tf32 planes
         const int KH = (HS + 31) / 32 * 32, Rp = (R + 31) / 32 * 32;
         // pack fusion of the attention operands: the projection's epilogue stores Q as fp32, K as the per-head image and V as the image of V^T
-        static const bool no_qkv_img = getenv("GVD_NO_QKV_IMG") != nullptr;
         const float* Wp = nullptr;
         long long ldwp = 0;
-        const bool qkv_img = fuse && att16 && !no_qkv_img && R % 2 == 0 && HS % 4 == 0 && linear_w_f16ss(w, m->wqk[l], H, (int)BR, 3 * HP, H, &Wp, &ldwp);
+        const bool qkv_img = fuse && att16 && R % 2 == 0 && HS % 4 == 0 && linear_w_f16ss(w, m->wqk[l], H, (int)BR, 3 * HP, H, &Wp, &ldwp);
         if (qkv_img) {
             GvdQkvImages qi{HP, HS, KH, nh, R, Rp, w.k_img, w.vt_img, GVD_ATT_SK, GVD_ATT_SV};
             ProfScope _pk("kernel.f16ss_gemm", st);
@@ -986,19 +975,13 @@ static int frame_branch_fwd(const gvd_model* m, const WS& w0, int B, int T, cons
         const int in = l == 0 ? H : 2 * G;
         float* out = l == 0 ? w.gru_out0 : w.conv;
         GVD_STAGE("frame.gru_in", linear_w(w, xin, in, m->gru_wih[l], in, m->gru_bih[l], w.gi, 6 * G, (int)BT, 6 * G, in, GVD_ACT_NONE, st));
-        if ((gvd_backend() & 32) != 0 && G % 4 == 0 && G <= 1024) {
-            // persistent layer kernel: W_hh resident in shared memory, one cooperative launch for all T steps of both directions
-            GVD_STAGE("frame.gru_layer", gvd_gru_layer(w.gi, m->gru_whh[l], m->gru_bhh[l], w.hstate, out, l == 1 ? sample_idx : nullptr, w.gru_bar, B, T, G, st));
-            continue;
-        }
         GVD_CHECK_CUDA(cudaMemsetAsync(w.hstate, 0, (size_t)2 * 2 * B * G * sizeof(float), st));
         {
             // tensor-core step kernel (bit 4): gh = W_hh h on wgmma from two pre-split operands with the gate math in the epilogue — one
             // launch per time step instead of a CUDA-core GEMM + a pointwise kernel
-            static const bool old_gru = getenv("GVD_GRU_OLD") != nullptr;
             const float* Wimg = nullptr;
             long long ldw = 0;
-            if (!old_gru && gvd_gemm_f16() && B <= 128 && G % 32 == 0 && gvd_packed_lookup(m->gru_whh[l], G, 6 * G, G, &Wimg, &ldw)) {
+            if (gvd_gemm_f16() && B <= 128 && G % 32 == 0 && gvd_packed_lookup(m->gru_whh[l], G, 6 * G, G, &Wimg, &ldw)) {
                 GVD_STAGE("frame.gru_layer_tc", gvd_gru_layer_f16(w.gi, Wimg, m->gru_bhh[l], w.hstate, w.h_img, out, l == 1 ? sample_idx : nullptr, B, T, G, st));
                 continue;
             }
@@ -1070,14 +1053,14 @@ static int frame_stages(const gvd_model* m, const WS& w, int B, int T, const flo
 
 // The frame stages next to the region stages (P2-P6) instead of behind them: the bi-GRU is 2 * 2 * T dependent launches of a few CTAs
 // that nothing else in the prologue depends on.  They run on a second stream; no GEMM here is persistent, so the chain's CTAs find SMs as
-// the region kernels' CTAs retire.  Off under the stage profiler (its per-stage times are meant to be serial) or with GVD_NO_FRAME_OVERLAP.
-static bool frame_overlap_on() { return g_prof_on.load(std::memory_order_relaxed) == 0 && getenv("GVD_NO_FRAME_OVERLAP") == nullptr; }
+// the region kernels' CTAs retire.  Off under the stage profiler (its per-stage times are meant to be serial).
+static bool frame_overlap_on() { return g_prof_on.load(std::memory_order_relaxed) == 0; }
 static int frame_fork(gvd_model* m, cudaStream_t st) {
     if (!m->frame_stream) {
         int lo = 0, hi = 0;
         GVD_CHECK_CUDA(cudaDeviceGetStreamPriorityRange(&lo, &hi));
-        // lowest priority by default: at the highest one the GRU chain can hold back every region kernel until it ends
-        GVD_CHECK_CUDA(cudaStreamCreateWithPriority(&m->frame_stream, cudaStreamNonBlocking, getenv("GVD_FRAME_PRIO_HIGH") ? hi : lo));
+        // lowest priority: at the highest one the GRU chain can hold back every region kernel until it ends
+        GVD_CHECK_CUDA(cudaStreamCreateWithPriority(&m->frame_stream, cudaStreamNonBlocking, lo));
         GVD_CHECK_CUDA(cudaEventCreateWithFlags(&m->ev_fork, cudaEventDisableTiming));
         GVD_CHECK_CUDA(cudaEventCreateWithFlags(&m->ev_join, cudaEventDisableTiming));
     }
@@ -1103,41 +1086,14 @@ static int prologue_run(gvd_model_t* m, int B, int V, int T, const float* segs_f
         GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_vid, video_idx, (size_t)B * 8, cudaMemcpyDeviceToDevice, st));
         GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_sidx, sample_idx, (size_t)B * 2 * 8, cudaMemcpyDeviceToDevice, st));
     }
-    const gvd_dims_t& d = m->d;
-    const int R = m->R;
     const bool overlap = frame_overlap_on();
     cudaStream_t fst = st;
-    // GVD_TRACE_OVERLAP: when did each stream finish (ms after the fork)?  Diagnostic only: synchronises the stream.
-    const bool otrace = overlap && getenv("GVD_TRACE_OVERLAP") != nullptr;
-    cudaEvent_t te[3] = {nullptr, nullptr, nullptr};
-    if (otrace) for (auto& e : te) GVD_CHECK_CUDA(cudaEventCreate(&e));
     if (overlap) { GVD_TRY(frame_fork(m, st)); fst = m->frame_stream; }
-    if (otrace) GVD_CHECK_CUDA(cudaEventRecord(te[0], st));
     const int rc_frame = frame_stages(m, w, B, T, segs_feat, (const long long*)num, (const long long*)sample_idx, fst, V > 0 ? w.in_vid : nullptr);
-    if (otrace) GVD_CHECK_CUDA(cudaEventRecord(te[1], fst));
     if (overlap && rc_frame != 0) frame_join(m, st);            // never leave the second stream dangling behind an error return
     if (rc_frame != 0) return rc_frame;
-    int rc = 0;
-    if (getenv("GVD_CHUNKED")) {          // measurement aid: the chunked schedule of the host-buffer entry point, without the copies
-        const int chunk = std::max(1, std::min(B, atoi(getenv("GVD_CHUNKED"))));
-        for (int c0 = 0; c0 < B && rc == 0; c0 += chunk) {
-            const int cb = std::min(chunk, B - c0);
-            rc = region_prologue(m, w, c0, cb, ppls + (size_t)c0 * R * 7, ppls_feat + (size_t)c0 * R * d.att_feat_size, pnt_mask + (size_t)c0 * (R + 1),
-                                 sim_mat_out ? sim_mat_out + (size_t)c0 * m->NC * R : nullptr, st);
-        }
-    } else {
-        rc = region_prologue(m, w, 0, B, ppls, ppls_feat, pnt_mask, sim_mat_out, st);          // P2-P6
-    }
-    if (otrace) GVD_CHECK_CUDA(cudaEventRecord(te[2], st));
+    const int rc = region_prologue(m, w, 0, B, ppls, ppls_feat, pnt_mask, sim_mat_out, st);          // P2-P6
     if (overlap) GVD_TRY(frame_join(m, st));
-    if (otrace) {
-        GVD_CHECK_CUDA(cudaStreamSynchronize(st));
-        float a = 0.f, b = 0.f;
-        cudaEventElapsedTime(&a, te[0], te[1]);
-        cudaEventElapsedTime(&b, te[0], te[2]);
-        fprintf(stderr, "[gvd] overlap trace: frame stream done %.2f ms, region stages done %.2f ms after the fork\n", a, b);
-        for (auto& e : te) cudaEventDestroy(e);
-    }
     return rc;
 }
 extern "C" GVD_API int gvd_prologue_fwd(gvd_model_t* m, int B, int T, const float* segs_feat, const float* ppls, const int64_t* num,
@@ -1179,7 +1135,7 @@ extern "C" GVD_API int gvd_decode_reset_state(gvd_model_t* m, int B, int T, void
 static bool core_skinny(const gvd_model* m, const WS& w, int B, int div) {
     const gvd_dims_t& d = m->d;
     const int H = d.rnn_size, A = d.att_hid_size, E = d.input_encoding_size;
-    return (gvd_backend() & 1) != 0 && H % 8 == 0 && (gvd_backend() & 8) != 0 && div == 1 && w.sk_part != nullptr && E % 4 == 0 &&
+    return gvd_backend_on(BK_TC | BK_SPLITK) && H % 8 == 0 && div == 1 && w.sk_part != nullptr && E % 4 == 0 &&
            gvd_skinny_splits(4 * H, E + H, B) > 0 && gvd_skinny_splits(2 * A, H, B) > 0 && gvd_skinny_splits(4 * H, 3 * H, B) > 0;
 }
 
@@ -1187,7 +1143,7 @@ static bool core_skinny(const gvd_model* m, const WS& w, int B, int div) {
 // granularity of every concatenated segment)
 static bool core_skinny_f16(const gvd_model* m) {
     const gvd_dims_t& d = m->d;
-    return (gvd_backend() & 16) != 0 && d.rnn_size % 32 == 0 && d.input_encoding_size % 32 == 0 && d.att_hid_size % 16 == 0;
+    return gvd_backend_on(BK_F16X3) && d.rnn_size % 32 == 0 && d.input_encoding_size % 32 == 0 && d.att_hid_size % 16 == 0;
 }
 
 // B = decode rows (clips x beam); rows [k*div, (k+1)*div) attend over clip k's features / masks
@@ -1202,8 +1158,8 @@ static int core_step(const gvd_model* m, const WS& w, int B, int T, int step, co
     float* h_att_nxt = w.h_att + (size_t)((step + 1) & 1) * BH;
     float* h_lang_cur = w.h_lang + (size_t)(step & 1) * BH;
     float* h_lang_nxt = w.h_lang + (size_t)((step + 1) & 1) * BH;
-    const bool tc = (gvd_backend() & 1) != 0 && H % 8 == 0;
-    // operand-swapped split-K products (gvd_skinny.cu): experimental, backend bit 3; one `pre` row per batch row only
+    const bool tc = gvd_backend_on(BK_TC) && H % 8 == 0;
+    // operand-swapped split-K products (gvd_skinny.cu, BK_SPLITK); one `pre` row per batch row only
     const bool skinny = core_skinny(m, w, B, div);
     const bool sk16 = skinny && core_skinny_f16(m);     // both operands pre-split: conversion-free products (skinny_f16_kernel)
     {   // attention LSTM: input cat(fc_feats, xt), xt = ReLU(embed[token]) (AttModel.py:138-139)
@@ -1336,7 +1292,7 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
     // sampler into the vocabulary-head GEMM epilogue (MODE_PICK of wg_gemm_kernel, last-CTA merge of the per-CTA partials) is
     // implemented and compared with the two other samplers and an fp64 reference in tests/test_gpu_decode_ops.py (through
     // gvd_op_logit_pick_tc); its merge is a serial chain on one CTA, so the loop only uses it when GVD_FUSED_PICK is set.
-    const bool tc = (gvd_backend() & 1) != 0 && H % 8 == 0;
+    const bool tc = gvd_backend_on(BK_TC) && H % 8 == 0;
     static const bool fused_pick = getenv("GVD_FUSED_PICK") != nullptr;
     const bool fused = tc && fused_pick && B <= 128 && !sample;     // the fused head has no multinomial sampler: sampling takes the split-K path
     for (int t = 0; t < L; ++t) {
@@ -1348,7 +1304,7 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
                                                              m->P("embed.0.weight"), w.xt, d.input_encoding_size, st));
         } else {
             const int E = d.input_encoding_size;
-            const int S = (tc && (gvd_backend() & 8) != 0 && w.sk_part) ? gvd_skinny_splits(V, H, B) : 0;
+            const int S = (tc && gvd_backend_on(BK_SPLITK) && w.sk_part) ? gvd_skinny_splits(V, H, B) : 0;
             const bool sk_core = core_skinny(m, w, B, 1);                       // then xt goes into the core step's concatenated input
             const bool sk16 = sk_core && core_skinny_f16(m);                    // ... and its fp16x3 image into xp_att
             // above 6144 words (reduce_pick / reduce_sample hold a row in one CTA's registers): the sliced tail, one CTA per (row, 1024 words)
@@ -1619,28 +1575,10 @@ extern "C" GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_si
 // Clip chunks of the host-buffer entry point.  The pipeline starts with one attention sub-batch (`unit` clips: the first kernel waits for the
 // first copy) and grows 1, 2, 3, 6, 9, 12, 12 ... units, so that the copy engine stays ahead of the compute stream; a short remainder joins
 // the last chunk.  The growth rule has not been re-tuned for the H100.
-// GVD_H2D_SCHED="3,6,9,..." (clips per chunk; a short list repeats its last entry) or GVD_H2D_CHUNK=n (uniform) override the rule.
 static std::vector<int> h2d_schedule(int B, int unit) {
     std::vector<int> s;
     int left = B;
     auto push = [&](int n) { n = std::max(1, std::min(n, left)); s.push_back(n); left -= n; };
-    if (const char* e = getenv("GVD_H2D_SCHED")) {
-        int last = 0;
-        for (const char* p = e; *p && left > 0;) {
-            char* q = nullptr;
-            const long v = strtol(p, &q, 10);
-            if (q == p) break;
-            if (v > 0) { last = (int)v; push(last); }
-            p = (*q == ',') ? q + 1 : q;
-        }
-        while (left > 0) push(last > 0 ? last : left);
-        return s;
-    }
-    if (const char* e = getenv("GVD_H2D_CHUNK")) {
-        const int c = std::max(1, atoi(e));
-        while (left > 0) push(c);
-        return s;
-    }
     const int grow[5] = {1, 2, 3, 6, 9};
     for (int i = 0; i < 5 && left > 0; ++i) push(left < (grow[i] + 2) * unit ? left : grow[i] * unit);
     while (left > 0) push(left < 16 * unit ? left : 12 * unit);
@@ -1691,15 +1629,12 @@ static int sample_greedy_host_run(gvd_model_t* m, int B, int V, int T, const flo
     if (big_segs) {
         segs_after = nchunks;
         if (overlap) {
-            const int want = getenv("GVD_H2D_SEGS_AFTER") ? atoi(getenv("GVD_H2D_SEGS_AFTER")) : (3 * B + 9) / 10;      // clips
+            const int want = (3 * B + 9) / 10;      // clips
             int acc = 0;
             segs_after = 0;
             while (segs_after < nchunks && acc < want) acc += sched[segs_after++];
         }
     }
-    const bool trace = getenv("GVD_TRACE") != nullptr;
-    const auto t_begin = std::chrono::steady_clock::now();
-    auto ms_since = [&]() { return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_begin).count(); };
     GVD_CHECK_CUDA(cudaEventRecord(ev_start, st));                       // the workspace may still be in use by earlier work on `st`
     GVD_CHECK_CUDA(cudaStreamWaitEvent(m->copy_stream, ev_start, 0));
     if (!big_segs) GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_segs, h_segs_feat, BT * FC * 4, cudaMemcpyHostToDevice, st));
@@ -1730,7 +1665,6 @@ static int sample_greedy_host_run(gvd_model_t* m, int B, int V, int T, const flo
         }
         if (big_segs && segs_after >= nchunks) GVD_TRY(copy_segs());
     }
-    if (trace) fprintf(stderr, "[gvd] %.2f ms: copies enqueued (%d chunks, frame features after chunk %d)\n", ms_since(), nchunks, big_segs ? segs_after : 0);
     int rc = 0;
     bool frame_done = false;
     auto run_frame = [&]() -> int {
@@ -1754,7 +1688,6 @@ static int sample_greedy_host_run(gvd_model_t* m, int B, int V, int T, const flo
     if (rc == 0 && !frame_done) rc = run_frame();
     if (overlap) { const int jr = frame_join(m, st); if (rc == 0) rc = jr; }
     if (rc != 0) { cudaStreamSynchronize(m->copy_stream); return rc; }            // (the copies read caller memory: never return with them in flight)
-    if (trace) fprintf(stderr, "[gvd] %.2f ms: prologue enqueued\n", ms_since());
     if (h_sim_mat_out) {   // the similarity matrix is final here: its D2H overlaps the 20-step decode loop
         GVD_CHECK_CUDA(cudaEventRecord(ev_sim, st));
         GVD_CHECK_CUDA(cudaStreamWaitEvent(m->copy_stream, ev_sim, 0));
@@ -1764,11 +1697,8 @@ static int sample_greedy_host_run(gvd_model_t* m, int B, int V, int T, const flo
     GVD_CHECK_CUDA(cudaMemcpyAsync(h_seq_out, w.out_seq, (size_t)B * L * 8, cudaMemcpyDeviceToHost, st));
     if (h_logprobs_out) GVD_CHECK_CUDA(cudaMemcpyAsync(h_logprobs_out, w.out_logp, (size_t)B * L * 4, cudaMemcpyDeviceToHost, st));
     if (h_att2_out) GVD_CHECK_CUDA(cudaMemcpyAsync(h_att2_out, w.out_att2, (size_t)B * L * R * 4, cudaMemcpyDeviceToHost, st));
-    if (trace) fprintf(stderr, "[gvd] %.2f ms: everything enqueued\n", ms_since());
     GVD_CHECK_CUDA(cudaStreamSynchronize(st));
-    if (trace) fprintf(stderr, "[gvd] %.2f ms: compute stream drained\n", ms_since());
     GVD_CHECK_CUDA(cudaStreamSynchronize(m->copy_stream));
-    if (trace) fprintf(stderr, "[gvd] %.2f ms: copy stream drained\n", ms_since());
     return 0;
 }
 extern "C" GVD_API int gvd_sample_greedy_host(gvd_model_t* m, int B, int T, const float* h_segs_feat, const float* h_ppls, const int64_t* h_num,
@@ -2147,7 +2077,7 @@ extern "C" GVD_API int gvd_op_self_attention_tc(const float* qkv, float* out, in
     cudaStream_t st = (cudaStream_t)stream;
     const size_t BR = (size_t)nb * R;
     float *khi = nullptr, *klo = nullptr, *vh = nullptr, *vl = nullptr;
-    const bool att16 = (gvd_backend() & 256) != 0;          // fp16x3 images instead of tf32 planes (same switch as the prologue)
+    const bool att16 = gvd_backend_on(BK_ATT_F16);          // fp16x3 images instead of tf32 planes (same switch as the prologue)
     const int KH = (hs + 31) / 32 * 32, Rp = (R + 31) / 32 * 32;
     auto body16 = [&]() -> int {
         GVD_CHECK_CUDA(cudaMalloc(&khi, BR * nh * KH * 4)); GVD_CHECK_CUDA(cudaMalloc(&vh, (size_t)nb * HP * Rp * 4));

@@ -129,6 +129,21 @@ __device__ __forceinline__ long long f16x3_word(int k_even) { return (long long)
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 bool gvd_pdl();
+
+// ---------------------------------------------------------------- backend bits (gvd_set_backend; default 923, include/gvd_b200.h)
+// Bits 2, 5 and 10 are inert: accepted so that stored flag values keep working, read by nothing.
+enum GvdBackendBit : int {
+    BK_TC = 1,                // bit 0: wgmma tensor cores for every GEMM-shaped stage (else fp32 CUDA cores)
+    BK_FUSED_ATTN = 2,        // bit 1: fused self-attention pair of the region encoder
+    BK_SPLITK = 8,            // bit 3: operand-swapped split-K decode products with the fused reduce + sampler
+    BK_F16X3 = 16,            // bit 4: fp16x3 instead of 3xTF32 in the forward GEMMs (pre-split constant weights)
+    BK_PDL = 64,              // bit 6: programmatic dependent launch in the decode loops
+    BK_SS_GEMM = 128,         // bit 7: conversion-free prologue GEMMs (both operands as fp16x3 images straight from TMA)
+    BK_ATT_F16 = 256,         // bit 8: fp16x3 images instead of tf32 planes in the fused self-attention pair
+    BK_PACK_FUSION = 512,     // bit 9: the producer of a prologue activation stores the operand image the next GEMM streams
+};
+int gvd_backend();
+static inline bool gvd_backend_on(int bits) { return (gvd_backend() & bits) == bits; }      // every bit of `bits` is set
 // launch helper: <<<>>> or, with backend bit 6, cudaLaunchKernelEx + the programmatic-serialization attribute
 template <typename... KArgs, typename... Args>
 static inline cudaError_t gvd_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {

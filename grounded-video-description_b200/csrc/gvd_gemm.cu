@@ -147,11 +147,10 @@ int launch(const GemmArgs& g, int batch, cudaStream_t stream) {
 
 }  // namespace
 
-int gvd_backend();
 int gvd_gemm_nt_tc(const GemmArgs& g, int batch, cudaStream_t stream);
 
 int gvd_gemm_nt(const GemmArgs& g, int batch, cudaStream_t stream) {
-    if ((gvd_backend() & 1) && g.M >= 32 && batch % g.nh == 0) return gvd_gemm_nt_tc(g, batch, stream);
+    if (gvd_backend_on(BK_TC) && g.M >= 32 && batch % g.nh == 0) return gvd_gemm_nt_tc(g, batch, stream);
     GVD_REQUIRE(g.M > 0 && g.N > 0 && g.K > 0, "gemm: empty problem M=%d N=%d K=%d", g.M, g.N, g.K);
     GVD_REQUIRE(g.K % 4 == 0 && g.lda % 4 == 0 && g.ldw % 4 == 0, "gemm: K/lda/ldw must be multiples of 4 (K=%d lda=%lld ldw=%lld)",
                 g.K, g.lda, g.ldw);

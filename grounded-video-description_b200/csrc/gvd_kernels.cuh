@@ -101,7 +101,6 @@ int gvd_beam_finish(const BeamBufs& bb, const int* bos_att, int B, int K, int L,
                     cudaStream_t st);
 
 // ---- wgmma / TMA GEMM (gvd_wgmma.cu)
-int gvd_backend();   // gvd_set_backend flags (gvd_api.cu)
 // operand-swapped split-K path for the skinny decode-step products (gvd_skinny.cu; backend bit 3)
 int gvd_skinny_splits(int Nw, int Ktot, int B);
 int gvd_skinny_splitk(const float* W, int Nw, int Ktot, const float* X, long long ldx, int B, int S, float* part, int ldp, cudaStream_t st);
@@ -175,10 +174,6 @@ int gvd_grounding_eval_hits(const float* pred, const float* ref, const int* nref
                             float thresh, cudaStream_t st);
 int gvd_grounding_gather(const float* ppls, const long long* idx, float* boxes, int B, int L, int NF, int P, int C, cudaStream_t st);
 int gvd_frame_argmax(const float* x, long long* out, long long rows, int NF, int P, cudaStream_t st);
-
-// persistent bidirectional GRU layer (gvd_gru.cu): one cooperative launch per layer instead of 2 launches per time step
-int gvd_gru_layer(const float* gi, const float* whh, const float* bhh, float* hbuf, float* out, const long long* sample_idx, unsigned int* bar,
-                  int B, int T, int G, cudaStream_t st);
 
 int gvd_gru_layer_f16(const float* gi, const float* Whh_img, const float* bhh, float* hstate, float* h_img, float* out, const long long* sample_idx, int B,
                       int T, int G, cudaStream_t st);

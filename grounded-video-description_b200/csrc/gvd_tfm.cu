@@ -379,7 +379,7 @@ inline int rup4i(int x) { return (x + 3) / 4 * 4; }
 
 // split-K planes of one skinny product (0: generic path, one plane)
 int tfm_splits(int Nw, int K, int B) {
-    if ((gvd_backend() & 9) != 9) return 0;                  // wgmma + split-K decode products (backend bits 0 and 3)
+    if (!gvd_backend_on(BK_TC | BK_SPLITK)) return 0;        // wgmma + split-K decode products
     return gvd_skinny_splits(Nw, K, B);
 }
 size_t tfm_part_floats(int Nw, int K, int B) { return (size_t)std::max(1, gvd_skinny_splits(Nw, K, B)) * B * rup4i(Nw); }
@@ -446,7 +446,7 @@ int tfm_check(const gvd_tfm_weights_t* w, int B, int L, int n0, int n1) {
 // With backend bit 4 and the weight's fp16x3 image at hand (Wimg; Ximg = scratch for the image of X): one small pack pass over the B activation
 // rows, then the conversion-free kernel of the greedy LSTM path (skinny_f16_kernel: TMA -> wgmma on both operand images, no conversion,
 // ) — the products of this loop are 2-20 MB of weights each, so their time is the fixed latency of the kernel.
-bool tfm_f16() { return (gvd_backend() & 16) != 0 && getenv("GVD_TFM_NO_F16") == nullptr; }
+bool tfm_f16() { return gvd_backend_on(BK_F16X3); }
 int tfm_product(const float* W, int Nw, int K, const float* X, long long ldx, int B, float* part, int ldp, int* S, cudaStream_t st,
                 const float* Wimg = nullptr, float* Ximg = nullptr, const float* Xready = nullptr) {
     const int sp = tfm_splits(Nw, K, B);
@@ -580,7 +580,7 @@ static int tfm_loop(const gvd_tfm_weights_t* w, const TfmWs& s, int B, int L, in
     const size_t smemH = (size_t)H * sizeof(float);
     int S = 1;
     // conversion-free products: the producers below store the operand images themselves (fi = fused images on; the conditions of tfm_product)
-    const bool fi = s.ximg && tfm_f16() && (gvd_backend() & 9) == 9 && B <= 128 && getenv("GVD_TFM_NO_IMG_FUSION") == nullptr;
+    const bool fi = s.ximg && tfm_f16() && gvd_backend_on(BK_TC | BK_SPLITK) && B <= 128;
     float *ix = fi ? s.ix : nullptr, *iy = fi ? s.iy : nullptr, *iz = fi ? s.iz : nullptr, *ica = fi ? s.ica : nullptr, *iff = fi ? s.iff : nullptr;
     for (int t = 0; t < L; ++t) {
         if (teacher) tfm_embed_kernel<<<dim3(gvd_cdiv(H, 256), B), 256, 0, st>>>(pe, w->out_w, (const long long*)teacher, L + 1, t, t, H, V, sqrt_d, s.x, ix);

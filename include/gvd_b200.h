@@ -225,12 +225,12 @@ GVD_API int gvd_grounding_extract(const float* att2, const float* ppls, int B, i
    0 for zero-area annotations, -1 for zero-area predictions) and hit_out [N] = max > iou_thresh; bit-exact vs the fp32 CPU code. */
 GVD_API int gvd_grounding_eval(const float* pred, const float* ref, const int* nref, int N, int F, int K, float iou_thresh,
                   float* max_iou_out, unsigned char* hit_out, void* stream);
-/* host-side planning helper of the experimental split-K decode products (backend bit 3): number of K splits used for a product
+/* host-side planning helper of the split-K decode products (backend bit 3): number of K splits used for a product
    with `weight_rows` x `k_total` weights and `batch_rows` activations rows, 0 if the shape falls back to the regular path */
 GVD_API int gvd_plan_skinny_splits(int weight_rows, int k_total, int batch_rows);
 /* host-side planning helper of gvd_sample_greedy_host: the clip chunks in which the fc6 region features cross PCIe (main.py:344-350 copies the
    whole batch in one piece).  `unit` = clips per self-attention sub-batch; writes at most `cap` chunk sizes to `chunks_out`, returns their number
-   (the sizes sum to batch_clips), or -1 with gvd_last_error() set.  Honours GVD_H2D_SCHED / GVD_H2D_CHUNK like the entry point itself. */
+   (the sizes sum to batch_clips), or -1 with gvd_last_error() set.  The entry point itself uses this schedule. */
 GVD_API int gvd_plan_h2d_chunks(int batch_clips, int unit, int* chunks_out, int cap);
 /* the same contraction on the wgmma tensor cores (3xTF32, fp32-faithful) */
 GVD_API int gvd_op_linear_tc(const float* A, int64_t lda, const float* W, int64_t ldw, const float* bias, float* C, int64_t ldc,
@@ -363,9 +363,10 @@ GVD_API int gvd_op_beam_search_scripted(const float* logits, const float* z, flo
 /* arithmetic backend switches: bit 0 wgmma tensor cores for every GEMM-shaped stage (0 = fp32 CUDA cores); bit 1 fused self-attention pair;
    bit 2 (4) inert; bit 3 (8) operand-swapped split-K decode products with fused
    reduce + sampler; bit 4 (16) fp16x3 instead of 3xTF32 in the forward GEMMs, pre-split weights, conversion-free decode step, tensor-core GRU;
-   bit 5 (32) cooperative GRU layer kernel (off); bit 6 (64) programmatic dependent launch in the decode loop (off); bit 7 (128)
+   bit 5 (32) inert; bit 6 (64) programmatic dependent launch in the decode loop (off); bit 7 (128)
    conversion-free prologue GEMMs; bit 8 (256) fp16x3 key / value images in the self-attention pair; bit 9 (512) pack fusion
-   (producers store the operand image of the next GEMM); bit 10 (1024) inert.  Default 923 = 1 + 2 + 8 + 16 + 128 + 256 + 512.  Every combination in
+   (producers store the operand image of the next GEMM); bit 10 (1024) inert.  The inert bits 2, 5 and 10 are accepted so that stored flag
+   values keep working; nothing reads them.  Default 923 = 1 + 2 + 8 + 16 + 128 + 256 + 512.  Every combination in
    tests/test_gpu_tcgen05.py meets the same parity bar. */
 GVD_API int gvd_set_backend(int flags);
 GVD_API int gvd_get_backend(void);

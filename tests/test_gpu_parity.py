@@ -108,20 +108,22 @@ def test_greedy_matches_oracle_and_reference_fixture(name):
     assert np.max(np.abs(logp.cpu().numpy() - fx["logp"])) <= TOL
 
 
-@pytest.mark.parametrize("env", [{}, {"GVD_H2D_SCHED": "2,1,2"}, {"GVD_H2D_SCHED": "1"}, {"GVD_H2D_CHUNK": "3"}, {"GVD_NO_FRAME_OVERLAP": "1"},
-                                 {"GVD_H2D_SCHED": "4", "GVD_NO_FRAME_OVERLAP": "1"}])
-def test_host_buffer_entry_point_matches_device_path(env, monkeypatch):
-    """gvd_sample_greedy_host (pinned host buffers -> chunked H2D on the copy stream -> per-chunk region stages, frame stages on their own
-    stream -> loop -> D2H) returns exactly the device path's outputs, whatever the chunk schedule (ragged, single-clip, uniform) and with
-    the frame stream on or off."""
-    for k, v in env.items():
-        monkeypatch.setenv(k, v)
+@pytest.mark.parametrize("serial", [False, True])
+def test_host_buffer_entry_point_matches_device_path(serial):
+    """gvd_sample_greedy_host (pinned host buffers -> H2D on the copy stream -> region stages, frame stages on their own stream -> loop
+    -> D2H) returns exactly the device path's outputs, also with the frame stages on the caller's stream (serial: under the stage profiler,
+    which runs them there).  The chunked schedule at the benchmarked size is checked by test_full_batch_properties_B100."""
     opt, sd, inp = build_case(CASES["greedy_small_B5"])
     model = _model(opt, sd)
     seq, att2, sim = _sample(model, inp)
     pinned = {k: inp[k].pin_memory() for k in ("segs_feat", "ppls", "num", "ppls_feat", "sample_idx", "pnt_mask")}
-    out = model._native.sample_greedy_host(pinned["segs_feat"], pinned["ppls"], pinned["num"], pinned["ppls_feat"],
-                                           pinned["sample_idx"], pinned["pnt_mask"])
+    capi.profile_enable(serial)
+    try:
+        out = model._native.sample_greedy_host(pinned["segs_feat"], pinned["ppls"], pinned["num"], pinned["ppls_feat"],
+                                               pinned["sample_idx"], pinned["pnt_mask"])
+    finally:
+        capi.profile_enable(False)
+        capi.profile_reset()
     assert torch.equal(out["seq"], seq.cpu())
     assert torch.equal(out["att2"], att2.cpu())
     assert torch.equal(out["sim"], sim.cpu())

@@ -1,5 +1,4 @@
-"""Measurement aid: the 20-step greedy loop alone (gvd_decode_greedy, graph replay) at B=100, default backend; argv[1] = T (default 10).
-Process-level switches (GVD_ATTN_RC, GVD_ATTN_TC, GVD_CLIP_CHUNK ...) are read when the workspace is laid out: one process per setting."""
+"""Measurement aid: the 20-step greedy loop alone (gvd_decode_greedy, graph replay) at B=100, default backend; argv[1] = T (default 10)."""
 import os
 import sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -22,5 +21,4 @@ torch.cuda.synchronize(); e0.record()
 for _ in range(10): out = nm.decode_greedy(B, T, dev["pnt_mask"])
 e1.record(); torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / 10
-print("T=%d RC=%s TC=%s CLIP_CHUNK=%s: prologue %.3f ms  loop %.3f ms (%.1f us/step)  tokens checksum %d" % (
-    T, os.environ.get("GVD_ATTN_RC"), os.environ.get("GVD_ATTN_TC"), os.environ.get("GVD_CLIP_CHUNK"), pro, ms, ms / 20 * 1e3, int(out[0].sum())), flush=True)
+print("T=%d: prologue %.3f ms  loop %.3f ms (%.1f us/step)  tokens checksum %d" % (T, pro, ms, ms / 20 * 1e3, int(out[0].sum())), flush=True)
