@@ -14,7 +14,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libgvd_b200.so")
 
 EXPORTS = [
-    "gvd_last_error", "gvd_version", "gvd_model_create", "gvd_model_create_mode", "gvd_model_create_modes", "gvd_model_destroy", "gvd_model_set_param",
+    "gvd_last_error", "gvd_version", "gvd_model_create", "gvd_model_create_mode", "gvd_model_create_modes", "gvd_model_create_opts", "gvd_model_destroy", "gvd_model_set_param",
     "gvd_model_num_params", "gvd_model_param_key", "gvd_model_finalize", "gvd_workspace_bytes",
     "gvd_workspace_tensor", "gvd_prologue_fwd", "gvd_decode_greedy", "gvd_decode_sample", "gvd_decode_step_fwd",
     "gvd_decode_reset_state", "gvd_sample_greedy_host", "gvd_op_linear", "gvd_op_tanh", "gvd_op_kernel_launches",
@@ -58,6 +58,7 @@ def lib():
     L.gvd_model_create.argtypes = [ctypes.POINTER(Dims), ctypes.POINTER(vp)]
     L.gvd_model_create_mode.argtypes = [ctypes.POINTER(Dims), ci, ctypes.POINTER(vp)]
     L.gvd_model_create_modes.argtypes = [ctypes.POINTER(Dims), ci, ci, ctypes.POINTER(vp)]
+    L.gvd_model_create_opts.argtypes = [ctypes.POINTER(Dims), ci, ci, ci, ci, ctypes.POINTER(vp)]
     L.gvd_model_destroy.argtypes = [vp]
     L.gvd_model_destroy.restype = None
     L.gvd_model_set_param.argtypes = [vp, ctypes.c_char_p, vp, sz, vp]
@@ -173,13 +174,14 @@ def profile_read():
 
 # opt.att_input_mode of the top-down captioner -> GVD_ATT_INPUT_* (include/gvd_b200.h)
 ATT_INPUT_MODES = {"both": 0, "featmap": 1, "dual_region": 2}
+ATT_INPUT_REGION = 3          # GVD_ATT_INPUT_REGION: only with enable_BUTD, for the transformer captioner's encoder
 
 
 def att_input_mode_code(opt):
     """The GVD_ATT_INPUT_* code of ``opt.att_input_mode`` for the top-down captioner (the transformer captioner's prologue and decode step
-    do not depend on it: 'both')."""
+    do not depend on it: 'both'; with enable_BUTD the prologue builds fc7-only region features: GVD_ATT_INPUT_REGION)."""
     if getattr(opt, "att_model", "topdown") == "transformer":
-        return ATT_INPUT_MODES["both"]
+        return ATT_INPUT_REGION if getattr(opt, "enable_BUTD", False) else ATT_INPUT_MODES["both"]
     return ATT_INPUT_MODES[getattr(opt, "att_input_mode", "both")]
 
 
@@ -202,22 +204,45 @@ def region_attn_mode_code(opt):
     return REGION_ATTN_MODES[mode]
 
 
+# opt.transfer_mode -> GVD_TRANSFER_* (include/gvd_b200.h): where the class side of the region-class similarity comes from (model.py:84-85,180-215)
+TRANSFER_MODES = {"cls": 0, "none": 1}
+# the reference's other values fail while it builds the module or runs its first forward, so they are refused with the reason
+_TRANSFER_REFUSED = {
+    "glove": "'glove' sizes the fc7 layer ctx2pool_grd [300, 2048] and the reference fails copying the detector's [2048, 2048] fc7 weights "
+             "into it (model.py:88-89,158,177)",
+    "both": "'both' makes fc7 2348 wide, so the region features are 300 columns wider than pool_embed was built for and the reference "
+            "fails reshaping them to pool_feat_size (model.py:86-87,70,370)",
+}
+
+
+def transfer_mode_code(opt):
+    """The GVD_TRANSFER_* code of ``opt.transfer_mode``."""
+    mode = getattr(opt, "transfer_mode", "cls")
+    if mode not in TRANSFER_MODES:
+        raise NotImplementedError("transfer_mode=%r: %s" % (mode, _TRANSFER_REFUSED.get(mode, "implemented: %s" % sorted(TRANSFER_MODES))))
+    return TRANSFER_MODES[mode]
+
+
 def dims_from_opt(opt):
     """Size fields misc/model.py:31-58 reads from ``opt``."""
     att_model = getattr(opt, "att_model", "topdown")
     if att_model not in ("topdown", "transformer"):
         raise NotImplementedError("att_model=%r: 'topdown' and 'transformer' are on the accelerated path" % (att_model,))
+    if getattr(opt, "enable_BUTD", False):
+        if getattr(opt, "att_input_mode", "both") != "region":
+            raise ValueError("enable_BUTD needs att_input_mode='region' (the reference asserts it, model.py:66, main.py:528-529); got %r"
+                             % (getattr(opt, "att_input_mode", "both"),))
+        if att_model == "topdown":
+            raise NotImplementedError("enable_BUTD needs att_input_mode='region', which the top-down captioner does not run")
     if att_model == "transformer" and getattr(opt, "att_input_mode", "both") not in ("both", "featmap", "region"):
         raise NotImplementedError("att_input_mode=%r" % (opt.att_input_mode,))          # model.py:571-576
     if att_model == "topdown" and getattr(opt, "att_input_mode", "both") not in ATT_INPUT_MODES:
         raise NotImplementedError("att_input_mode=%r: the top-down captioner implements %s" % (opt.att_input_mode, sorted(ATT_INPUT_MODES)))
     region_attn_mode_code(opt)
-    for field, want in (("t_attn_mode", "bigru"), ("transfer_mode", "cls")):
-        if getattr(opt, field, want) != want:
-            raise NotImplementedError("%s=%r: only %r (the reference default, cfgs/anet_res101_vg_feat_10x100prop.yml) "
-                                      "is implemented" % (field, getattr(opt, field), want))
-    if getattr(opt, "enable_BUTD", False):
-        raise NotImplementedError("enable_BUTD is not on the accelerated path")
+    transfer_mode_code(opt)
+    if getattr(opt, "t_attn_mode", "bigru") != "bigru":
+        raise NotImplementedError("t_attn_mode=%r: only 'bigru' (the reference default, cfgs/anet_res101_vg_feat_10x100prop.yml) "
+                                  "is implemented" % (opt.t_attn_mode,))
     if getattr(opt, "seq_per_img", 1) != 1:
         raise NotImplementedError("seq_per_img must be 1 (cfgs/anet_res101_vg_feat_10x100prop.yml:14)")
     return Dims(int(opt.vocab_size), int(opt.detect_size), int(opt.input_encoding_size), int(opt.rnn_size),
@@ -234,11 +259,14 @@ class NativeModel:
         self.dims = dims_from_opt(opt)
         self.att_input_mode = att_input_mode_code(opt)
         self.region_attn_mode = region_attn_mode_code(opt)
+        self.transfer_mode = transfer_mode_code(opt)
         self._h = ctypes.c_void_p()
         if not torch.cuda.is_available():
             raise GvdError("gvd_b200 has no CPU path: a CUDA device is required")
         self.device = torch.cuda.current_device()      # the weight arena and every workspace live on this device
-        check(self._L.gvd_model_create_modes(ctypes.byref(self.dims), self.att_input_mode, self.region_attn_mode, ctypes.byref(self._h)))
+        self.butd = bool(getattr(opt, "enable_BUTD", False))
+        check(self._L.gvd_model_create_opts(ctypes.byref(self.dims), self.att_input_mode, self.region_attn_mode, self.transfer_mode,
+                                            int(self.butd), ctypes.byref(self._h)))
         self._live = None                              # (B, T, beam, nbox) of the prologue whose outputs sit in the workspace
         self._live_V = 0                               # ... and its video count (0: a per-clip prologue)
         self.R = self.dims.num_sampled_frm * self.dims.num_prop_per_frm

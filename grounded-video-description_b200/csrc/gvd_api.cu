@@ -189,6 +189,7 @@ struct gvd_model {
     gvd_dims_t d;
     int att_mode = GVD_ATT_INPUT_BOTH;   // opt.att_input_mode (GVD_ATT_INPUT_*): what the language LSTM reads, AttModel.py:144-156
     int region_form = GVD_REGION_ATTN_MIX;   // opt.region_attn_mode (GVD_REGION_ATTN_*): the region attentions' score, AttModel.py:79-96
+    bool butd = false;                       // opt.enable_BUTD: the region features are fc7 alone (model.py:65-69,357-364)
     int R, G, NC, FCX, FCXp, PIN, PINp, NCp, Vp, HS, HP, nheads, rgb, motion;
     std::vector<int> head_off, head_size;
     std::vector<Param> params;
@@ -247,7 +248,21 @@ extern "C" GVD_API int gvd_model_create_mode(const gvd_dims_t* dims, int att_inp
 }
 
 extern "C" GVD_API int gvd_model_create_modes(const gvd_dims_t* dims, int att_input_mode, int region_attn_mode, gvd_model_t** out) {
+    return gvd_model_create_opts(dims, att_input_mode, region_attn_mode, GVD_TRANSFER_CLS, 0, out);
+}
+
+extern "C" GVD_API int gvd_model_create_opts(const gvd_dims_t* dims, int att_input_mode, int region_attn_mode, int transfer_mode, int butd,
+                                             gvd_model_t** out) {
     GVD_REQUIRE(dims && out, "model_create: null argument");
+    GVD_REQUIRE(transfer_mode == GVD_TRANSFER_CLS || transfer_mode == GVD_TRANSFER_NONE,
+                "model_create: transfer_mode %d is not implemented (0 = 'cls', 1 = 'none'; 'glove' and 'both' fail in the reference)", transfer_mode);
+    GVD_REQUIRE(butd == 0 || butd == 1, "model_create: butd must be 0 or 1 (got %d)", butd);
+    // BUTD and 'region' come together: the reference asserts the pair (model.py:66), and 'region' is only the transformer captioner's encoder
+    GVD_REQUIRE((att_input_mode == GVD_ATT_INPUT_REGION) == (butd == 1),
+                "model_create: enable_BUTD needs att_input_mode 'region' (model.py:66), and 'region' is only built with enable_BUTD (att_input_mode %d, "
+                "butd %d)", att_input_mode, butd);
+    if (butd) att_input_mode = GVD_ATT_INPUT_BOTH;   // checked above; the modes below are the top-down decode's
+
     GVD_REQUIRE(region_attn_mode == GVD_REGION_ATTN_MIX || region_attn_mode == GVD_REGION_ATTN_MIX_MUL || region_attn_mode == GVD_REGION_ATTN_DP,
                 "model_create: region_attn_mode %d is not implemented (0 = 'mix', 1 = 'mix_mul', 2 = 'dp')", region_attn_mode);
     GVD_REQUIRE(att_input_mode == GVD_ATT_INPUT_BOTH || att_input_mode == GVD_ATT_INPUT_FEATMAP || att_input_mode == GVD_ATT_INPUT_DUAL_REGION,
@@ -267,6 +282,7 @@ extern "C" GVD_API int gvd_model_create_modes(const gvd_dims_t* dims, int att_in
     m->d = d;
     m->att_mode = att_input_mode;
     m->region_form = region_attn_mode;
+    m->butd = butd == 1;
     const int H = d.rnn_size, A = d.att_hid_size, E = d.input_encoding_size, V = d.vocab_size, D = d.detect_size;
     m->R = d.num_sampled_frm * d.num_prop_per_frm;
     GVD_REQUIRE(!d.obj_interact || m->R % 4 == 0, "obj_interact needs R %% 4 == 0 (R=%d)", m->R);
@@ -275,7 +291,7 @@ extern "C" GVD_API int gvd_model_create_modes(const gvd_dims_t* dims, int att_in
     m->NCp = rup4(m->NC);
     m->FCX = d.fc_feat_size + 50;
     m->FCXp = rup4(m->FCX);
-    m->PIN = d.att_feat_size + 300 + D + 1;
+    m->PIN = butd ? d.att_feat_size : d.att_feat_size + 300 + D + 1;      // BUTD: pool_embed reads fc7 alone (model.py:65-69)
     m->PINp = rup4(m->PIN);
     m->Vp = rup4(V);
     m->rgb = 2048;
@@ -288,7 +304,7 @@ extern "C" GVD_API int gvd_model_create_modes(const gvd_dims_t* dims, int att_in
     m->HP = m->HS * m->nheads;
     const int G = m->G;
     // the reference state_dict (SURVEY.md 8b), float entries only
-    add_param(m, "vis_classifiers_bias", D + 1);
+    if (transfer_mode == GVD_TRANSFER_CLS) add_param(m, "vis_classifiers_bias", D + 1);   // 'none' has no class bias (model.py:196-203)
     add_param(m, "loc_fc.0.weight", 300 * 5); add_param(m, "loc_fc.0.bias", 300);
     add_param(m, "embed.0.weight", (size_t)V * E);
     add_param(m, "vis_embed.0.weight", (size_t)(D + 1) * 2048);
@@ -785,6 +801,14 @@ extern "C" GVD_API float* gvd_workspace_tensor(const gvd_model_t* m, void* works
 }
 
 // V < 0: the layout the last prologue on this workspace left (video_of); V >= 0: that layout explicitly (a prologue about to run)
+// the top-down captioner's decode and teacher-forced entry points: a BUTD model ('region') only feeds the transformer captioner
+static int require_topdown(const gvd_model* m, const char* who) {
+    GVD_REQUIRE(m, "%s: null model", who);
+    GVD_REQUIRE(!m->butd, "%s: this model was built with enable_BUTD (att_input_mode 'region'), which only the transformer captioner runs; "
+                "the top-down captioner does not take 'region'", who);
+    return 0;
+}
+
 static int check_ws(const gvd_model* m, int B, int T, void* workspace, size_t bytes, WS* w, int beam = 1, int nbox = 0, int V = -1) {
     GVD_REQUIRE(m && m->finalized, "model not finalized (call gvd_model_finalize after setting every parameter)");
     GVD_REQUIRE(B >= 1 && T >= 1, "bad batch/frames B=%d T=%d", B, T);
@@ -1010,19 +1034,29 @@ static int region_prologue(const gvd_model* m, const WS& w0, int c0, int cb, con
     const bool fuse = pack_fusion() && H % 64 == 0 && linear_w_f16ss(w, m->P("ctx2pool.weight"), H, (int)BR, A, H) &&
                       linear_w_f16ss(w, m->pool_embed_w, m->PINp, (int)BR, H, m->PINp) && linear_w_f16ss(w, m->vis_relu, 2048, (int)BR, m->NC, 2048) &&
                       (!d.obj_interact || linear_w_f16ss(w, m->wqk[0], H, (int)BR, 3 * m->HP, H));
-    GVD_STAGE("region.fc7", linear_w(w, ppls_feat, d.att_feat_size, m->P("ctx2pool_grd.0.weight"), d.att_feat_size, m->P("ctx2pool_grd.0.bias"), w.g_pool,
-                       2048, (int)BR, 2048, d.att_feat_size, GVD_ACT_RELU, st, nullptr, nullptr, nullptr, fuse ? w.img_g : nullptr));
-    // P3 region-class similarity, stored region-major: simT[(b,r), c] (model.py:519-535)
-    GVD_STAGE("region.sim_gemm", linear_w(w, w.g_pool, 2048, m->vis_relu, 2048, m->P("vis_classifiers_bias"), w.simT, m->NCp, (int)BR, m->NC, 2048, GVD_ACT_NONE, st,
-                                          nullptr, nullptr, fuse ? w.img_g : nullptr));
-    GVD_STAGE("region.sim_softmax", gvd_sim_softmax(w.simT, pnt_mask, B, R, m->NC, m->NCp, st));
+    // BUTD with pack fusion: every reader of fc7 (pool_embed, the similarity) streams its operand image, so the epilogue stores the image alone
+    GVD_STAGE("region.fc7", linear_w(w, ppls_feat, d.att_feat_size, m->P("ctx2pool_grd.0.weight"), d.att_feat_size, m->P("ctx2pool_grd.0.bias"),
+                                     m->butd && fuse ? nullptr : w.g_pool, 2048, (int)BR, 2048, d.att_feat_size, GVD_ACT_RELU, st, nullptr, nullptr, nullptr,
+                                     fuse ? w.img_g : nullptr));
+    // P3 region-class similarity, stored region-major: simT[(b,r), c] (model.py:519-535); transfer_mode 'none' has no class bias (P() is NULL).
+    // BUTD: the region features do not read it (model.py:357-364), so it runs only for the caller's sim_mat_out
+    if (!m->butd || sim_mat_out) {
+        GVD_STAGE("region.sim_gemm", linear_w(w, w.g_pool, 2048, m->vis_relu, 2048, m->P("vis_classifiers_bias"), w.simT, m->NCp, (int)BR, m->NC, 2048, GVD_ACT_NONE,
+                                              st, nullptr, nullptr, fuse ? w.img_g : nullptr));
+        GVD_STAGE("region.sim_softmax", gvd_sim_softmax(w.simT, pnt_mask, B, R, m->NC, m->NCp, st));
+    }
     if (sim_mat_out) GVD_STAGE("region.sim_transpose", gvd_transpose(w.simT, sim_mat_out, B, R, m->NC, m->NCp, st));
-    // P4 region embedding (model.py:537-547)
-    const int PINi = (m->PINp + 31) / 32 * 32;
-    GVD_STAGE("region.pool_in", gvd_pool_in(w.g_pool, ppls, w.simT, m->P("loc_fc.0.weight"), m->P("loc_fc.0.bias"), fuse ? nullptr : w.pool_in, BR, 2048, 300, m->NC,
-                                            m->NCp, m->PINp, d.num_sampled_frm, st, fuse ? w.a_pk : nullptr, PINi));
-    GVD_STAGE("region.pool_embed", linear_w(w, w.pool_in, m->PINp, m->pool_embed_w, m->PINp, m->P("pool_embed.0.bias"), w.pool_embed, H, (int)BR, H, m->PINp,
-                       GVD_ACT_RELU, st, nullptr, nullptr, fuse ? w.a_pk : nullptr, fuse ? w.img_h : nullptr));
+    // P4 region embedding (model.py:537-547); BUTD: pool_embed on fc7 alone, K = 2048 (model.py:65-69,384)
+    if (m->butd) {
+        GVD_STAGE("region.pool_embed", linear_w(w, w.g_pool, 2048, m->pool_embed_w, m->PINp, m->P("pool_embed.0.bias"), w.pool_embed, H, (int)BR, H, 2048,
+                                                GVD_ACT_RELU, st, nullptr, nullptr, fuse ? w.img_g : nullptr, fuse ? w.img_h : nullptr));
+    } else {
+        const int PINi = (m->PINp + 31) / 32 * 32;
+        GVD_STAGE("region.pool_in", gvd_pool_in(w.g_pool, ppls, w.simT, m->P("loc_fc.0.weight"), m->P("loc_fc.0.bias"), fuse ? nullptr : w.pool_in, BR, 2048, 300,
+                                                m->NC, m->NCp, m->PINp, d.num_sampled_frm, st, fuse ? w.a_pk : nullptr, PINi));
+        GVD_STAGE("region.pool_embed", linear_w(w, w.pool_in, m->PINp, m->pool_embed_w, m->PINp, m->P("pool_embed.0.bias"), w.pool_embed, H, (int)BR, H, m->PINp,
+                                                GVD_ACT_RELU, st, nullptr, nullptr, fuse ? w.a_pk : nullptr, fuse ? w.img_h : nullptr));
+    }
     // P5 object interaction (model.py:550-551)
     if (d.obj_interact) GVD_TRY(obj_interact_fwd(m, w0, c0, cb, st, fuse));
     // P6 (model.py:554)
@@ -1110,6 +1144,7 @@ extern "C" GVD_API int gvd_prologue_fwd_video(gvd_model_t* m, int B, int V, int 
 
 // ------------------------------------------------------------------------------------ decode
 extern "C" GVD_API int gvd_decode_reset_state(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes, void* stream) {
+    GVD_TRY(require_topdown(m, "decode_reset_state"));
     WS w;
     GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
     cudaStream_t st = (cudaStream_t)stream;
@@ -1265,6 +1300,7 @@ static int core_step(const gvd_model* m, const WS& w, int B, int T, int step, co
 extern "C" GVD_API int gvd_decode_step_fwd(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes, int step,
                                    const int64_t* tokens, const uint8_t* att_mask, const uint8_t* out_mask, float* att2_logits_out,
                                    int64_t att2_stride_b, float* h_lang_out, void* stream) {
+    GVD_TRY(require_topdown(m, "decode_step"));
     WS w;
     GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
     GVD_REQUIRE(tokens && att_mask && out_mask && att2_logits_out && step >= 0, "decode_step: null argument");
@@ -1397,6 +1433,7 @@ static int decode_loop_run(gvd_model_t* m, const WS& w, int B, int T, void* work
 
 extern "C" GVD_API int gvd_decode_greedy(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes, const uint8_t* pnt_mask,
                                  int64_t* seq_out, float* logprobs_out, float* att2_logits_out, void* stream) {
+    GVD_TRY(require_topdown(m, "decode_greedy"));
     WS w;
     GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
     GVD_REQUIRE(pnt_mask && seq_out && att2_logits_out, "decode_greedy: null argument");
@@ -1406,6 +1443,7 @@ extern "C" GVD_API int gvd_decode_greedy(gvd_model_t* m, int B, int T, void* wor
 
 extern "C" GVD_API int gvd_decode_sample(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes, const uint8_t* pnt_mask,
                                  uint64_t seed, float temperature, int64_t* seq_out, float* logprobs_out, float* att2_logits_out, void* stream) {
+    GVD_TRY(require_topdown(m, "decode_sample"));
     WS w;
     GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
     GVD_REQUIRE(pnt_mask && seq_out && att2_logits_out, "decode_sample: null argument");
@@ -1431,6 +1469,7 @@ extern "C" GVD_API int gvd_teacher_fwd(gvd_model_t* m, int B, int T, int nbox, i
                                        const int64_t* seq, const int64_t* input_cls, const float* ppls, const float* gt_boxes,
                                        const uint8_t* mask_boxes, const uint8_t* frm_mask, const uint8_t* pnt_mask, float* losses_out,
                                        int64_t* att_idx_out, int64_t* grd_idx_out, int32_t* sim_target_out, int32_t* cls_pred_out, void* stream) {
+    GVD_TRY(require_topdown(m, "teacher_fwd"));
     WS w;
     GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w, 1, nbox));
     const gvd_dims_t& d = m->d;
@@ -1463,7 +1502,8 @@ extern "C" GVD_API int gvd_teacher_fwd(gvd_model_t* m, int B, int T, int nbox, i
         const float* h = w.h_lang + (size_t)((i + 1) & 1) * B * H;
         GVD_CHECK_CUDA(cudaMemcpy2DAsync(w.outs + (size_t)i * H, (size_t)S * H * 4, h, (size_t)H * 4, (size_t)H * 4, B, cudaMemcpyDeviceToDevice, st));
     }
-    // grounding logits: ReLU(vis_embed)[cls] . g_pool^T + bias[cls] + att2 logits, masked (model.py:469-486)
+    // grounding logits: ReLU(vis_embed)[cls] . g_pool^T + bias[cls] + att2 logits, masked (model.py:469-486); no bias term in transfer_mode
+    // 'none' (P() is NULL)
     GVD_STAGE("teacher.ground", gvd_gather_class_rows(m->vis_relu, (const long long*)input_cls, w.emb, w.cls_idx, B, S, L1, V, 2048, m->NC, st));
     {
         GemmArgs g{};
@@ -1536,6 +1576,7 @@ static int beam_search_run(const BeamBufs& bb, int* bos_att, float* gather_tmp, 
 // B1/B2: beam search for every clip at once (misc/model.py:700-742 + misc/CaptionModelBU.py:104-185, repaired semantics)
 extern "C" GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_size, void* workspace, size_t workspace_bytes,
                                        const uint8_t* pnt_mask, int64_t* seq_out, float* logprobs_out, int64_t* att2_idx_out, void* stream) {
+    GVD_TRY(require_topdown(m, "beam_decode"));
     GVD_REQUIRE(beam_size >= 2, "beam_decode: beam_size must be >= 2 (use gvd_decode_greedy for 1)");
     WS w;
     GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w, beam_size));
@@ -1598,6 +1639,7 @@ static int sample_greedy_host_run(gvd_model_t* m, int B, int V, int T, const flo
                                   const float* h_ppls_feat, const int64_t* h_sample_idx, const int64_t* h_video_idx, const uint8_t* h_pnt_mask,
                                   void* workspace, size_t workspace_bytes, int64_t* h_seq_out, float* h_logprobs_out, float* h_att2_out,
                                   float* h_sim_mat_out, void* stream) {
+    GVD_TRY(require_topdown(m, "sample_greedy_host"));
     WS w;
     GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w, 1, 0, V));
     GVD_REQUIRE(h_segs_feat && h_ppls && h_num && h_ppls_feat && h_sample_idx && h_pnt_mask && h_seq_out && (V == 0 || h_video_idx),

@@ -106,7 +106,8 @@ __global__ void gather_class_rows_kernel(const float* __restrict__ vis_relu, con
         *reinterpret_cast<float4*>(emb + (long long)row * D2 + d) = *reinterpret_cast<const float4*>(vis_relu + c * D2 + d);
 }
 
-// G[b,i,r] = dot + bias[cls] + z[b,i,r], then -1e8 where masked (model.py:472-486, _grounder :267-278)
+// G[b,i,r] = dot + bias[cls] + z[b,i,r], then -1e8 where masked (model.py:472-486, _grounder :267-278).  cls_bias NULL: the module has no
+// class bias (transfer_mode 'none', model.py:475-476), G = dot + z
 __global__ void grounding_finish_kernel(float* __restrict__ G, const float* __restrict__ z, const float* __restrict__ cls_bias,
                                         const int* __restrict__ cls_idx, const unsigned char* __restrict__ mask, long long mask_stride_row,
                                         int mask_per_step, int S, int R, long long total) {
@@ -116,7 +117,10 @@ __global__ void grounding_finish_kernel(float* __restrict__ G, const float* __re
     const long long row = idx / R;                 // b*S + i
     const long long b = row / S;
     const unsigned char m = mask_per_step ? mask[row * mask_stride_row + 1 + r] : mask[b * mask_stride_row + 1 + r];
-    G[idx] = m ? GVD_MIN_VALUE : (G[idx] + cls_bias[cls_idx[row]] + z[idx]);
+    if (m) { G[idx] = GVD_MIN_VALUE; return; }
+    float g = G[idx];
+    if (cls_bias) g += cls_bias[cls_idx[row]];
+    G[idx] = g + z[idx];
 }
 
 // per (b,i): nll = -(logit[target] - lse) and whether the position counts (utils.py:126-136)

@@ -67,7 +67,8 @@ class AttModel(CaptionModel):
                                             num_sampled_frm=opt.num_sampled_frm, obj_interact=getattr(opt, "obj_interact", False),
                                             att_input_mode=self.att_input_mode, region_attn_mode=self.region_attn_mode)
         self.vis_encoding_size = 2048
-        self.pool_feat_size = self.att_feat_size + 300 + self.detect_size + 1
+        # BUTD: the region features are fc7 alone (model.py:65-69); the reference asserts att_input_mode 'region' (dims_from_opt)
+        self.pool_feat_size = self.att_feat_size if self.enable_BUTD else self.att_feat_size + 300 + self.detect_size + 1
 
         H, A, E = self.rnn_size, self.att_hid_size, self.input_encoding_size
         p = self.drop_prob_lm
@@ -90,7 +91,8 @@ class AttModel(CaptionModel):
             self.cap_model = TransformerDecoder(H, 0, self.vocab_size, d_hidden=H // 2, n_layers=2, n_heads=6, drop_ratio=0.2)
         self.context_enc = nn.GRU(H, H // 2, 2, dropout=0.2, bidirectional=True, batch_first=True)
         self.ctx2pool_grd = _seq(nn.Linear(self.att_feat_size, self.vis_encoding_size), nn.ReLU(), nn.Dropout(p))
-        self.vis_classifiers_bias = nn.Parameter(torch.zeros(self.detect_size + 1))
+        if self.transfer_mode == "cls":             # transfer_mode 'none' builds no class bias (model.py:180-215)
+            self.vis_classifiers_bias = nn.Parameter(torch.zeros(self.detect_size + 1))
         self._init_from_detectron(opt)
 
         self._native = None
@@ -100,10 +102,12 @@ class AttModel(CaptionModel):
     # ------------------------------------------------------------------ constructor side effects
     def _init_from_detectron(self, opt):
         """fc7 / class-score transfer from ``data/detectron_weights/*.pkl`` (CWD-relative, as in the
-        reference: model.py:173-211).  Missing files only warn: checkpoints overwrite these values."""
+        reference: model.py:173-211).  Missing files only warn: checkpoints overwrite these values.
+        transfer_mode 'none' transfers fc7 only: vis_embed keeps its default init (model.py:214-215)."""
         d = "data/detectron_weights"
         try:
-            w = {k: pickle.load(open(os.path.join(d, k + ".pkl"), "rb")) for k in ("fc7_w", "fc7_b", "cls_score_w", "cls_score_b")}
+            names = ("fc7_w", "fc7_b") + (("cls_score_w", "cls_score_b") if self.transfer_mode == "cls" else ())
+            w = {k: pickle.load(open(os.path.join(d, k + ".pkl"), "rb")) for k in names}
         except (FileNotFoundError, OSError):
             warnings.warn("data/detectron_weights/*.pkl not found: ctx2pool_grd / vis_embed keep their default init "
                           "(load a checkpoint before use)")
@@ -112,6 +116,8 @@ class AttModel(CaptionModel):
             fs = self.att_feat_size
             self.ctx2pool_grd[0].weight[:fs].copy_(torch.from_numpy(w["fc7_w"]))
             self.ctx2pool_grd[0].bias[:fs].copy_(torch.from_numpy(w["fc7_b"]))
+            if self.transfer_mode != "cls":
+                return
             cw, cb = torch.from_numpy(w["cls_score_w"]), torch.from_numpy(w["cls_score_b"])
             assert len(opt.itod) + 1 == opt.glove_clss.size(0)
             assert len(opt.vg_cls) == opt.glove_vg_cls.size(0)
@@ -154,6 +160,8 @@ class AttModel(CaptionModel):
         o.wtoi = {"UNK": str(d.unk_idx)}
         o.att_model, o.att_input_mode = self.att_model, self.att_input_mode     # the language LSTM's input (AttModel.py:144-156)
         o.region_attn_mode = self.region_attn_mode                              # the region attention's score (AttModel.py:79-96)
+        o.transfer_mode = self.transfer_mode                                    # whether the similarity has a class bias (model.py:84-85)
+        o.enable_BUTD = self.enable_BUTD                                        # fc7-only region features (model.py:65-69)
         return o
 
     @staticmethod
@@ -195,6 +203,7 @@ class AttModel(CaptionModel):
         nm = self._native_model()
         sim = nm.prologue(segs_feat.float().contiguous(), ppls.float().contiguous(), num.long().contiguous(),
                           ppls_feat.float().contiguous(), sample_idx.long().contiguous(), self._u8(pnt_mask).contiguous(),
+                          want_sim=not self.enable_BUTD,       # BUTD (transformer only): nothing reads the similarity, so it is not computed
                           beam=beam, nbox=nbox,     # the workspace is sized for the decode that follows
                           video_idx=video_idx.contiguous() if video_idx is not None else None)
         return nm, sim

@@ -59,7 +59,7 @@ def state_dict_spec(opt):
     H, A, E, V, D = opt.rnn_size, opt.att_hid_size, opt.input_encoding_size, opt.vocab_size, opt.detect_size
     F = opt.att_feat_size
     fc = opt.fc_feat_size + 50
-    pool = F + 300 + D + 1
+    pool = F if getattr(opt, "enable_BUTD", False) else F + 300 + D + 1      # BUTD: pool_embed reads fc7 alone (model.py:65-69)
     G = H // 2
     spec = []
 
@@ -68,7 +68,8 @@ def state_dict_spec(opt):
         if bias:
             spec.append((name + ".bias", (out,), "uniform", inp))
 
-    spec.append(("vis_classifiers_bias", (D + 1,), "normal", 50.0))
+    if getattr(opt, "transfer_mode", "cls") == "cls":                  # 'none' has no class bias (model.py:180-215)
+        spec.append(("vis_classifiers_bias", (D + 1,), "normal", 50.0))
     lin("loc_fc.0", 300, 5)
     spec.append(("embed.0.weight", (V, E), "normal", 1.0))
     spec.append(("vis_embed.0.weight", (D + 1, 2048), "normal", 50.0))

@@ -230,15 +230,20 @@ class TrainStep:
         if regions:
             ppls_feat = inp["ppls_feat"]
             g_pool = D_(ops.lin(ppls_feat, W["ctx2pool_grd.0.weight"], W["ctx2pool_grd.0.bias"], True), "lm", "fc7")
-            Wc = D_(ops.relu(W["vis_embed.0.weight"]), "lm", "vis_cls")                     # ONE mask for the class table (model.py:320-321)
-            simT_raw = ops.lin(g_pool, Wc, W["vis_classifiers_bias"], False)                 # B, R, C (region-major)
-            simT_raw = ops.masked_fill(simT_raw, pmask.unsqueeze(-1).expand_as(simT_raw), MIN_VALUE)
-            simT = ops.softmax(simT_raw, 1.0)                                                # softmax over the classes
+            if getattr(opt, "enable_BUTD", False):
+                # BUTD (model.py:357-364): pool_embed reads the dropped-out fc7 output; no similarity, loc_fc, label features or LayerNorms
+                Wc = simT = loc_in = loc = ln_g = ln_loc = ln_sim = None
+                pool_in = g_pool
+            else:
+                Wc = D_(ops.relu(W["vis_embed.0.weight"]), "lm", "vis_cls")                 # ONE mask for the class table (model.py:320-321)
+                simT_raw = ops.lin(g_pool, Wc, W.get("vis_classifiers_bias"), False)         # B, R, C (region-major); no bias in transfer_mode 'none'
+                simT_raw = ops.masked_fill(simT_raw, pmask.unsqueeze(-1).expand_as(simT_raw), MIN_VALUE)
+                simT = ops.softmax(simT_raw, 1.0)                                            # softmax over the classes
 
-            loc_in = ops.cat((ops.scale(ppls[:, :, :4].contiguous(), 1.0 / 720.0), ops.scale(ppls[:, :, 4:5].contiguous(), 1.0 / float(opt.num_sampled_frm))), -1)
-            loc = D_(ops.lin(loc_in, W["loc_fc.0.weight"], W["loc_fc.0.bias"], True), "loc", "loc")
-            ln_g, ln_loc, ln_sim = ops.ln(g_pool), ops.ln(loc), ops.ln(simT)
-            pool_in = ops.cat((ln_g, ln_loc, ln_sim), -1)
+                loc_in = ops.cat((ops.scale(ppls[:, :, :4].contiguous(), 1.0 / 720.0), ops.scale(ppls[:, :, 4:5].contiguous(), 1.0 / float(opt.num_sampled_frm))), -1)
+                loc = D_(ops.lin(loc_in, W["loc_fc.0.weight"], W["loc_fc.0.bias"], True), "loc", "loc")
+                ln_g, ln_loc, ln_sim = ops.ln(g_pool), ops.ln(loc), ops.ln(simT)
+                pool_in = ops.cat((ln_g, ln_loc, ln_sim), -1)
             pool_embed = D_(ops.lin(pool_in, W["pool_embed.0.weight"], W["pool_embed.0.bias"], True), "lm", "pool_embed")
             pool = pool_embed
 
@@ -340,13 +345,15 @@ class TrainStep:
         g_pool, simT, pmask = pt["g_pool"], pt["simT"], pt["pmask"]
         if dpool_feats is not None:
             dg_pool, dsimT = self._pool_bwd(pt, W, opt, grads, D_, dpool_feats, dp_pool, dg_pool, dsimT)
-        n_g = g_pool.shape[-1]
-        dsim_raw = ops.masked_fill(ops.softmax_bwd(dsimT, simT, 1.0), pmask.unsqueeze(-1).expand_as(simT), 0.0)      # B, R, C
-        dsr2, gp2 = dsim_raw.reshape(-1, dsim_raw.shape[-1]), g_pool.reshape(-1, n_g)
-        dg_sim = ops.mm_nn(dsr2, pt["Wc"]).reshape(tuple(g_pool.shape))
-        dg_pool = dg_sim if dg_pool is None else ops.add(dg_pool, dg_sim)
-        self._acc(grads, "vis_embed.0.weight", ops.relu_bwd(D_(ops.mm_tn(dsr2, gp2), "lm", "vis_cls"), W["vis_embed.0.weight"]))
-        self._acc(grads, "vis_classifiers_bias", ops.colsum(dsr2))
+        if dsimT is not None:                            # (BUTD: no similarity, so vis_embed and the class bias get no gradient)
+            n_g = g_pool.shape[-1]
+            dsim_raw = ops.masked_fill(ops.softmax_bwd(dsimT, simT, 1.0), pmask.unsqueeze(-1).expand_as(simT), 0.0)  # B, R, C
+            dsr2, gp2 = dsim_raw.reshape(-1, dsim_raw.shape[-1]), g_pool.reshape(-1, n_g)
+            dg_sim = ops.mm_nn(dsr2, pt["Wc"]).reshape(tuple(g_pool.shape))
+            dg_pool = dg_sim if dg_pool is None else ops.add(dg_pool, dg_sim)
+            self._acc(grads, "vis_embed.0.weight", ops.relu_bwd(D_(ops.mm_tn(dsr2, gp2), "lm", "vis_cls"), W["vis_embed.0.weight"]))
+            if "vis_classifiers_bias" in W:
+                self._acc(grads, "vis_classifiers_bias", ops.colsum(dsr2))
         self._lin_bwd(ops.relu_bwd(D_(dg_pool, "lm", "fc7"), g_pool), pt["ppls_feat"], W, "ctx2pool_grd.0", grads, need_dx=False)
 
     def _pool_bwd(self, pt, W, opt, grads, D_, dpool_feats, dp_pool, dg_pool, dsimT):
@@ -382,6 +389,8 @@ class TrainStep:
                     dx = ops.add(dx, self._lin_bwd(ops.cat(parts, -1), tp["x"], W, p + "selfattn.layer.%s" % nm, grads))
                 dpool = dx
         dpool_in = self._lin_bwd(ops.relu_bwd(D_(dpool, "lm", "pool_embed"), pt["pool_embed"]), pt["pool_in"], W, "pool_embed.0", grads)
+        if getattr(opt, "enable_BUTD", False):            # pool_embed read fc7 directly: its input gradient is fc7's (model.py:357-364)
+            return dpool_in if dg_pool is None else ops.add(dg_pool, dpool_in), dsimT
         n_g, n_l = g_pool.shape[-1], loc.shape[-1]
         dg_ln = ops.ln_bwd(dpool_in[..., :n_g].contiguous(), pt["ln_g"], g_pool)
         dg_pool = dg_ln if dg_pool is None else ops.add(dg_pool, dg_ln)
@@ -483,7 +492,11 @@ class TrainStep:
         gmask = tgt["fm_all"][:, :S].contiguous()
         emb_cls_raw = ops.gather_rows(W["vis_embed.0.weight"], cls_idx).reshape(B, S, -1)
         emb_cls = D_(ops.relu(emb_cls_raw), "lm", "vis_word")
-        grd = ops.add(ops.add(ops.bmm_nt(emb_cls, g_pool), ops.gather_rows(W["vis_classifiers_bias"].unsqueeze(1).contiguous(), cls_idx).reshape(B, S, 1).expand(B, S, z_all.shape[-1]).contiguous()), z_all)
+        cls_bias = W.get("vis_classifiers_bias")                                         # None in transfer_mode 'none' (model.py:472-476)
+        grd = ops.bmm_nt(emb_cls, g_pool)
+        if cls_bias is not None:
+            grd = ops.add(grd, ops.gather_rows(cls_bias.unsqueeze(1).contiguous(), cls_idx).reshape(B, S, 1).expand(B, S, z_all.shape[-1]).contiguous())
+        grd = ops.add(grd, z_all)
         grd = ops.masked_fill(grd, gmask, MIN_VALUE)
         att2_loss, dz_unit = ops.pos_nll(z_all, pos)
         grd_loss, dgrd_unit = ops.pos_nll(grd, pos)
@@ -510,7 +523,8 @@ class TrainStep:
                 dg_pool = ops.add(dg_pool, ops.bmm_tn(dgrd, emb_cls))                        # [B,S,R]^T [B,S,D] -> [B,R,D]
                 demb = ops.relu_bwd(D_(ops.bmm_nn(dgrd, g_pool), "lm", "vis_word"), emb_cls_raw)   # [B,S,R] [B,R,D] -> [B,S,D]
                 self._acc(grads, "vis_embed.0.weight", ops.index_add_rows(W["vis_embed.0.weight"].shape[0], cls_idx, demb.reshape(B * S, -1)))
-                self._acc(grads, "vis_classifiers_bias", ops.index_add_rows(W["vis_classifiers_bias"].shape[0], cls_idx, ops.rowsum(dgrd.reshape(B * S, -1)).reshape(-1, 1)).reshape(-1))
+                if cls_bias is not None:
+                    self._acc(grads, "vis_classifiers_bias", ops.index_add_rows(cls_bias.shape[0], cls_idx, ops.rowsum(dgrd.reshape(B * S, -1)).reshape(-1, 1)).reshape(-1))
             dsimT = ops.scale(dsimT_unit, w_cls) if w_cls else (ops.zeros(tuple(simT.shape)) if region_grad else None)
 
             # ========================================================== backward, BPTT over the decode steps

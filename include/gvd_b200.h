@@ -60,10 +60,12 @@ GVD_API int gvd_model_create(const gvd_dims_t* dims, gvd_model_t** out);   /* at
  *               masks, read in one pass; the returned logits are the first one's.  No temporal attention: the prologue skips the frame
  *               branch (att_embed, BatchNorm, bi-GRU, ctx2att).  The parameter list gains core.attention2_dual.{h2att,alpha_net}.* and
  *               core.dual_pointer.0.* (after core.attention2.*, before core.i2h_2.*).
- * 'region' is not implemented: gvd_model_create_mode and gvd_model_create_modes reject it. */
+ *   REGION  (3) only with enable_BUTD through gvd_model_create_opts: the transformer captioner's encoder reads the region features alone;
+ *               the top-down captioner does not run 'region' (every top-down decode and teacher-forced entry point rejects such a model). */
 #define GVD_ATT_INPUT_BOTH 0
 #define GVD_ATT_INPUT_FEATMAP 1
 #define GVD_ATT_INPUT_DUAL_REGION 2
+#define GVD_ATT_INPUT_REGION 3
 GVD_API int gvd_model_create_mode(const gvd_dims_t* dims, int att_input_mode, gvd_model_t** out);   /* region_attn_mode 'mix' */
 /* opt.region_attn_mode (opts.py:63-64, AttModel.py:56-108): how the region attention Attention2 (and attention2_dual in DUAL_REGION)
  * scores proposal r against the query q = h2att(h_att).  The temporal attention is additive in every mode; the grounding is unchanged.
@@ -77,6 +79,25 @@ GVD_API int gvd_model_create_mode(const gvd_dims_t* dims, int att_input_mode, gv
 #define GVD_REGION_ATTN_MIX_MUL 1
 #define GVD_REGION_ATTN_DP 2
 GVD_API int gvd_model_create_modes(const gvd_dims_t* dims, int att_input_mode, int region_attn_mode, gvd_model_t** out);
+/* opt.transfer_mode (opts.py:62, model.py:84-85,180-215): how the class side of the region-class similarity comes from the detector.
+ *   CLS  (0) vis_embed and the model-level vis_classifiers_bias [D+1] start from the detector's classifier (the default);
+ *   NONE (1) the "no knowledge transfer" ablation: the module has no vis_classifiers_bias, so the similarity (model.py:326-336,524-533,
+ *            652-661) and the teacher-forced grounding logits (model.py:472-476) carry no class bias, and the parameter list is one entry
+ *            shorter (the first one).  Everything else is that of CLS.
+ * 'glove' and 'both' cannot run in the reference and are rejected: 'glove' sizes the fc7 layer ctx2pool_grd [300, 2048] and fails copying
+ * the detector's [2048, 2048] fc7 weights into it (model.py:88-89,158,177); 'both' makes fc7 2348 wide, so the region features reach
+ * pool_embed 300 columns wider than it was built for: the reference fails reshaping them to pool_feat_size (model.py:86-87,70,370). */
+#define GVD_TRANSFER_CLS 0
+#define GVD_TRANSFER_NONE 1
+/* butd = opt.enable_BUTD (opts.py:66, model.py:65-69,357-364,537-547): the bottom-up baseline.  The region features are the fc7 output
+ * alone: no location embedding, no label features, no LayerNorms, so pool_embed.0.weight is [rnn_size, att_feat_size = 2048] (loc_fc.* stays
+ * in the parameter list: the reference builds it, unused).  It needs att_input_mode GVD_ATT_INPUT_REGION (the reference asserts the pair,
+ * model.py:66), and REGION needs butd = 1; any other pairing is rejected.  The prologue then skips the region-embedding row kernel, runs the
+ * similarity stage only when sim_mat_out is given, and (with pack fusion) fc7 stores only the operand image its readers stream, so the
+ * workspace's "g_pool" is not written.  Such a model serves the transformer captioner (gvd_prologue_fwd + pool_feats into gvd_tfm_*);
+ * the top-down decode, beam, teacher-forced, single-step and host-buffer entry points reject it. */
+GVD_API int gvd_model_create_opts(const gvd_dims_t* dims, int att_input_mode, int region_attn_mode, int transfer_mode, int butd,
+                                  gvd_model_t** out);
 GVD_API void gvd_model_destroy(gvd_model_t* m);
 /* Copy one state_dict entry (by its reference key, e.g. "core.att_lstm.weight_ih") from a
  * DEVICE fp32 buffer of `numel` elements into the model's packed weight arena. */
