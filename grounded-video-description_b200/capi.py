@@ -25,6 +25,7 @@ EXPORTS = [
     "gvd_tfm_workspace_bytes", "gvd_tfm_decode_greedy", "gvd_tfm_teacher_fwd",
     "gvd_grounding_extract", "gvd_grounding_eval", "gvd_plan_skinny_splits", "gvd_plan_h2d_chunks", "gvd_workspace_bytes_beam", "gvd_beam_decode", "gvd_workspace_bytes_teacher", "gvd_teacher_fwd",
     "gvd_workspace_bytes_video", "gvd_prologue_fwd_video", "gvd_sample_greedy_host_video", "gvd_op_attention_video",
+    "gvd_workspace_bytes_beam_att2", "gvd_beam_decode_att2", "gvd_op_beam_att2_scripted",
     # training-step primitives (csrc/gvd_train.cu; bound in train_ops.py)
     "gvd_tr_adam_first_step", "gvd_tr_adam_flat", "gvd_tr_sgd_flat", "gvd_tr_adamax_flat", "gvd_tr_grad_norm", "gvd_tr_sumsq_scratch_bytes", "gvd_tr_att_scores_bwd", "gvd_tr_att_scores_fwd", "gvd_tr_att_scores_mul_bwd", "gvd_tr_att_scores_mul_fwd", "gvd_tr_bn_bwd", "gvd_tr_bn_normalize", "gvd_tr_cls_nll", "gvd_tr_colsum", "gvd_tr_count_inv", "gvd_tr_scalar_mul", "gvd_tr_dropout", "gvd_tr_ew", "gvd_tr_gather_rows", "gvd_tr_gemm_nt_batched", "gvd_tr_gru_cell_bwd", "gvd_tr_gru_cell_fwd", "gvd_tr_index_add_rows", "gvd_tr_lm_nll", "gvd_tr_ln_bwd", "gvd_tr_ln_fwd", "gvd_tr_ln_star_bwd", "gvd_tr_ln_star_fwd", "gvd_tr_lstm_cell_bwd", "gvd_tr_lstm_cell_fwd", "gvd_tr_mean_dim1", "gvd_tr_mha_bwd", "gvd_tr_mha_fwd", "gvd_tr_outer_rows", "gvd_tr_outer_rows_acc", "gvd_tr_pos_nll", "gvd_tr_rowsum", "gvd_tr_softmax_bwd", "gvd_tr_softmax_fwd", "gvd_tr_sum_all", "gvd_tr_targets", "gvd_tr_transpose",
 ]
@@ -71,6 +72,9 @@ def lib():
     L.gvd_workspace_bytes_beam.argtypes = [vp, ci, ci, ci]
     L.gvd_workspace_bytes_beam.restype = sz
     L.gvd_beam_decode.argtypes = [vp, ci, ci, ci, vp, sz, vp, vp, vp, vp, vp]
+    L.gvd_workspace_bytes_beam_att2.argtypes = [vp, ci, ci, ci, ci]
+    L.gvd_workspace_bytes_beam_att2.restype = sz
+    L.gvd_beam_decode_att2.argtypes = [vp, ci, ci, ci, vp, sz, vp, vp, vp, vp, vp, vp]
     L.gvd_workspace_bytes_teacher.argtypes = [vp, ci, ci, ci]
     L.gvd_workspace_bytes_teacher.restype = sz
     L.gvd_teacher_fwd.argtypes = [vp, ci, ci, ci, ci, ci, vp, sz, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp, vp]
@@ -116,6 +120,7 @@ def lib():
     L.gvd_op_beam_topk.argtypes = [vp, i64, ci, ci, ci, vp, vp, vp]
     L.gvd_op_row_argmax.argtypes = [vp, i64, ci, ci, vp, vp]
     L.gvd_op_beam_search_scripted.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
+    L.gvd_op_beam_att2_scripted.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp, vp]
     L.gvd_set_backend.argtypes = [ci]
     L.gvd_tfm_workspace_bytes.argtypes = [vp, ci, ci, ci, ci]
     L.gvd_tfm_workspace_bytes.restype = sz
@@ -320,11 +325,12 @@ class NativeModel:
         del keep
 
     # ---- workspace
-    def workspace(self, B, T, beam=1, nbox=0, V=None):
+    def workspace(self, B, T, beam=1, nbox=0, V=None, att2=False):
         """The (single) live workspace, sized for a decode with `beam` rows per clip and `nbox` GT boxes.  The prologue's outputs
         live INSIDE it, so a decode entry point that would need a larger allocation than the one the prologue ran in raises instead
         of silently reallocating (and then decoding from uninitialised memory): size it up front with prologue(..., beam=, nbox=).
-        V: the layout of a video-indexed batch of V videos (0: per clip); None: the layout of the live prologue's batch."""
+        V: the layout of a video-indexed batch of V videos (0: per clip); None: the layout of the live prologue's batch.
+        att2 (beam > 1): also the logit history of beam_decode_att2."""
         self._check_device()
         key = (B, T, self.device)
         ws = self._ws.get(key)
@@ -336,11 +342,16 @@ class NativeModel:
             need = int(self._L.gvd_workspace_bytes_beam(self._h, B, T, beam))
             if nbox:
                 need = max(need, int(self._L.gvd_workspace_bytes_teacher(self._h, B, T, nbox)))
+        if att2 and beam > 1:
+            need = max(need, int(self._L.gvd_workspace_bytes_beam_att2(self._h, B, V, T, beam)))
+        # the prologue lays the workspace out for one decode row per clip, and a beam layout can be the smaller one (B * beam > 128 rows
+        # have no split-K slots)
+        need = max(need, int(self._L.gvd_workspace_bytes_video(self._h, B, V, T, 1, 0)) if V else int(self._L.gvd_workspace_bytes(self._h, B, T)))
         if ws is not None and ws.numel() < need:
             if self._live is not None and self._live[:2] == (B, T) and (beam > 1 or nbox > 0):
                 raise GvdError("the workspace holding this batch's prologue outputs (sized for beam=%d, nbox=%d) is too small for the requested "
-                               "decode (beam=%d, nbox=%d): call prologue(..., beam=%d, nbox=%d) first" %
-                               (self._live[2], self._live[3], beam, nbox, beam, nbox))
+                               "decode (beam=%d, nbox=%d%s): call prologue(..., beam=%d, nbox=%d%s) first" %
+                               (self._live[2], self._live[3], beam, nbox, ", att2" if att2 else "", beam, nbox, ", att2=True" if att2 else ""))
             ws = None                              # a larger layout was requested before any prologue ran in it: reallocate
         if ws is None:
             self._live, self._live_V = None, 0
@@ -364,15 +375,16 @@ class NativeModel:
         return ws[off:off + 4 * n].view(torch.float32).view(*shape)
 
     # ---- hot path
-    def prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, want_sim=True, beam=1, nbox=0, video_idx=None):
+    def prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, want_sim=True, beam=1, nbox=0, video_idx=None, att2=False):
         """video_idx (int64 [B], CUDA): a video-indexed batch.  segs_feat then holds the frame features of V videos [V,T,F] and clip b is
-        event b of video video_idx[b] with its window sample_idx[b]; every result equals the per-clip prologue on segs_feat[video_idx]."""
+        event b of video video_idx[b] with its window sample_idx[b]; every result equals the per-clip prologue on segs_feat[video_idx].
+        att2: size the workspace for beam_decode_att2 as well."""
         self._check_device(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, video_idx)
         T = segs_feat.shape[1]
         B = check_video_batch(segs_feat, video_idx, ppls, num, ppls_feat, sample_idx, pnt_mask) if video_idx is not None else segs_feat.shape[0]
         V = segs_feat.shape[0] if video_idx is not None else 0
         self._live, self._live_V = None, 0
-        ws = self.workspace(B, T, beam, nbox, V)
+        ws = self.workspace(B, T, beam, nbox, V, att2)
         sim = torch.empty(B, self.dims.detect_size + 1, self.R, dtype=torch.float32, device="cuda") if want_sim else None
         common = (_dev(ppls, torch.float32, "ppls"), _dev(num, torch.int64, "num"), _dev(ppls_feat, torch.float32, "ppls_feat"),
                   _dev(sample_idx, torch.int64, "sample_idx"))
@@ -421,6 +433,21 @@ class NativeModel:
                                       _dev(pnt_mask, torch.uint8, "pnt_mask"), ctypes.c_void_p(seq.data_ptr()),
                                       ctypes.c_void_p(logp.data_ptr()), ctypes.c_void_p(att.data_ptr()), _stream()))
         return seq, logp, att
+
+    def beam_decode_att2(self, B, T, beam_size, pnt_mask):
+        """beam_decode plus the region-attention logits of each returned caption [B,L,R] (gvd_beam_decode_att2): row t is the logit row the
+        caption's own beam used to pick word t, rows after its last word are 0.  The prologue must have run with att2=True."""
+        ws = self.workspace(B, T, beam_size, att2=True)
+        L = self.dims.seq_length
+        seq = torch.empty(B, L, dtype=torch.int64, device="cuda")
+        logp = torch.empty(B, L, dtype=torch.float32, device="cuda")
+        att = torch.empty(B, L, dtype=torch.int64, device="cuda")
+        att2 = torch.empty(B, L, self.R, dtype=torch.float32, device="cuda")
+        check(self._L.gvd_beam_decode_att2(self._h, B, T, int(beam_size), ctypes.c_void_p(ws.data_ptr()), ws.numel(),
+                                           _dev(pnt_mask, torch.uint8, "pnt_mask"), ctypes.c_void_p(seq.data_ptr()),
+                                           ctypes.c_void_p(logp.data_ptr()), ctypes.c_void_p(att.data_ptr()), ctypes.c_void_p(att2.data_ptr()),
+                                           _stream()))
+        return seq, logp, att, att2
 
     def teacher_forward(self, B, T, S, mode, seq, input_cls, ppls, gt_boxes, mask_boxes, frm_mask, pnt_mask):
         """'MLE' (mode 0) -> losses[4]; 'GRD' (mode 1) -> (att_idx, grd_idx, sim_target, cls_pred)."""
@@ -828,6 +855,21 @@ def op_beam_search_scripted(logits, z, probe, K):
     check(lib().gvd_op_beam_search_scripted(_dev(logits, torch.float32, "logits"), _dev(z, torch.float32, "z"), _dev(probe, torch.float32, "probe"),
                                             B, int(K), L, V, R, H, _ptr(seq), _ptr(logp), _ptr(att), _ptr(parents), _stream()))
     return seq, logp, att, parents
+
+
+def op_beam_att2_scripted(logits, z, probe, K):
+    """op_beam_search_scripted plus att2 [B, L, R] (pre-filled with NaN): the rows of z the returned caption used (gvd_op_beam_att2_scripted)."""
+    L, BK, V = logits.shape
+    R, H = z.shape[2], probe.shape[1]
+    B = BK // K
+    seq = torch.full((B, L), -7, dtype=torch.int64, device="cuda")
+    logp = torch.full((B, L), float("nan"), dtype=torch.float32, device="cuda")
+    att = torch.full((B, L), -7, dtype=torch.int64, device="cuda")
+    parents = torch.full((L, BK), -7, dtype=torch.int32, device="cuda")
+    att2 = torch.full((B, L, R), float("nan"), dtype=torch.float32, device="cuda")
+    check(lib().gvd_op_beam_att2_scripted(_dev(logits, torch.float32, "logits"), _dev(z, torch.float32, "z"), _dev(probe, torch.float32, "probe"),
+                                          B, int(K), L, V, R, H, _ptr(seq), _ptr(logp), _ptr(att), _ptr(parents), _ptr(att2), _stream()))
+    return seq, logp, att, parents, att2
 
 
 def op_linear(A, W, bias=None, act=0, tc=False):

@@ -588,6 +588,7 @@ struct WS {
     BeamBufs bb;
     int* bos_att;
     float *z_rows, *gather_tmp;
+    float* att2_hist;                  // gvd_beam_decode_att2 only: [L][B*K][R] (with bb.parent_hist / bb.done_step)
     // teacher-forced path (MLE / GRD)
     float *ov, *outs, *z_all, *emb, *G, *logits_all, *part_sum;
     unsigned char *labels, *fm;
@@ -610,7 +611,9 @@ static void attn_chunking(int B, int R, int T, int* RC, int* TC) {
     *TC = pick(T);
 }
 
-static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, int nbox = 0, int V = 0) {
+// att2_hist (beam > 1): also the beam's logit history for gvd_beam_decode_att2, after every other slot so that the layout without it is
+// unchanged
+static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, int nbox = 0, int V = 0, bool att2_hist = false) {
     const gvd_dims_t& d = m->d;
     const int H = d.rnn_size, A = d.att_hid_size, R = m->R, G = m->G;
     WS w{};
@@ -747,6 +750,12 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
         w.part_cnt = (int*)take(std::max((size_t)B * L, (size_t)B * NB) * 4);
         w.tok_col = (long long*)take((size_t)B * 8);
     }
+    if (beam > 1 && att2_hist) {
+        const size_t L = d.seq_length;
+        w.att2_hist = (float*)take(L * BD * R * 4);       // step t's region-attention logits of every beam row, [L][B*K][R]
+        w.bb.parent_hist = (int*)take(L * BD * 4);
+        w.bb.done_step = (int*)take((size_t)B * 4);
+    }
     w.bytes = off;
     return w;
 }
@@ -762,6 +771,11 @@ extern "C" GVD_API size_t gvd_workspace_bytes_teacher(const gvd_model_t* m, int 
 extern "C" GVD_API size_t gvd_workspace_bytes_beam(const gvd_model_t* m, int B, int T, int beam_size) {
     if (!m || B < 1 || T < 1 || beam_size < 1) return 0;
     return ws_layout(m, B, T, nullptr, beam_size).bytes;
+}
+
+extern "C" GVD_API size_t gvd_workspace_bytes_beam_att2(const gvd_model_t* m, int B, int V, int T, int beam_size) {
+    if (!m || B < 1 || V < 0 || T < 1 || beam_size < 2) return 0;
+    return ws_layout(m, B, T, nullptr, beam_size, 0, V, true).bytes;
 }
 
 extern "C" GVD_API size_t gvd_workspace_bytes_video(const gvd_model_t* m, int B, int V, int T, int beam_size, int nbox) {
@@ -809,11 +823,12 @@ static int require_topdown(const gvd_model* m, const char* who) {
     return 0;
 }
 
-static int check_ws(const gvd_model* m, int B, int T, void* workspace, size_t bytes, WS* w, int beam = 1, int nbox = 0, int V = -1) {
+static int check_ws(const gvd_model* m, int B, int T, void* workspace, size_t bytes, WS* w, int beam = 1, int nbox = 0, int V = -1,
+                    bool att2_hist = false) {
     GVD_REQUIRE(m && m->finalized, "model not finalized (call gvd_model_finalize after setting every parameter)");
     GVD_REQUIRE(B >= 1 && T >= 1, "bad batch/frames B=%d T=%d", B, T);
     GVD_REQUIRE(workspace && ((uintptr_t)workspace & 255) == 0, "workspace must be a 256-byte aligned device pointer");
-    *w = ws_layout(m, B, T, workspace, beam, nbox, V < 0 ? video_of(m, workspace, B, T) : V);
+    *w = ws_layout(m, B, T, workspace, beam, nbox, V < 0 ? video_of(m, workspace, B, T) : V, att2_hist);
     GVD_REQUIRE(bytes >= w->bytes, "workspace too small: %zu < %zu bytes", bytes, w->bytes);
     return 0;
 }
@@ -1536,11 +1551,13 @@ extern "C" GVD_API int gvd_teacher_fwd(gvd_model_t* m, int B, int T, int nbox, i
 //   then for t = 0 .. L-1: logits(t), beam_topk, beam_update and, but at the last step (the reference runs one more, unused, core step),
 //   the recurrent rows of state(t) reordered to the surviving beams (CaptionModelBU.py:85-89), scores(t + 1), row_argmax; finally beam_finish.
 // scores(t) runs model step t on bb.tokens and returns its region scores [B*K, R]; logits(t, &ld) returns step t's logits [B*K, V] (pitch
-// ld); state(t, bufs) fills at most 4 recurrent [B*K, H] buffers and returns their number.  parents_out: optional [L][B*K] copy of every
-// step's bb.parent.
+// ld); state(t, bufs) fills at most 4 recurrent [B*K, H] buffers and returns their number.  bb.parent_hist / bb.done_step (optional) keep
+// every step's parents and the finishing step.  att2_out (optional, needs both): the region scores of the returned caption [B, L, R]
+// gathered along its ancestor chain by beam_backtrack; scores(t) must then have left step t's scores at z_hist + t * B*K*R.
 template <class Scores, class Logits, class State>
 static int beam_search_run(const BeamBufs& bb, int* bos_att, float* gather_tmp, int B, int K, int L, int V, int R, int H, int64_t* seq_out,
-                           float* lp_out, int64_t* att_out, int* parents_out, cudaStream_t st, Scores scores, Logits logits, State state) {
+                           float* lp_out, int64_t* att_out, const float* z_hist, float* att2_out, cudaStream_t st, Scores scores, Logits logits,
+                           State state) {
     const int BK = B * K;
     GVD_CHECK_CUDA(cudaMemsetAsync(bb.tokens, 0, (size_t)BK * 8, st));
     GVD_CHECK_CUDA(cudaMemsetAsync(bb.seq, 0, (size_t)B * L * K * 4, st));
@@ -1558,7 +1575,6 @@ static int beam_search_run(const BeamBufs& bb, int* bos_att, float* gather_tmp, 
         GVD_TRY(logits(t, &lg, &ld));
         GVD_STAGE("beam.topk", gvd_beam_topk(lg, ld, BK, V, K, bb.topv, bb.topi, st));
         GVD_STAGE("beam.update", gvd_beam_update(bb, B, K, L, t, st));
-        if (parents_out) GVD_CHECK_CUDA(cudaMemcpyAsync(parents_out + (size_t)t * BK, bb.parent, (size_t)BK * 4, cudaMemcpyDeviceToDevice, st));
         if (t == L - 1) break;
         float* bufs[4];
         const int n = state(t, bufs);
@@ -1570,16 +1586,20 @@ static int beam_search_run(const BeamBufs& bb, int* bos_att, float* gather_tmp, 
         GVD_STAGE("beam.argmax", gvd_row_argmax(z, R, BK, R, bb.att_ind, st));
     }
     GVD_STAGE("beam.finish", gvd_beam_finish(bb, bos_att, B, K, L, (long long*)seq_out, lp_out, (long long*)att_out, st));
+    if (att2_out) GVD_STAGE("beam.backtrack", gvd_beam_backtrack(bb, z_hist, (long long)BK * R, B, K, L, R, att2_out, st));
     return 0;
 }
 
-// B1/B2: beam search for every clip at once (misc/model.py:700-742 + misc/CaptionModelBU.py:104-185, repaired semantics)
-extern "C" GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_size, void* workspace, size_t workspace_bytes,
-                                       const uint8_t* pnt_mask, int64_t* seq_out, float* logprobs_out, int64_t* att2_idx_out, void* stream) {
+// B1/B2: beam search for every clip at once (misc/model.py:700-742 + misc/CaptionModelBU.py:104-185, repaired semantics).  att2_logits_out
+// (gvd_beam_decode_att2): each step's region scores land in the workspace's history instead of z_rows, and the returned caption's rows are
+// gathered from it at the end.
+static int beam_decode(gvd_model_t* m, int B, int T, int beam_size, void* workspace, size_t workspace_bytes, const uint8_t* pnt_mask,
+                       int64_t* seq_out, float* logprobs_out, int64_t* att2_idx_out, float* att2_logits_out, void* stream) {
     GVD_TRY(require_topdown(m, "beam_decode"));
     GVD_REQUIRE(beam_size >= 2, "beam_decode: beam_size must be >= 2 (use gvd_decode_greedy for 1)");
     WS w;
-    GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w, beam_size));
+    const bool hist = att2_logits_out != nullptr;
+    GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w, beam_size, 0, -1, hist));
     GVD_REQUIRE(pnt_mask && seq_out && logprobs_out && att2_idx_out, "beam_decode: null argument");
     cudaStream_t st = (cudaStream_t)stream;
     const gvd_dims_t& d = m->d;
@@ -1595,8 +1615,9 @@ extern "C" GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_si
     }
     // core step t on the beam tokens; step 0 is the <bos> step (model.py:723-733), whose K rows of a clip are identical
     auto scores = [&](int t, const float** z) {
-        *z = w.z_rows;
-        return core_step(m, w, BK, T, t, w.bb.tokens, pnt_mask, pnt_mask, w.z_rows, R, st, K);
+        float* zt = hist ? w.att2_hist + (size_t)t * BK * R : w.z_rows;
+        *z = zt;
+        return core_step(m, w, BK, T, t, w.bb.tokens, pnt_mask, pnt_mask, zt, R, st, K);
     };
     auto logits = [&](int t, const float** lg, long long* ld) {
         const float* h_lang = w.h_lang + (size_t)((t + 1) & 1) * BKH;   // state parity written by the previous core step
@@ -1610,7 +1631,18 @@ extern "C" GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_si
         bufs[0] = w.h_att + (size_t)par * BKH; bufs[1] = w.c_att; bufs[2] = w.h_lang + (size_t)par * BKH; bufs[3] = w.c_lang;
         return 4;
     };
-    return beam_search_run(w.bb, w.bos_att, w.gather_tmp, B, K, L, V, R, H, seq_out, logprobs_out, att2_idx_out, nullptr, st, scores, logits, state);
+    return beam_search_run(w.bb, w.bos_att, w.gather_tmp, B, K, L, V, R, H, seq_out, logprobs_out, att2_idx_out, w.att2_hist, att2_logits_out, st,
+                           scores, logits, state);
+}
+extern "C" GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_size, void* workspace, size_t workspace_bytes,
+                                       const uint8_t* pnt_mask, int64_t* seq_out, float* logprobs_out, int64_t* att2_idx_out, void* stream) {
+    return beam_decode(m, B, T, beam_size, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_idx_out, nullptr, stream);
+}
+extern "C" GVD_API int gvd_beam_decode_att2(gvd_model_t* m, int B, int T, int beam_size, void* workspace, size_t workspace_bytes,
+                                            const uint8_t* pnt_mask, int64_t* seq_out, float* logprobs_out, int64_t* att2_idx_out,
+                                            float* att2_logits_out, void* stream) {
+    GVD_REQUIRE(att2_logits_out, "beam_decode_att2: null att2_logits_out");
+    return beam_decode(m, B, T, beam_size, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_idx_out, att2_logits_out, stream);
 }
 
 // Clip chunks of the host-buffer entry point.  The pipeline starts with one attention sub-batch (`unit` clips: the first kernel waits for the
@@ -2072,14 +2104,14 @@ extern "C" GVD_API int gvd_op_row_argmax(const float* z, int64_t ld, int rows, i
 // gvd_beam_decode's bookkeeping (beam_search_run) with the model replaced by a script: step t's logits are logits[t] [B*K, V], the region
 // scores of core step t are z[t] [B*K, R] (t = 0: <bos>), and the recurrent state is one probe buffer [B*K, H] that is reordered like the
 // model's state.  The bookkeeping buffers are allocated here.  Test hook.
-extern "C" GVD_API int gvd_op_beam_search_scripted(const float* logits, const float* z, float* probe, int B, int K, int L, int V, int R, int H,
-                                                   int64_t* seq_out, float* logp_out, int64_t* att2_idx_out, int* parents_out, void* stream) {
+static int beam_search_scripted(const float* logits, const float* z, float* probe, int B, int K, int L, int V, int R, int H, int64_t* seq_out,
+                                float* logp_out, int64_t* att2_idx_out, int* parents_out, float* att2_out, void* stream) {
     GVD_REQUIRE(logits && z && probe && seq_out && logp_out && att2_idx_out && parents_out && B >= 1 && V >= 1 && R >= 1 && H >= 4 && H % 4 == 0,
                 "op_beam_search_scripted: bad arguments");
     GVD_REQUIRE(K >= 1 && L >= 1, "op_beam_search_scripted: beam_size and seq_length must be >= 1");
     cudaStream_t st = (cudaStream_t)stream;
     const size_t BK = (size_t)B * K, BLK = (size_t)B * L * K;
-    const size_t n4 = 3 * BLK + 2 * BK * K + 4 * BK + 2 * (size_t)B + 2 * (size_t)B * L;   // 4-byte words after the gather rows and tokens
+    const size_t n4 = 3 * BLK + 2 * BK * K + 4 * BK + 3 * (size_t)B + 2 * (size_t)B * L;   // 4-byte words after the gather rows and tokens
     char* buf = nullptr;
     GVD_CHECK_CUDA(cudaMallocAsync((void**)&buf, BK * H * 4 + BK * 8 + n4 * 4, st));
     float* gather_tmp = (float*)buf;                                 // [B*K, H], 16-byte rows
@@ -2090,14 +2122,27 @@ extern "C" GVD_API int gvd_op_beam_search_scripted(const float* logits, const fl
     bb.seq = take(BLK); bb.att = take(BLK); bb.lp = (float*)take(BLK); bb.topv = (float*)take(BK * K); bb.topi = take(BK * K);
     bb.sums = (float*)take(BK); bb.parent = take(BK); bb.att_ind = take(BK);
     int* bos_att = take(BK);
-    bb.done_flag = take(B); bb.done_slot = take(B); bb.done_seq = take((size_t)B * L); bb.done_lp = (float*)take((size_t)B * L);
+    bb.done_flag = take(B); bb.done_slot = take(B); bb.done_step = take(B); bb.done_seq = take((size_t)B * L); bb.done_lp = (float*)take((size_t)B * L);
+    bb.parent_hist = parents_out;
     auto scores = [&](int t, const float** zt) { *zt = z + (size_t)t * BK * R; return 0; };
     auto step_logits = [&](int t, const float** lg, long long* ld) { *lg = logits + (size_t)t * BK * V; *ld = V; return 0; };
     auto state = [&](int, float** bufs) { bufs[0] = probe; return 1; };
-    const int rc = beam_search_run(bb, bos_att, gather_tmp, B, K, L, V, R, H, seq_out, logp_out, att2_idx_out, parents_out, st, scores, step_logits,
+    const int rc = beam_search_run(bb, bos_att, gather_tmp, B, K, L, V, R, H, seq_out, logp_out, att2_idx_out, z, att2_out, st, scores, step_logits,
                                    state);
     cudaFreeAsync(buf, st);
     return rc;
+}
+extern "C" GVD_API int gvd_op_beam_search_scripted(const float* logits, const float* z, float* probe, int B, int K, int L, int V, int R, int H,
+                                                   int64_t* seq_out, float* logp_out, int64_t* att2_idx_out, int* parents_out, void* stream) {
+    return beam_search_scripted(logits, z, probe, B, K, L, V, R, H, seq_out, logp_out, att2_idx_out, parents_out, nullptr, stream);
+}
+// ... and the region scores of the returned caption, gathered along its ancestor chain from the script's z (gvd_beam_decode_att2's
+// att2_logits_out).  Test hook.
+extern "C" GVD_API int gvd_op_beam_att2_scripted(const float* logits, const float* z, float* probe, int B, int K, int L, int V, int R, int H,
+                                                 int64_t* seq_out, float* logp_out, int64_t* att2_idx_out, int* parents_out, float* att2_out,
+                                                 void* stream) {
+    GVD_REQUIRE(att2_out, "op_beam_att2_scripted: null att2_out");
+    return beam_search_scripted(logits, z, probe, B, K, L, V, R, H, seq_out, logp_out, att2_idx_out, parents_out, att2_out, stream);
 }
 // Batched short-K product C[b,h] = A[b,:,h*hs:(h+1)*hs] . W[b,:,h*hs:(h+1)*hs]^T through the A-stationary kernel (the attention-score shape)
 extern "C" GVD_API int gvd_op_scores_tc(const float* A, const float* W, float* C, int nb, int nh, int M, int N, int hs, int64_t ld, void* stream) {

@@ -120,6 +120,7 @@ __global__ void beam_update_kernel(BeamBufs bb, int B, int K, int L, int t) {
         if (t >= 1) att[t * K + v] = pw[v];
         sums[v] = pp[v];
         bb.parent[(long long)b * K + v] = pq[v];
+        if (bb.parent_hist) bb.parent_hist[((long long)t * B + b) * K + v] = pq[v];
         bb.tokens[(long long)b * K + v] = ptok[v];
     }
     for (int v = 0; v < K; ++v) {
@@ -127,6 +128,7 @@ __global__ void beam_update_kernel(BeamBufs bb, int B, int K, int L, int t) {
             if (!bb.done_flag[b]) {                       // first pushed beam wins (see file header)
                 bb.done_flag[b] = 1;
                 bb.done_slot[b] = v;
+                if (bb.done_step) bb.done_step[b] = t;
                 for (int tt = 0; tt < L; ++tt) {
                     bb.done_seq[(long long)b * L + tt] = tt <= t ? seq[tt * K + v] : 0;
                     bb.done_lp[(long long)b * L + tt] = tt <= t ? lp[tt * K + v] : 0.f;
@@ -185,6 +187,44 @@ __global__ void beam_finish_kernel(BeamBufs bb, const int* __restrict__ bos_att,
     att_out[idx] = t == 0 ? bos_att[b * K] : bb.att[((long long)b * L + t) * K + bb.done_slot[b]];
 }
 
+// The region-attention logits the returned caption used (one CTA per clip).  Word t of the beam in slot s at step t was picked from the
+// logits of old row parent_t[s] of step t, and that row is the beam's slot at step t - 1: walking the parents back from (done_step,
+// done_slot) gives the row of every step.  hist holds step t's rows [B*K][R] at hist + t * step_stride.  out [B][L][R]: the rows up to
+// the finishing step, zeros after it.  VEC: R, step_stride and both pointers allow float4 accesses.
+template <bool VEC>
+__global__ void __launch_bounds__(256) beam_backtrack_kernel(BeamBufs bb, const float* __restrict__ hist, long long step_stride, int B, int K,
+                                                             int L, int R, float* __restrict__ out) {
+    __shared__ int par[BEAM_MAXL * BEAM_MAXK];
+    __shared__ int src[BEAM_MAXL];
+    const int b = blockIdx.x;
+    for (int i = threadIdx.x; i < L * K; i += blockDim.x) par[i] = bb.parent_hist[((long long)(i / K) * B + b) * K + i % K];
+    __syncthreads();
+    const int tf = bb.done_step[b];
+    if (threadIdx.x == 0) {
+        int slot = bb.done_slot[b];
+        for (int t = tf; t >= 0; --t) {
+            slot = par[t * K + slot];
+            src[t] = b * K + slot;
+        }
+    }
+    __syncthreads();
+    float* o = out + (long long)b * L * R;
+    if (VEC) {
+        const int R4 = R / 4;
+        for (int i = threadIdx.x; i < L * R4; i += blockDim.x) {
+            const int t = i / R4, c = i - t * R4;
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (t <= tf) v = __ldg(reinterpret_cast<const float4*>(hist + t * step_stride + (long long)src[t] * R) + c);
+            reinterpret_cast<float4*>(o + (long long)t * R)[c] = v;
+        }
+    } else {
+        for (int i = threadIdx.x; i < L * R; i += blockDim.x) {
+            const int t = i / R, c = i - t * R;
+            o[i] = t <= tf ? __ldg(hist + t * step_stride + (long long)src[t] * R + c) : 0.f;
+        }
+    }
+}
+
 }  // namespace
 
 int gvd_beam_topk(const float* logits, long long ld, int rows, int V, int K, float* topv, int* topi, cudaStream_t st) {
@@ -212,6 +252,16 @@ int gvd_row_argmax(const float* z, long long ld, int rows, int R, int* out, cuda
 int gvd_beam_finish(const BeamBufs& bb, const int* bos_att, int B, int K, int L, long long* seq_out, float* lp_out, long long* att_out,
                     cudaStream_t st) {
     beam_finish_kernel<<<gvd_cdiv((long long)B * L, 256), 256, 0, st>>>(bb, bos_att, B, K, L, seq_out, lp_out, att_out);
+    GVD_CHECK_LAUNCH();
+    return 0;
+}
+int gvd_beam_backtrack(const BeamBufs& bb, const float* hist, long long step_stride, int B, int K, int L, int R, float* out, cudaStream_t st) {
+    GVD_REQUIRE(bb.parent_hist && bb.done_step && K <= BEAM_MAXK && L <= BEAM_MAXL, "beam: backtrack needs the parent history");
+    const bool vec = R % 4 == 0 && step_stride % 4 == 0 && ((uintptr_t)hist & 15) == 0 && ((uintptr_t)out & 15) == 0;
+    if (vec)
+        beam_backtrack_kernel<true><<<B, 256, 0, st>>>(bb, hist, step_stride, B, K, L, R, out);
+    else
+        beam_backtrack_kernel<false><<<B, 256, 0, st>>>(bb, hist, step_stride, B, K, L, R, out);
     GVD_CHECK_LAUNCH();
     return 0;
 }

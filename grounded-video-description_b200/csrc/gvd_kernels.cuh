@@ -92,6 +92,7 @@ struct BeamBufs {
     int *seq, *att, *parent, *att_ind, *done_flag, *done_slot, *topi, *done_seq;   // seq/att: [B][L][K]; topi: [B*K][K]
     float *lp, *sums, *topv, *done_lp;                                              // lp: [B][L][K]; sums: [B][K]; topv: [B*K][K]
     long long* tokens;                                                              // [B*K]
+    int *parent_hist, *done_step;      // optional (NULL: not kept): every step's parent [L][B*K]; the step at which done_slot finished [B]
 };
 int gvd_beam_topk(const float* logits, long long ld, int rows, int V, int K, float* topv, int* topi, cudaStream_t st);
 int gvd_beam_update(const BeamBufs& bb, int B, int K, int L, int t, cudaStream_t st);
@@ -99,6 +100,7 @@ int gvd_beam_gather_rows(const float* src, float* dst, const int* parent, int B,
 int gvd_row_argmax(const float* z, long long ld, int rows, int R, int* out, cudaStream_t st);
 int gvd_beam_finish(const BeamBufs& bb, const int* bos_att, int B, int K, int L, long long* seq_out, float* lp_out, long long* att_out,
                     cudaStream_t st);
+int gvd_beam_backtrack(const BeamBufs& bb, const float* hist, long long step_stride, int B, int K, int L, int R, float* out, cudaStream_t st);
 
 // ---- wgmma / TMA GEMM (gvd_wgmma.cu)
 // operand-swapped split-K path for the skinny decode-step products (gvd_skinny.cu; backend bit 3)

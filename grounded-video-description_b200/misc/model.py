@@ -199,12 +199,12 @@ class AttModel(CaptionModel):
             return seq, att2, sim_mat
         raise ValueError("unknown forward mode %r (expected 'MLE', 'GRD' or 'sample')" % (opt,))
 
-    def _prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, beam=1, nbox=0, video_idx=None):
+    def _prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, beam=1, nbox=0, video_idx=None, att2=False):
         nm = self._native_model()
         sim = nm.prologue(segs_feat.float().contiguous(), ppls.float().contiguous(), num.long().contiguous(),
                           ppls_feat.float().contiguous(), sample_idx.long().contiguous(), self._u8(pnt_mask).contiguous(),
                           want_sim=not self.enable_BUTD,       # BUTD (transformer only): nothing reads the similarity, so it is not computed
-                          beam=beam, nbox=nbox,     # the workspace is sized for the decode that follows
+                          beam=beam, nbox=nbox, att2=att2,     # the workspace is sized for the decode that follows
                           video_idx=video_idx.contiguous() if video_idx is not None else None)
         return nm, sim
 
@@ -215,11 +215,18 @@ class AttModel(CaptionModel):
 
         Sampling draws from softmax(logits / temperature) like the reference's torch.multinomial, but through counter-based noise keyed by
         a per-call seed (gvd_decode_sample): the seed is one draw from torch's default CPU generator, so torch.manual_seed(s) reproduces a
-        call and successive calls differ.  The draws of a row depend on its index in the batch: splitting a batch changes them."""
+        call and successive calls differ.  The draws of a row depend on its index in the batch: splitting a batch changes them.
+
+        eval_opt['att2_weights'] = True asks for the region-attention logits [B,L,R] of the returned captions as the second output of
+        'sample', the input of extract_grounding.  Greedy and multinomial decoding return them anyway; beam search then returns them
+        instead of its region index per word (see _sample_beam)."""
         sample_max = opt.get("sample_max", 1)
         beam_size = opt.get("beam_size", 1)
         temperature = opt.get("temperature", 1.0)
         video_idx = opt.get("video_idx")
+        if opt.get("att2_weights") and self.att_model == "transformer":
+            raise NotImplementedError("att2_weights: the transformer captioner has no region attention to return (its 'sample' returns zeros "
+                                      "there, model.py:578)")
         if beam_size > 1:
             if self.att_model == "transformer":
                 raise NotImplementedError("the transformer captioner decodes greedily (Decoder.greedy, transformer.py:214); the reference has no "
@@ -272,13 +279,23 @@ class AttModel(CaptionModel):
         The reference crashes here as shipped (12 arguments into the 10-argument core, and `forward`
         unpacks 4 values from the 3 returned); this implements the documented minimal repair
         (SURVEY.md App. A.5 / B D1-D4) and returns 4 values so that `forward(..., 'sample')` works:
-        (seq, seqLogprobs, att2 region INDEX per word [B,L], sim_mat)."""
+        (seq, seqLogprobs, att2 region INDEX per word [B,L], sim_mat).
+
+        opt['att2_weights'] = True: the third value is instead the region-attention logits [B,L,R] fp32 of each returned caption, the
+        grounding that greedy decoding returns: row t is the masked logit row the caption's own beam used to pick word t (row 0 the <bos>
+        step, later rows those of the beam's ancestors, found through the search's parent pointers), rows after the caption's last word 0.
+        They equal the logits of the teacher-forced pass on the caption, and feed extract_grounding as they are."""
         beam_size = opt.get("beam_size", 10)
+        att2 = bool(opt.get("att2_weights", False))
         if self.training:
             raise capi.GvdError("'sample' runs in eval mode (main.py:315); call model.eval()")
         B, T = ppls.size(0), segs_feat.size(1)
-        nm, sim = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, beam=beam_size, video_idx=opt.get("video_idx"))
-        seq, logp, att = nm.beam_decode(B, T, beam_size, self._u8(pnt_mask).contiguous())
+        nm, sim = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, beam=beam_size, video_idx=opt.get("video_idx"), att2=att2)
+        mask = self._u8(pnt_mask).contiguous()
+        if att2:
+            seq, logp, _, att2_w = nm.beam_decode_att2(B, T, beam_size, mask)
+            return seq, logp, att2_w, sim
+        seq, logp, att = nm.beam_decode(B, T, beam_size, mask)
         return seq, logp, att, sim
 
     def _forward_train(self, segs_feat, input_seq, gt_seq, ppls, gt_boxes, mask_boxes, num, ppls_feat, frm_mask, sample_idx, pnt_mask):

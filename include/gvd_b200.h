@@ -199,6 +199,23 @@ GVD_API int gvd_beam_decode(gvd_model_t* m, int B, int T, int beam_size, void* w
                     int64_t* att2_idx_out,        /* [B,L] argmax region index per word   */
                     void* stream);
 
+/* ---- the same beam search, grounded: additionally the region-attention logits of the returned caption (the second output of
+ * forward(..., 'sample') with eval_opt['att2_weights']).  Row t of att2_logits_out is the masked logit row [R] (as gvd_decode_greedy
+ * returns them) that the caption's own beam used to pick word t: row 0 is the <bos> step, row t that of the beam's ancestor at step t,
+ * found by following the parent pointers back from the slot and step at which the caption finished.  Rows after the caption's last word
+ * are 0.  seq_out / logprobs_out / att2_idx_out equal gvd_beam_decode's bit for bit.
+ * Workspace: gvd_workspace_bytes_beam_att2(B, V, T, beam_size) (V = 0: the layout of gvd_prologue_fwd, V > 0: gvd_prologue_fwd_video's):
+ * gvd_workspace_bytes_beam / _video plus a logit history [L][B*beam][R] fp32, the parents of every step and the finishing steps, laid out
+ * after every other slot.  0 for beam_size < 2. */
+GVD_API size_t gvd_workspace_bytes_beam_att2(const gvd_model_t* m, int B, int V, int T, int beam_size);
+GVD_API int gvd_beam_decode_att2(gvd_model_t* m, int B, int T, int beam_size, void* workspace, size_t workspace_bytes,
+                    const uint8_t* pnt_mask,      /* [B,R+1]                              */
+                    int64_t* seq_out,             /* [B,L]                                */
+                    float* logprobs_out,          /* [B,L]                                */
+                    int64_t* att2_idx_out,        /* [B,L] as gvd_beam_decode             */
+                    float* att2_logits_out,       /* [B,L,R] the caption's logit rows     */
+                    void* stream);
+
 /* ---- T1-T6 / G1: teacher-forced forward (misc/model.py:283-489) after gvd_prologue_fwd on the same batch,
  * eval-mode arithmetic (no dropout, BatchNorm running statistics).  Workspace: gvd_workspace_bytes_teacher().
  *   mode 0 'MLE': losses_out[4] = lm, att2, ground, cls (utils.py:122-152, model.py:345-350)
@@ -381,6 +398,9 @@ GVD_API int gvd_op_row_argmax(const float* z, int64_t ld, int rows, int R, int* 
  * gvd_beam_decode returns them; parents_out [L][B*K] int32: every step's parent beam of each new beam (index within the clip). */
 GVD_API int gvd_op_beam_search_scripted(const float* logits, const float* z, float* probe, int B, int K, int L, int V, int R, int H,
                   int64_t* seq_out, float* logp_out, int64_t* att2_idx_out, int* parents_out, void* stream);
+/* ... the same, plus att2_out [B, L, R]: the rows of z the returned caption used, gathered as gvd_beam_decode_att2 gathers them. */
+GVD_API int gvd_op_beam_att2_scripted(const float* logits, const float* z, float* probe, int B, int K, int L, int V, int R, int H,
+                  int64_t* seq_out, float* logp_out, int64_t* att2_idx_out, int* parents_out, float* att2_out, void* stream);
 /* arithmetic backend switches: bit 0 wgmma tensor cores for every GEMM-shaped stage (0 = fp32 CUDA cores); bit 1 fused self-attention pair;
    bit 2 (4) inert; bit 3 (8) operand-swapped split-K decode products with fused
    reduce + sampler; bit 4 (16) fp16x3 instead of 3xTF32 in the forward GEMMs, pre-split weights, conversion-free decode step, tensor-core GRU;
