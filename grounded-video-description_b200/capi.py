@@ -26,6 +26,7 @@ EXPORTS = [
     "gvd_grounding_extract", "gvd_grounding_eval", "gvd_plan_skinny_splits", "gvd_plan_h2d_chunks", "gvd_workspace_bytes_beam", "gvd_beam_decode", "gvd_workspace_bytes_teacher", "gvd_teacher_fwd",
     "gvd_workspace_bytes_video", "gvd_prologue_fwd_video", "gvd_sample_greedy_host_video", "gvd_op_attention_video",
     "gvd_workspace_bytes_beam_att2", "gvd_beam_decode_att2", "gvd_op_beam_att2_scripted",
+    "gvd_workspace_bytes_sample_n", "gvd_decode_sample_n", "gvd_op_attention_path",
     # training-step primitives (csrc/gvd_train.cu; bound in train_ops.py)
     "gvd_tr_adam_first_step", "gvd_tr_adam_flat", "gvd_tr_sgd_flat", "gvd_tr_adamax_flat", "gvd_tr_grad_norm", "gvd_tr_sumsq_scratch_bytes", "gvd_tr_att_scores_bwd", "gvd_tr_att_scores_fwd", "gvd_tr_att_scores_mul_bwd", "gvd_tr_att_scores_mul_fwd", "gvd_tr_bn_bwd", "gvd_tr_bn_normalize", "gvd_tr_cls_nll", "gvd_tr_colsum", "gvd_tr_count_inv", "gvd_tr_scalar_mul", "gvd_tr_dropout", "gvd_tr_ew", "gvd_tr_gather_rows", "gvd_tr_gemm_nt_batched", "gvd_tr_gru_cell_bwd", "gvd_tr_gru_cell_fwd", "gvd_tr_index_add_rows", "gvd_tr_lm_nll", "gvd_tr_ln_bwd", "gvd_tr_ln_fwd", "gvd_tr_ln_star_bwd", "gvd_tr_ln_star_fwd", "gvd_tr_lstm_cell_bwd", "gvd_tr_lstm_cell_fwd", "gvd_tr_mean_dim1", "gvd_tr_mha_bwd", "gvd_tr_mha_fwd", "gvd_tr_outer_rows", "gvd_tr_outer_rows_acc", "gvd_tr_pos_nll", "gvd_tr_rowsum", "gvd_tr_softmax_bwd", "gvd_tr_softmax_fwd", "gvd_tr_sum_all", "gvd_tr_targets", "gvd_tr_transpose",
 ]
@@ -87,6 +88,9 @@ def lib():
     L.gvd_sample_greedy_host_video.argtypes = [vp, ci, ci, ci, vp, vp, vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp]
     L.gvd_decode_greedy.argtypes = [vp, ci, ci, vp, sz, vp, vp, vp, vp, vp]
     L.gvd_decode_sample.argtypes = [vp, ci, ci, vp, sz, vp, ctypes.c_uint64, ctypes.c_float, vp, vp, vp, vp]
+    L.gvd_workspace_bytes_sample_n.argtypes = [vp, ci, ci, ci, ci]
+    L.gvd_workspace_bytes_sample_n.restype = sz
+    L.gvd_decode_sample_n.argtypes = [vp, ci, ci, ci, vp, sz, vp, ctypes.c_uint64, ctypes.c_float, vp, vp, vp, vp]
     L.gvd_decode_step_fwd.argtypes = [vp, ci, ci, vp, sz, ci, vp, vp, vp, vp, i64, vp, vp]
     L.gvd_decode_reset_state.argtypes = [vp, ci, ci, vp, sz, vp]
     L.gvd_sample_greedy_host.argtypes = [vp, ci, ci, vp, vp, vp, vp, vp, vp, vp, sz, vp, vp, vp, vp, vp]
@@ -117,6 +121,7 @@ def lib():
     L.gvd_op_attention_mode.argtypes = L.gvd_op_attention.argtypes[:-1] + [ci, vp, vp, vp, i64, vp]
     L.gvd_op_attention_form.argtypes = L.gvd_op_attention_mode.argtypes[:-1] + [ci, vp]
     L.gvd_op_attention_video.argtypes = L.gvd_op_attention_form.argtypes[:-1] + [vp, vp, vp, vp]
+    L.gvd_op_attention_path.argtypes = L.gvd_op_attention_video.argtypes[:-1] + [ci, vp]
     L.gvd_op_beam_topk.argtypes = [vp, i64, ci, ci, ci, vp, vp, vp]
     L.gvd_op_row_argmax.argtypes = [vp, i64, ci, ci, vp, vp]
     L.gvd_op_beam_search_scripted.argtypes = [vp, vp, vp, ci, ci, ci, ci, ci, ci, vp, vp, vp, vp, vp]
@@ -325,12 +330,12 @@ class NativeModel:
         del keep
 
     # ---- workspace
-    def workspace(self, B, T, beam=1, nbox=0, V=None, att2=False):
+    def workspace(self, B, T, beam=1, nbox=0, V=None, att2=False, rows=1):
         """The (single) live workspace, sized for a decode with `beam` rows per clip and `nbox` GT boxes.  The prologue's outputs
         live INSIDE it, so a decode entry point that would need a larger allocation than the one the prologue ran in raises instead
         of silently reallocating (and then decoding from uninitialised memory): size it up front with prologue(..., beam=, nbox=).
         V: the layout of a video-indexed batch of V videos (0: per clip); None: the layout of the live prologue's batch.
-        att2 (beam > 1): also the logit history of beam_decode_att2."""
+        att2 (beam > 1): also the logit history of beam_decode_att2.  rows (> 1): decode_sample_n with that many sampled rows per clip."""
         self._check_device()
         key = (B, T, self.device)
         ws = self._ws.get(key)
@@ -344,14 +349,17 @@ class NativeModel:
                 need = max(need, int(self._L.gvd_workspace_bytes_teacher(self._h, B, T, nbox)))
         if att2 and beam > 1:
             need = max(need, int(self._L.gvd_workspace_bytes_beam_att2(self._h, B, V, T, beam)))
+        if rows > 1:
+            need = max(need, int(self._L.gvd_workspace_bytes_sample_n(self._h, B, V, T, rows)))
         # the prologue lays the workspace out for one decode row per clip, and a beam layout can be the smaller one (B * beam > 128 rows
         # have no split-K slots)
         need = max(need, int(self._L.gvd_workspace_bytes_video(self._h, B, V, T, 1, 0)) if V else int(self._L.gvd_workspace_bytes(self._h, B, T)))
         if ws is not None and ws.numel() < need:
-            if self._live is not None and self._live[:2] == (B, T) and (beam > 1 or nbox > 0):
+            if self._live is not None and self._live[:2] == (B, T) and (beam > 1 or nbox > 0 or rows > 1):
                 raise GvdError("the workspace holding this batch's prologue outputs (sized for beam=%d, nbox=%d) is too small for the requested "
-                               "decode (beam=%d, nbox=%d%s): call prologue(..., beam=%d, nbox=%d%s) first" %
-                               (self._live[2], self._live[3], beam, nbox, ", att2" if att2 else "", beam, nbox, ", att2=True" if att2 else ""))
+                               "decode (beam=%d, nbox=%d%s%s): call prologue(..., beam=%d, nbox=%d%s%s) first" %
+                               (self._live[2], self._live[3], beam, nbox, ", att2" if att2 else "", ", rows=%d" % rows if rows > 1 else "", beam,
+                                nbox, ", att2=True" if att2 else "", ", rows=%d" % rows if rows > 1 else ""))
             ws = None                              # a larger layout was requested before any prologue ran in it: reallocate
         if ws is None:
             self._live, self._live_V = None, 0
@@ -375,16 +383,17 @@ class NativeModel:
         return ws[off:off + 4 * n].view(torch.float32).view(*shape)
 
     # ---- hot path
-    def prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, want_sim=True, beam=1, nbox=0, video_idx=None, att2=False):
+    def prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, want_sim=True, beam=1, nbox=0, video_idx=None, att2=False,
+                 rows=1):
         """video_idx (int64 [B], CUDA): a video-indexed batch.  segs_feat then holds the frame features of V videos [V,T,F] and clip b is
         event b of video video_idx[b] with its window sample_idx[b]; every result equals the per-clip prologue on segs_feat[video_idx].
-        att2: size the workspace for beam_decode_att2 as well."""
+        att2: size the workspace for beam_decode_att2 as well; rows: for decode_sample_n with that many captions per clip."""
         self._check_device(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, video_idx)
         T = segs_feat.shape[1]
         B = check_video_batch(segs_feat, video_idx, ppls, num, ppls_feat, sample_idx, pnt_mask) if video_idx is not None else segs_feat.shape[0]
         V = segs_feat.shape[0] if video_idx is not None else 0
         self._live, self._live_V = None, 0
-        ws = self.workspace(B, T, beam, nbox, V, att2)
+        ws = self.workspace(B, T, beam, nbox, V, att2, rows)
         sim = torch.empty(B, self.dims.detect_size + 1, self.R, dtype=torch.float32, device="cuda") if want_sim else None
         common = (_dev(ppls, torch.float32, "ppls"), _dev(num, torch.int64, "num"), _dev(ppls_feat, torch.float32, "ppls_feat"),
                   _dev(sample_idx, torch.int64, "sample_idx"))
@@ -420,6 +429,21 @@ class NativeModel:
         check(self._L.gvd_decode_sample(self._h, B, T, ctypes.c_void_p(ws.data_ptr()), ws.numel(), _dev(pnt_mask, torch.uint8, "pnt_mask"),
                                         int(seed) & 0xFFFFFFFFFFFFFFFF, float(temperature), ctypes.c_void_p(seq.data_ptr()),
                                         ctypes.c_void_p(logp.data_ptr()), ctypes.c_void_p(att2.data_ptr()), _stream()))
+        return seq, logp, att2
+
+    def decode_sample_n(self, B, T, n, pnt_mask, seed, temperature=1.0):
+        """n multinomial captions per clip from one prologue (gvd_decode_sample_n): seq [B*n,L], logp [B*n,L], att2 [B*n,L,R], caption j of
+        clip b in row b*n + j; equal to decode_sample on the batch repeated with repeat_interleave(n).  The prologue must have run with rows=n
+        (n > 1); pnt_mask [B,R+1] per clip."""
+        n = int(n)
+        ws = self.workspace(B, T, rows=n)
+        L = self.dims.seq_length
+        seq = torch.empty(B * n, L, dtype=torch.int64, device="cuda")
+        logp = torch.empty(B * n, L, dtype=torch.float32, device="cuda")
+        att2 = torch.empty(B * n, L, self.R, dtype=torch.float32, device="cuda")
+        check(self._L.gvd_decode_sample_n(self._h, B, T, n, ctypes.c_void_p(ws.data_ptr()), ws.numel(), _dev(pnt_mask, torch.uint8, "pnt_mask"),
+                                          int(seed) & 0xFFFFFFFFFFFFFFFF, float(temperature), ctypes.c_void_p(seq.data_ptr()),
+                                          ctypes.c_void_p(logp.data_ptr()), ctypes.c_void_p(att2.data_ptr()), _stream()))
         return seq, logp, att2
 
     def beam_decode(self, B, T, beam_size, pnt_mask):
@@ -783,7 +807,7 @@ def op_gru_layer(path, gi, Whh, bhh, sample_idx=None):
 
 def op_attention(p_pool, pool, p_conv, conv, w1, b1, w2, b2, att_mask, out_mask, z_out, partial, x_out, RC, TC, q=None, q_part=None,
                  q_bias=None, ticket=None, x_pk=None, feat_div=1, att_input_mode=None, gate_w=None, gate_b=None, gate_h=None,
-                 region_attn_mode=None, _video=None):
+                 region_attn_mode=None, _video=None, path=None):
     """The decode attention of B query rows through gvd_op_attention.  Features [B / feat_div, N, A | H]; q [B, 2A] or its split-K planes
     q_part [q_S, B, 2A] + q_bias [2A]; att_mask [B / feat_div, R+1]; out_mask [B / feat_div, R+1] or a [B / feat_div, R+1] column window
     of a wider mask (its row pitch is passed); z_out [B, R] and x_out [B, H] (x_pk [B, rup32(H)] int32 words) may be column windows of
@@ -791,7 +815,8 @@ def op_attention(p_pool, pool, p_conv, conv, w1, b1, w2, b2, att_mask, out_mask,
     (None: gvd_op_attention, i.e. 'both'); with 'featmap' x_out = att and `pool` may be None.  'dual_region': q = [attention2_dual query |
     attention2 query], w1 / b1 the dual alpha_net, p_conv / conv may be None, partial [B, 2 nch_r, H+4], the gate gate_w [H], gate_b [1] over
     the rows of gate_h [B, H] (dense rows, any pitch).  region_attn_mode 'mix' / 'mix_mul' / 'dp' (None: 'mix' through gvd_op_attention(_mode));
-    in 'dp' the region alpha_net (w2 / b2, and w1 / b1 in 'dual_region') may be None."""
+    in 'dp' the region alpha_net (w2 / b2, and w1 / b1 in 'dual_region') may be None.  path 0 / 1: the per-row or the row-grouped kernel
+    through gvd_op_attention_path (None: the entry the other arguments select, which runs the per-row kernel)."""
     Bf, R, A = p_pool.shape
     T, H = (conv.shape[1], conv.shape[2]) if conv is not None else (1, x_out.shape[-1])
     B = (q if q is not None else q_part[0]).shape[0]
@@ -802,7 +827,14 @@ def op_attention(p_pool, pool, p_conv, conv, w1, b1, w2, b2, att_mask, out_mask,
             _dev(p_conv, torch.float32, "p_conv") if p_conv is not None else None, _dev(conv, torch.float32, "conv") if conv is not None else None, _ptr(q), _ptr(q_part), q_S, _ptr(q_bias), _ptr(w1), _ptr(b1),
             _ptr(w2), _ptr(b2), _ptr(att_mask), _ptr(out_mask), out_mask.stride(0), _ptr(z_out), _pitch(z_out), _ptr(partial), _ptr(ticket),
             _ptr(x_out), _pitch(x_out), _ptr(x_pk), _pitch(x_pk), B, R, T, A, H, int(RC), int(TC), int(feat_div))
-    if _video is not None:
+    if path is not None:
+        vid, win, cb = _video if _video is not None else (None, None, None)
+        check(lib().gvd_op_attention_path(*args, ATT_INPUT_MODES[att_input_mode or "both"], _ptr(gate_w), _ptr(gate_b), _ptr(gate_h),
+                                          _pitch(gate_h), REGION_ATTN_MODES[region_attn_mode or "mix"],
+                                          _dev(vid, torch.int64, "video_idx") if vid is not None else None,
+                                          _dev(win, torch.int64, "sample_idx") if win is not None else None,
+                                          _dev(cb, torch.float32, "ctx_bias") if cb is not None else None, int(path), _stream()))
+    elif _video is not None:
         vid, win, cb = _video
         check(lib().gvd_op_attention_video(*args, ATT_INPUT_MODES[att_input_mode or "both"], _ptr(gate_w), _ptr(gate_b), _ptr(gate_h),
                                            _pitch(gate_h), REGION_ATTN_MODES[region_attn_mode or "mix"], _dev(vid, torch.int64, "video_idx"),

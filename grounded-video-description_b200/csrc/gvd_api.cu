@@ -181,7 +181,7 @@ __global__ void bn_affine_kernel(const float* w, const float* b, const float* me
 
 // ------------------------------------------------------------------------------------ model
 struct Param { std::string key; size_t numel; size_t off; bool set; };
-struct LoopKey { int B, T, backend; void* ws; size_t ws_bytes; int V; };   // what a captured decode loop depends on
+struct LoopKey { int B, T, backend; void* ws; size_t ws_bytes; int V, div; };   // what a captured decode loop depends on
 // a workspace whose prologue ran on a video-indexed batch (gvd_prologue_fwd_video): the decode entries lay it out for V videos
 struct VideoWs { void* ws; int B, T, V; };
 
@@ -217,13 +217,17 @@ struct gvd_model {
     // cudaGraphLaunch (no per-launch host cost, back-to-back scheduling on the device)
     cudaStream_t capture_stream = nullptr;
     cudaGraphExec_t greedy_exec = nullptr;
-    LoopKey greedy_key{0, 0, 0, nullptr, 0, 0};
+    LoopKey greedy_key{0, 0, 0, nullptr, 0, 0, 0};
     long long greedy_nodes = 0;      // kernel launches inside one replay (counted while capturing)
     // the multinomial-sampling loop has a graph of its own (alternating greedy and sampling calls re-capture neither); its seed and
     // temperature are read from the workspace, so a new draw replays the same graph
     cudaGraphExec_t sample_exec = nullptr;
-    LoopKey sample_key{0, 0, 0, nullptr, 0, 0};
+    LoopKey sample_key{0, 0, 0, nullptr, 0, 0, 0};
     long long sample_nodes = 0;
+    // ... and the loop over n sampled rows per clip (gvd_decode_sample_n), one more graph keyed by (B, T, n)
+    cudaGraphExec_t sample_n_exec = nullptr;
+    LoopKey sample_n_key{0, 0, 0, nullptr, 0, 0, 0};
+    long long sample_n_nodes = 0;
     std::vector<VideoWs> video_ws;   // set by the video prologues, cleared by a per-clip prologue on the same workspace
 
     float* P(const std::string& k) const {
@@ -414,6 +418,7 @@ extern "C" GVD_API void gvd_model_destroy(gvd_model_t* m) {
     if (m->ev_join) cudaEventDestroy(m->ev_join);
     if (m->greedy_exec) cudaGraphExecDestroy(m->greedy_exec);
     if (m->sample_exec) cudaGraphExecDestroy(m->sample_exec);
+    if (m->sample_n_exec) cudaGraphExecDestroy(m->sample_n_exec);
     if (m->capture_stream) cudaStreamDestroy(m->capture_stream);
     delete m;
 }
@@ -596,6 +601,7 @@ struct WS {
     long long* tok_col;
     int RC, TC, nch_r, nch_t, clip_chunk, beam, nbox;
     int V;                             // > 0: video-indexed batch, the frame tensors hold V videos' rows (V = 0: one copy per clip)
+    bool rows_n;                       // gvd_decode_sample_n: `beam` sampled rows per clip, no beam bookkeeping, row-sized loop outputs
     long long* in_vid;                 // [B] video of each clip (V > 0); the windows stay in in_sidx
     size_t bytes;
 };
@@ -613,7 +619,11 @@ static void attn_chunking(int B, int R, int T, int* RC, int* TC) {
 
 // att2_hist (beam > 1): also the beam's logit history for gvd_beam_decode_att2, after every other slot so that the layout without it is
 // unchanged
-static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, int nbox = 0, int V = 0, bool att2_hist = false) {
+// rows_n (beam > 1): the layout of gvd_decode_sample_n, `beam` sampled rows per clip; the loop's workspace-resident outputs then have one row
+// per sampled caption and move to the end, so the prologue's slots stay where a per-clip layout has them (the per-clip out_seq / out_logp /
+// out_att2 slots stay allocated and unused in this layout)
+static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, int nbox = 0, int V = 0, bool att2_hist = false,
+                    bool rows_n = false) {
     const gvd_dims_t& d = m->d;
     const int H = d.rnn_size, A = d.att_hid_size, R = m->R, G = m->G;
     WS w{};
@@ -625,6 +635,7 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
     const size_t BD = (size_t)B * beam;       // decode rows (beam rows of one clip share its features)
     w.beam = beam;
     w.V = V;
+    w.rows_n = rows_n && beam > 1;
     attn_chunking((int)BD, R, T, &w.RC, &w.TC);
     gvd_attn_chunks(R, T, w.RC, w.TC, &w.nch_r, &w.nch_t);
     w.clip_chunk = std::max(1, std::min(B, (int)(100000000ll / ((long long)m->nheads * R * R * 4 + 1))));   // S chunk ~<= 100 MB (L2)
@@ -713,7 +724,7 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
         w.vt_rec = (float*)take(gvd_vocab_rec_floats((int)BD, d.vocab_size) * 4);
         w.vt_ticket = (int*)take(BD * 4);
     }
-    if (beam > 1) {
+    if (beam > 1 && !w.rows_n) {
         const size_t L = d.seq_length, K = beam;
         w.bb.seq = (int*)take((size_t)B * L * K * 4);
         w.bb.att = (int*)take((size_t)B * L * K * 4);
@@ -750,7 +761,12 @@ static WS ws_layout(const gvd_model* m, int B, int T, void* base, int beam = 1, 
         w.part_cnt = (int*)take(std::max((size_t)B * L, (size_t)B * NB) * 4);
         w.tok_col = (long long*)take((size_t)B * 8);
     }
-    if (beam > 1 && att2_hist) {
+    if (w.rows_n) {
+        w.out_seq = (long long*)take(BD * d.seq_length * 8);
+        w.out_logp = (float*)take(BD * d.seq_length * 4);
+        w.out_att2 = (float*)take(BD * d.seq_length * R * 4);
+    }
+    if (beam > 1 && att2_hist && !w.rows_n) {
         const size_t L = d.seq_length;
         w.att2_hist = (float*)take(L * BD * R * 4);       // step t's region-attention logits of every beam row, [L][B*K][R]
         w.bb.parent_hist = (int*)take(L * BD * 4);
@@ -776,6 +792,11 @@ extern "C" GVD_API size_t gvd_workspace_bytes_beam(const gvd_model_t* m, int B, 
 extern "C" GVD_API size_t gvd_workspace_bytes_beam_att2(const gvd_model_t* m, int B, int V, int T, int beam_size) {
     if (!m || B < 1 || V < 0 || T < 1 || beam_size < 2) return 0;
     return ws_layout(m, B, T, nullptr, beam_size, 0, V, true).bytes;
+}
+
+extern "C" GVD_API size_t gvd_workspace_bytes_sample_n(const gvd_model_t* m, int B, int V, int T, int n) {
+    if (!m || B < 1 || V < 0 || T < 1 || n < 1) return 0;
+    return ws_layout(m, B, T, nullptr, n, 0, V, false, true).bytes;
 }
 
 extern "C" GVD_API size_t gvd_workspace_bytes_video(const gvd_model_t* m, int B, int V, int T, int beam_size, int nbox) {
@@ -824,11 +845,11 @@ static int require_topdown(const gvd_model* m, const char* who) {
 }
 
 static int check_ws(const gvd_model* m, int B, int T, void* workspace, size_t bytes, WS* w, int beam = 1, int nbox = 0, int V = -1,
-                    bool att2_hist = false) {
+                    bool att2_hist = false, bool rows_n = false) {
     GVD_REQUIRE(m && m->finalized, "model not finalized (call gvd_model_finalize after setting every parameter)");
     GVD_REQUIRE(B >= 1 && T >= 1, "bad batch/frames B=%d T=%d", B, T);
     GVD_REQUIRE(workspace && ((uintptr_t)workspace & 255) == 0, "workspace must be a 256-byte aligned device pointer");
-    *w = ws_layout(m, B, T, workspace, beam, nbox, V < 0 ? video_of(m, workspace, B, T) : V, att2_hist);
+    *w = ws_layout(m, B, T, workspace, beam, nbox, V < 0 ? video_of(m, workspace, B, T) : V, att2_hist, rows_n);
     GVD_REQUIRE(bytes >= w->bytes, "workspace too small: %zu < %zu bytes", bytes, w->bytes);
     return 0;
 }
@@ -1158,11 +1179,8 @@ extern "C" GVD_API int gvd_prologue_fwd_video(gvd_model_t* m, int B, int V, int 
 }
 
 // ------------------------------------------------------------------------------------ decode
-extern "C" GVD_API int gvd_decode_reset_state(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes, void* stream) {
-    GVD_TRY(require_topdown(m, "decode_reset_state"));
-    WS w;
-    GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
-    cudaStream_t st = (cudaStream_t)stream;
+// zero recurrent state and tickets of the layout's B * beam decode rows
+static int reset_state(const gvd_model* m, const WS& w, int B, cudaStream_t st) {
     const size_t n = (size_t)B * w.beam * m->d.rnn_size * sizeof(float);
     GVD_CHECK_CUDA(cudaMemsetAsync(w.h_att, 0, 2 * n, st));     // init_hidden: zeros (model.py:237-240)
     GVD_CHECK_CUDA(cudaMemsetAsync(w.c_att, 0, n, st));
@@ -1180,12 +1198,19 @@ extern "C" GVD_API int gvd_decode_reset_state(gvd_model_t* m, int B, int T, void
     return 0;
 }
 
+extern "C" GVD_API int gvd_decode_reset_state(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes, void* stream) {
+    GVD_TRY(require_topdown(m, "decode_reset_state"));
+    WS w;
+    GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w));
+    return reset_state(m, w, B, (cudaStream_t)stream);
+}
+
 // does the core step run its three products operand-swapped + split along K (gvd_skinny.cu)?  Then xt / h_att / h_lang live inside the
 // concatenated LSTM inputs xcat_att = [xt | h_att] and xcat_lang = [att + att2 | h_att | h_lang].
 static bool core_skinny(const gvd_model* m, const WS& w, int B, int div) {
     const gvd_dims_t& d = m->d;
     const int H = d.rnn_size, A = d.att_hid_size, E = d.input_encoding_size;
-    return gvd_backend_on(BK_TC | BK_SPLITK) && H % 8 == 0 && div == 1 && w.sk_part != nullptr && E % 4 == 0 &&
+    return gvd_backend_on(BK_TC | BK_SPLITK) && H % 8 == 0 && (div == 1 || w.rows_n) && w.sk_part != nullptr && E % 4 == 0 &&
            gvd_skinny_splits(4 * H, E + H, B) > 0 && gvd_skinny_splits(2 * A, H, B) > 0 && gvd_skinny_splits(4 * H, 3 * H, B) > 0;
 }
 
@@ -1196,7 +1221,8 @@ static bool core_skinny_f16(const gvd_model* m) {
     return gvd_backend_on(BK_F16X3) && d.rnn_size % 32 == 0 && d.input_encoding_size % 32 == 0 && d.att_hid_size % 16 == 0;
 }
 
-// B = decode rows (clips x beam); rows [k*div, (k+1)*div) attend over clip k's features / masks
+// B = decode rows (clips x beam or sampled rows); rows [k*div, (k+1)*div) attend over clip k's features / masks.  The split-K products take
+// any div in the sampled-rows layout (no beam reorder of the recurrent rows, which would have to reach into the concatenated inputs)
 static int core_step(const gvd_model* m, const WS& w, int B, int T, int step, const long long* tokens, const unsigned char* att_mask,
                      const unsigned char* out_mask, float* z_out, long long z_stride_b, cudaStream_t st, int div = 1, long long out_mask_stride = 0,
                      bool xt_ready = false) {
@@ -1331,13 +1357,15 @@ extern "C" GVD_API int gvd_decode_step_fwd(gvd_model_t* m, int B, int T, void* w
 // S1: the 21-iteration decode loop (model.py:579-624) enqueued on `st`; every pointer is fixed for a given workspace, so the
 // whole enqueue is capturable as a CUDA graph.  sample == nullptr: greedy (top-2 + UNK rule, sample_max = 1); otherwise multinomial
 // sampling (sample_max = 0) with the seed and temperature the kernels read from the parameter block `sample`.
+// div > 1 (gvd_decode_sample_n): B = clips x div decode rows in the sampled-rows layout, rows [k*div, (k+1)*div) of clip k.
 static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void* workspace, size_t workspace_bytes, const uint8_t* pnt_mask,
                                  int64_t* seq_out, float* logprobs_out, float* att2_logits_out, cudaStream_t st,
-                                 const GvdSampleParams* sample = nullptr) {
+                                 const GvdSampleParams* sample = nullptr, int div = 1) {
     GvdF16Scope f16;
     const gvd_dims_t& d = m->d;
     const int H = d.rnn_size, V = d.vocab_size, L = d.seq_length, R = m->R;
-    GVD_TRY(gvd_decode_reset_state(m, B, T, workspace, workspace_bytes, (void*)st));
+    if (div > 1) GVD_TRY(reset_state(m, w, B / div, st));
+    else GVD_TRY(gvd_decode_reset_state(m, B, T, workspace, workspace_bytes, (void*)st));
     GVD_CHECK_CUDA(cudaMemsetAsync(w.it, 0, (size_t)B * sizeof(long long), st));            // <bos> = 0 (model.py:587-588)
     // The pick kernel also writes the next step's xt = ReLU(embed[token]) (no separate embedding launch).  Folding the whole
     // sampler into the vocabulary-head GEMM epilogue (MODE_PICK of wg_gemm_kernel, last-CTA merge of the per-CTA partials) is
@@ -1347,7 +1375,7 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
     static const bool fused_pick = getenv("GVD_FUSED_PICK") != nullptr;
     const bool fused = tc && fused_pick && B <= 128 && !sample;     // the fused head has no multinomial sampler: sampling takes the split-K path
     for (int t = 0; t < L; ++t) {
-        GVD_TRY(core_step(m, w, B, T, t, w.it, pnt_mask, pnt_mask, att2_logits_out + (size_t)t * R, (long long)L * R, st, 1, 0, tc && t > 0));
+        GVD_TRY(core_step(m, w, B, T, t, w.it, pnt_mask, pnt_mask, att2_logits_out + (size_t)t * R, (long long)L * R, st, div, 0, tc && t > 0));
         const float* h = w.h_lang + (size_t)((t + 1) & 1) * B * H;
         if (fused) {
             GVD_STAGE("decode.logit_pick", gvd_logit_pick_tc(h, H, m->P("logit.weight"), H, m->P("logit.bias"), B, V, H, d.unk_idx, w.pk_part,
@@ -1356,7 +1384,7 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
         } else {
             const int E = d.input_encoding_size;
             const int S = (tc && gvd_backend_on(BK_SPLITK) && w.sk_part) ? gvd_skinny_splits(V, H, B) : 0;
-            const bool sk_core = core_skinny(m, w, B, 1);                       // then xt goes into the core step's concatenated input
+            const bool sk_core = core_skinny(m, w, B, div);                     // then xt goes into the core step's concatenated input
             const bool sk16 = sk_core && core_skinny_f16(m);                    // ... and its fp16x3 image into xp_att
             // above 6144 words (reduce_pick / reduce_sample hold a row in one CTA's registers): the sliced tail, one CTA per (row, 1024 words)
             auto vocab_tail = [&](const float* part, int nplanes, const float* bias, float* xt, float* xt_pk) {
@@ -1411,22 +1439,23 @@ static int decode_greedy_enqueue(gvd_model_t* m, const WS& w, int B, int T, void
 // The decode loop through its captured graph: built on the first call for (B, T, backend, workspace) and replayed afterwards.
 static int decode_loop_run(gvd_model_t* m, const WS& w, int B, int T, void* workspace, size_t workspace_bytes, const uint8_t* pnt_mask,
                            int64_t* seq_out, float* logprobs_out, float* att2_logits_out, cudaStream_t st, const GvdSampleParams* sample,
-                           cudaGraphExec_t& exec, LoopKey& key, long long& nodes) {
+                           cudaGraphExec_t& exec, LoopKey& key, long long& nodes, int div = 1) {
     const int L = m->d.seq_length, R = m->R;
     // Direct enqueue when the stage profiler is on (its events cannot be captured) or when asked (GVD_NO_GRAPH: per-kernel profiling)
     static const bool no_graph = getenv("GVD_NO_GRAPH") != nullptr;
     if (no_graph || g_prof_on.load(std::memory_order_relaxed) != 0)
-        return decode_greedy_enqueue(m, w, B, T, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_logits_out, st, sample);
+        return decode_greedy_enqueue(m, w, B, T, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_logits_out, st, sample, div);
     // Graph path: the loop reads the mask from / writes its results to workspace-resident buffers (fixed addresses), the caller's
     // tensors are copied in / out around the replay.
-    if (!exec || key.B != B || key.T != T || key.backend != gvd_backend() || key.ws != workspace || key.ws_bytes != workspace_bytes || key.V != w.V) {
+    if (!exec || key.B != B || key.T != T || key.backend != gvd_backend() || key.ws != workspace || key.ws_bytes != workspace_bytes || key.V != w.V ||
+        key.div != div) {
         if (exec) { cudaGraphExecDestroy(exec); exec = nullptr; }
         if (!m->capture_stream) GVD_CHECK_CUDA(cudaStreamCreateWithFlags(&m->capture_stream, cudaStreamNonBlocking));
         cudaGraph_t graph = nullptr;
         GVD_CHECK_CUDA(cudaStreamBeginCapture(m->capture_stream, cudaStreamCaptureModeThreadLocal));
         const long long l0 = g_launches.load();
         const int rc = decode_greedy_enqueue(m, w, B, T, workspace, workspace_bytes, w.in_mask, (int64_t*)w.out_seq, w.out_logp, w.out_att2,
-                                             m->capture_stream, sample);
+                                             m->capture_stream, sample, div);
         const cudaError_t ce = cudaStreamEndCapture(m->capture_stream, &graph);
         nodes = g_launches.load() - l0;
         g_launches.store(l0);                              // capturing launches nothing
@@ -1435,9 +1464,9 @@ static int decode_loop_run(gvd_model_t* m, const WS& w, int B, int T, void* work
         const cudaError_t ie = cudaGraphInstantiate(&exec, graph, 0);
         cudaGraphDestroy(graph);
         GVD_CHECK_CUDA(ie);
-        key = {B, T, gvd_backend(), workspace, workspace_bytes, w.V};
+        key = {B, T, gvd_backend(), workspace, workspace_bytes, w.V, div};
     }
-    if (pnt_mask != w.in_mask) GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_mask, pnt_mask, (size_t)B * (R + 1), cudaMemcpyDeviceToDevice, st));
+    if (pnt_mask != w.in_mask) GVD_CHECK_CUDA(cudaMemcpyAsync(w.in_mask, pnt_mask, (size_t)(B / div) * (R + 1), cudaMemcpyDeviceToDevice, st));
     GVD_CHECK_CUDA(cudaGraphLaunch(exec, st));
     g_launches.fetch_add(nodes, std::memory_order_relaxed);
     if (seq_out != (int64_t*)w.out_seq) GVD_CHECK_CUDA(cudaMemcpyAsync(seq_out, w.out_seq, (size_t)B * L * 8, cudaMemcpyDeviceToDevice, st));
@@ -1469,6 +1498,25 @@ extern "C" GVD_API int gvd_decode_sample(gvd_model_t* m, int B, int T, void* wor
     GVD_CHECK_CUDA(cudaMemcpyAsync(w.sample_par, &par, sizeof(par), cudaMemcpyHostToDevice, st));
     return decode_loop_run(m, w, B, T, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_logits_out, st, w.sample_par,
                            m->sample_exec, m->sample_key, m->sample_nodes);
+}
+
+extern "C" GVD_API int gvd_decode_sample_n(gvd_model_t* m, int B, int T, int n, void* workspace, size_t workspace_bytes, const uint8_t* pnt_mask,
+                                           uint64_t seed, float temperature, int64_t* seq_out, float* logprobs_out, float* att2_logits_out,
+                                           void* stream) {
+    GVD_REQUIRE(n >= 1, "decode_sample_n: n must be >= 1 (got %d)", n);
+    if (n == 1)
+        return gvd_decode_sample(m, B, T, workspace, workspace_bytes, pnt_mask, seed, temperature, seq_out, logprobs_out, att2_logits_out, stream);
+    GVD_TRY(require_topdown(m, "decode_sample_n"));
+    GVD_REQUIRE(B <= INT_MAX / n, "decode_sample_n: B * n overflows");
+    WS w;
+    GVD_TRY(check_ws(m, B, T, workspace, workspace_bytes, &w, n, 0, -1, false, true));
+    GVD_REQUIRE(pnt_mask && seq_out && att2_logits_out, "decode_sample_n: null argument");
+    GVD_REQUIRE(std::isfinite(temperature) && temperature > 0.f, "decode_sample_n: temperature must be finite and > 0 (got %g)", (double)temperature);
+    cudaStream_t st = (cudaStream_t)stream;
+    const GvdSampleParams par{(uint32_t)(seed & 0xffffffffull), (uint32_t)(seed >> 32), temperature, 0u};
+    GVD_CHECK_CUDA(cudaMemcpyAsync(w.sample_par, &par, sizeof(par), cudaMemcpyHostToDevice, st));
+    return decode_loop_run(m, w, B * n, T, workspace, workspace_bytes, pnt_mask, seq_out, logprobs_out, att2_logits_out, st, w.sample_par,
+                           m->sample_n_exec, m->sample_n_key, m->sample_n_nodes, n);
 }
 
 namespace {
@@ -2017,7 +2065,7 @@ static int op_attention(const float* p_pool, const float* pool, const float* p_c
                         int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
                         int B, int R, int T, int A, int H, int RC, int TC, int feat_div, int att_input_mode,
                         const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld, int region_attn_mode,
-                        const int64_t* video_idx, const int64_t* sample_idx, const float* ctx_bias, void* stream) {
+                        const int64_t* video_idx, const int64_t* sample_idx, const float* ctx_bias, void* stream, int path = 0) {
     GVD_REQUIRE(att_input_mode == GVD_ATT_INPUT_BOTH || att_input_mode == GVD_ATT_INPUT_FEATMAP || att_input_mode == GVD_ATT_INPUT_DUAL_REGION,
                 "op_attention: unknown att_input_mode %d", att_input_mode);
     GVD_REQUIRE(region_attn_mode == GVD_REGION_ATTN_MIX || region_attn_mode == GVD_REGION_ATTN_MIX_MUL || region_attn_mode == GVD_REGION_ATTN_DP,
@@ -2042,7 +2090,7 @@ static int op_attention(const float* p_pool, const float* pool, const float* p_c
     if (dp) { a.w2 = a.b2 = nullptr; if (dual) a.w1 = a.b1 = nullptr; }          // the kernel must not need them
     a.vid = (const long long*)video_idx; a.win = (const long long*)sample_idx; a.ctx_bias = ctx_bias;
     cudaStream_t st = (cudaStream_t)stream;
-    GVD_TRY(gvd_attn_partial(a, st));
+    GVD_TRY(gvd_attn_partial_path(a, path, st));
     if (ticket) return 0;
     int nch_r, nch_t;
     gvd_attn_chunks(R, T, RC, TC, &nch_r, &nch_t);
@@ -2070,6 +2118,22 @@ extern "C" GVD_API int gvd_op_attention_video(const float* p_pool, const float* 
     return op_attention(p_pool, pool, p_conv, conv, q, q_part, q_S, q_bias, w1, b1, w2, b2, att_mask, out_mask, out_mask_stride, z_out,
                         z_stride_b, partial, ticket, x_out, x_ld, x_pk, x_pk_ld, B, R, T, A, H, RC, TC, feat_div, att_input_mode, gate_w,
                         gate_b, gate_h, gate_ld, region_attn_mode, video_idx, sample_idx, ctx_bias, stream);
+}
+// gvd_op_attention_video's arguments (video_idx / sample_idx / ctx_bias may be NULL: per-clip features) and the kernel: path 0 =
+// attn_partial_kernel (one CTA per row, what the decode runs), 1 = attn_group_kernel (one CTA per group of a clip's rows).  Test and
+// measurement hook.
+extern "C" GVD_API int gvd_op_attention_path(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                                             const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,
+                                             const float* b2, const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out,
+                                             int64_t z_stride_b, float* partial, int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld,
+                                             int B, int R, int T, int A, int H, int RC, int TC, int feat_div, int att_input_mode,
+                                             const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld, int region_attn_mode,
+                                             const int64_t* video_idx, const int64_t* sample_idx, const float* ctx_bias, int path, void* stream) {
+    GVD_REQUIRE(path == 0 || path == 1, "op_attention_path: path must be 0 (per row) or 1 (row groups), got %d", path);
+    GVD_REQUIRE(!video_idx || (sample_idx && ctx_bias), "op_attention_path: video rows need sample_idx and ctx_bias");
+    return op_attention(p_pool, pool, p_conv, conv, q, q_part, q_S, q_bias, w1, b1, w2, b2, att_mask, out_mask, out_mask_stride, z_out,
+                        z_stride_b, partial, ticket, x_out, x_ld, x_pk, x_pk_ld, B, R, T, A, H, RC, TC, feat_div, att_input_mode, gate_w,
+                        gate_b, gate_h, gate_ld, region_attn_mode, video_idx, sample_idx, ctx_bias, stream, path);
 }
 extern "C" GVD_API int gvd_op_attention_mode(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
                                              const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2,

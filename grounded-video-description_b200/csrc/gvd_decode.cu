@@ -21,6 +21,10 @@
 //                          temporal chunks are additive in every mode.
 //                          Video-indexed batches (AttnArgs::vid): a clip's temporal chunks stream only its window's rows of
 //                          the video's unmasked features; the first one adds the closed-form out-of-window softmax term.
+//   attn_group_kernel    : the same attention for up to 8 rows that share a clip's features (sampled captions, beam rows) per CTA: each
+//                          chunk is streamed once and scored against every query of the group.  Bit-identical to attn_partial_kernel
+//                          per row; measured slower than it on shared features (L2 serves the per-row kernel's repeated reads), so the
+//                          decode does not select it (gvd_attn_partial_path, DESIGN §3).
 //   attn_combine_kernel  : merges the chunk partials (flash-decoding style) into att + att2.
 //   greedy_pick_kernel   : log_softmax + top-2 + UNK rule (misc/model.py:590-594,615).
 #include "../../include/gvd_b200.h"
@@ -604,6 +608,384 @@ __global__ void __launch_bounds__(ATT_THREADS, FORM == GVD_REGION_ATTN_MIX ? 0 :
     if (tid == 0) a.ticket[b] = 0;                       // ready for the next step
 }
 
+// =====================================================================================
+// row-grouped attention partials: up to ATT_GMAX rows that attend over one clip's features (sampled captions, beam rows) per CTA
+// =====================================================================================
+// ATT_GMAX = ATT_CWARPS: one softmax warp per row of the group, and at A = 512 the group's queries (G * A floats, twice in dual_region) and
+// score vectors still fit next to the 96 KB ring in one CTA's shared memory (up to ~150 KB); phase B keeps G (dual: 2 G) float4 accumulators
+// per thread in registers.  The decode does not select this kernel (gvd_attn_partial, DESIGN §3: slower than the per-row kernel on the same
+// shared features at the measured rows per clip); gvd_op_attention_path runs it.
+constexpr int ATT_GMAX = ATT_CWARPS;
+
+// att_row_sum with the query in shared memory (the row group's queries do not fit in registers).  The same terms in the same order as
+// att_row_sum on register queries: AJ > 0 takes the projected row from v4 (registers, loaded once for every query of the group).
+template <int AJ, int F>
+__device__ __forceinline__ float att_row_sum_sq(const float4* v4, const float* pr, const float* qg, const float4* w4, const float* ws, int A,
+                                                int lane) {
+    float sum = 0.f;
+    if (AJ > 0) {
+#pragma unroll
+        for (int j = 0; j < AJ; ++j) {
+            const float4 qv = *reinterpret_cast<const float4*>(qg + lane * 4 + 128 * j);
+            sum = att_term<F>(w4[j].x, v4[j].x, qv.x, sum);
+            sum = att_term<F>(w4[j].y, v4[j].y, qv.y, sum);
+            sum = att_term<F>(w4[j].z, v4[j].z, qv.z, sum);
+            sum = att_term<F>(w4[j].w, v4[j].w, qv.w, sum);
+        }
+    } else {
+        for (int a0 = lane * 4; a0 < A; a0 += 128) {
+            const float4 v = *reinterpret_cast<const float4*>(pr + a0);
+            const float4 qv = *reinterpret_cast<const float4*>(qg + a0);
+            const float4 wv = F == GVD_REGION_ATTN_DP ? make_float4(0.f, 0.f, 0.f, 0.f) : *reinterpret_cast<const float4*>(ws + a0);
+            sum = att_term<F>(wv.x, v.x, qv.x, sum);
+            sum = att_term<F>(wv.y, v.y, qv.y, sum);
+            sum = att_term<F>(wv.z, v.z, qv.z, sum);
+            sum = att_term<F>(wv.w, v.w, qv.w, sum);
+        }
+    }
+    return sum;
+}
+
+// sum_c acc_c e^{m_c - M} / sum_c l_c e^{m_c - M} over the chunk records [c0, c1) of one row: attn_partial_kernel's merge, chunk for chunk
+__device__ __forceinline__ float4 merge_part(const float* base, int c0, int c1, int H, int h0) {
+    float M = -INFINITY;
+    for (int cc = c0; cc < c1; ++cc) M = fmaxf(M, __ldcg(base + (long long)cc * (H + 4)));
+    float L = 0.f;
+    float4 s4 = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int cc = c0; cc < c1; ++cc) {
+        const float* pc = base + (long long)cc * (H + 4);
+        const float sc = expf(__ldcg(pc) - M);
+        L = fmaf(__ldcg(pc + 1), sc, L);
+        const float4 v = __ldcg(reinterpret_cast<const float4*>(pc + 4 + h0));
+        s4.x = fmaf(v.x, sc, s4.x); s4.y = fmaf(v.y, sc, s4.y); s4.z = fmaf(v.z, sc, s4.z); s4.w = fmaf(v.w, sc, s4.w);
+    }
+    return make_float4(s4.x / L, s4.y / L, s4.z / L, s4.w / L);
+}
+
+__device__ __forceinline__ void store_x(const AttnArgs& a, int b, int h0, float4 res) {
+    *reinterpret_cast<float4*>(a.x_out + (long long)b * (a.x_ld ? a.x_ld : a.H) + h0) = res;
+    if (a.x_pk) {
+        uint32_t hi0, lo0, hi1, lo1;
+        f16x3_split_pair(res.x, res.y, GVD_F16_SA, hi0, lo0);
+        f16x3_split_pair(res.z, res.w, GVD_F16_SA, hi1, lo1);
+        uint32_t* d = reinterpret_cast<uint32_t*>(a.x_pk) + (long long)b * a.x_pk_ld + f16x3_word(h0);
+        *reinterpret_cast<uint2*>(d) = make_uint2(hi0, hi1);
+        *reinterpret_cast<uint2*>(d + 16) = make_uint2(lo0, lo1);
+    }
+}
+
+// Every row of the group equals attn_partial_kernel's result for that row bit for bit: the same chunks, the same lane -> element mapping of
+// the scores (att_row_sum_sq), the same warp_sum trees, the same per-row softmax and weighted-sum order, the same merge.  Grid: (clip, row
+// group, chunk); the group's rows b0 .. b0 + G - 1 share the clip's features, masks and (video rows) window, so each chunk's projected and
+// feature rows are streamed once for all G queries.  The group's last chunk CTA (ticket of row b0) merges all its rows.
+template <int AJ, int FORM>
+__global__ void __launch_bounds__(ATT_THREADS, 1) attn_group_kernel(AttnArgs a, int nch_r, int nch_t, int ngroups) {
+    extern __shared__ __align__(128) unsigned char smem[];
+    const bool featmap = a.mode == GVD_ATT_INPUT_FEATMAP, dual = a.mode == GVD_ATT_INPUT_DUAL_REGION;
+    const int nq = dual ? 2 : 1;                                // score vectors per row
+    const int A = a.A, H = a.H;
+    float* z_s = reinterpret_cast<float*>(smem + ATT_NST * ATT_STAGE_BYTES);   // [nq][GMAX][MAXC] (dual: attention2, then attention2_dual)
+    float* e_s = z_s + nq * ATT_GMAX * ATT_MAXC;                               // [nq][GMAX][MAXC]
+    float* ml = e_s + nq * ATT_GMAX * ATT_MAXC;                                // [nq][GMAX][2] + merge flag
+    float* red = ml + 2 * nq * ATT_GMAX + 4;                                   // [GMAX][CWARPS] gate partial sums
+    uint64_t* full = reinterpret_cast<uint64_t*>(red + ATT_GMAX * ATT_CWARPS);
+    uint64_t* empty = full + ATT_NST;
+    float* qs = reinterpret_cast<float*>(empty + ATT_NST);     // [nq][GMAX][A] (dual: attention2 queries, then the dual ones)
+    float* ws = qs + nq * ATT_GMAX * A;                         // [nq][A]
+
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int nch = nch_r + nch_t;
+    const int c = blockIdx.x % nch, grp = (blockIdx.x / nch) % ngroups, fb = blockIdx.x / nch / ngroups;
+    const int div = a.feat_div > 1 ? a.feat_div : 1;
+    const int g0 = grp * ATT_GMAX, G = min(ATT_GMAX, div - g0), b0 = fb * div + g0;
+    const bool region = c < nch_r;
+    const int N = region ? a.R : a.T;
+    const int chunk = region ? a.RC : a.TC;
+    int r0 = region ? c * chunk : (c - nch_r) * chunk;
+    int nrows = min(chunk, N - r0);
+    long long frow = fb;
+    int n_out = 0;
+    if (a.vid && !region) {
+        const long long lo = max(a.win[2 * fb], 0ll), hi = min(a.win[2 * fb + 1], (long long)N);
+        const int wlo = (int)min(lo, (long long)N), whi = (int)max(hi, (long long)wlo);
+        const int c0 = max(r0, wlo), c1 = min(r0 + nrows, whi);
+        frow = a.vid[fb];
+        if (c == nch_r) n_out = N - (whi - wlo);
+        r0 = c0;
+        nrows = max(c1 - c0, 0);
+    }
+    const float* p_rows = (region ? a.p_pool : a.p_conv) + (frow * N + r0) * A;
+    const float* f_rows = (region ? a.pool : a.conv) + (frow * N + r0) * H;
+    const int rows_pa = ATT_STAGE_BYTES / (A * 4), rows_pb = ATT_STAGE_BYTES / (H * 4);
+    const int n_pa = (nrows + rows_pa - 1) / rows_pa, n_pb = (featmap && region) ? 0 : (nrows + rows_pb - 1) / rows_pb;
+
+    if (tid == 0) {
+        for (int s = 0; s < ATT_NST; ++s) {
+            mbar_init(&full[s], 1);
+            mbar_init(&empty[s], ATT_CWARPS);
+        }
+        mbar_fence_init();
+    }
+    __syncthreads();
+
+    if (tid == 0) pdl_trigger();
+    if (warp == ATT_CWARPS) {
+        if (lane == 0) {
+            for (int i = 0; i < n_pa + n_pb; ++i) {
+                const int s = i % ATT_NST;
+                const uint32_t ph = (uint32_t)(i / ATT_NST) & 1u;
+                mbar_wait(&empty[s], ph ^ 1u);
+                const float* src;
+                uint32_t bytes;
+                if (i < n_pa) {
+                    const int row0 = i * rows_pa, nr = min(rows_pa, nrows - row0);
+                    src = p_rows + (long long)row0 * A;
+                    bytes = (uint32_t)nr * A * 4u;
+                } else {
+                    const int row0 = (i - n_pa) * rows_pb, nr = min(rows_pb, nrows - row0);
+                    src = f_rows + (long long)row0 * H;
+                    bytes = (uint32_t)nr * H * 4u;
+                }
+                mbar_expect_tx(&full[s], bytes);
+                bulk_g2s(smem + (size_t)s * ATT_STAGE_BYTES, src, bytes, &full[s]);
+            }
+        }
+        return;
+    }
+
+    // ---------------------------------------------------------------- consumers
+    pdl_wait();
+    // the group's queries: row b's slice q[b, off .. off + A) (or its split-K partials summed onto the bias in plane order); dual_region
+    // keeps attention2's query (second half) in slot 0 and the dual query (first half) in slot 1
+    for (int qi = 0; qi < nq; ++qi) {
+        const int off = dual ? (qi == 0 ? A : 0) : (region ? A : 0);
+        for (int i = tid; i < G * A; i += ATT_CWARPS * 32) {
+            const int g = i / A, k = i - g * A;
+            const long long at = (long long)(b0 + g) * 2 * A + off + k;
+            float v;
+            if (a.q) {
+                v = a.q[at];
+            } else {
+                v = __ldg(a.q_bias + off + k);
+                for (int s = 0; s < a.q_S; ++s) v += __ldcg(a.q_part + s * a.q_plane + at);
+            }
+            qs[(qi * ATT_GMAX + g) * A + k] = v;
+        }
+    }
+    const bool has_w = !(FORM == GVD_REGION_ATTN_DP && (region || dual));
+    const float* w = dual ? a.w2 : (region ? a.w2 : a.w1);
+    const float bias = has_w ? __ldg(dual ? a.b2 : (region ? a.b2 : a.b1)) : 0.f;
+    const float bias_d = dual && has_w ? __ldg(a.b1) : 0.f;
+    if (has_w) {
+        for (int i = tid; i < A; i += ATT_CWARPS * 32) ws[i] = w[i];
+        if (dual) for (int i = tid; i < A; i += ATT_CWARPS * 32) ws[A + i] = a.w1[i];
+    }
+    float4 w4[AJ > 0 ? AJ : 1];
+    if (AJ > 0 && !dual) {
+#pragma unroll
+        for (int j = 0; j < AJ; ++j) w4[j] = has_w ? __ldg(reinterpret_cast<const float4*>(w + lane * 4 + 128 * j)) : make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+    consumer_bar();
+
+    // phase A: the scores of every streamed row against each of the group's queries
+    auto phase_a = [&](auto form) {
+        constexpr int F = decltype(form)::value;
+        for (int i = 0; i < n_pa; ++i) {
+            const int s = i % ATT_NST;
+            const uint32_t ph = (uint32_t)(i / ATT_NST) & 1u;
+            mbar_wait(&full[s], ph);
+            const float* st = reinterpret_cast<const float*>(smem + (size_t)s * ATT_STAGE_BYTES);
+            const int row0 = i * rows_pa, nr = min(rows_pa, nrows - row0);
+            for (int rr = warp; rr < nr; rr += ATT_CWARPS) {
+                const float* pr = st + (long long)rr * A;
+                const int rl = row0 + rr;
+                bool am = false, om = false;
+                if (region && lane == 0) {
+                    const long long mi = (long long)fb * (a.R + 1) + 1 + r0 + rl;
+                    const long long oi = a.out_mask_stride ? (long long)fb * a.out_mask_stride + 1 + r0 + rl : mi;
+                    am = a.att_mask[mi] != 0;
+                    om = a.out_mask[oi] != 0;
+                }
+                if (dual) {
+                    // attn_dual_consumer's generic loop: both scores from one read of each element
+                    for (int g = 0; g < G; ++g) {
+                        const float* q2 = qs + g * A;
+                        const float* qd = qs + (ATT_GMAX + g) * A;
+                        float sum = 0.f, sum_d = 0.f;
+                        for (int a0 = lane * 4; a0 < A; a0 += 128) {
+                            const float4 v = *reinterpret_cast<const float4*>(pr + a0);
+                            const float4 qv = *reinterpret_cast<const float4*>(q2 + a0), wv = *reinterpret_cast<const float4*>(ws + a0);
+                            const float4 qv2 = *reinterpret_cast<const float4*>(qd + a0), wv2 = *reinterpret_cast<const float4*>(ws + A + a0);
+                            sum = att_term<F>(wv.x, v.x, qv.x, sum);
+                            sum = att_term<F>(wv.y, v.y, qv.y, sum);
+                            sum = att_term<F>(wv.z, v.z, qv.z, sum);
+                            sum = att_term<F>(wv.w, v.w, qv.w, sum);
+                            sum_d = att_term<F>(wv2.x, v.x, qv2.x, sum_d);
+                            sum_d = att_term<F>(wv2.y, v.y, qv2.y, sum_d);
+                            sum_d = att_term<F>(wv2.z, v.z, qv2.z, sum_d);
+                            sum_d = att_term<F>(wv2.w, v.w, qv2.w, sum_d);
+                        }
+                        sum = warp_sum(sum);
+                        sum_d = warp_sum(sum_d);
+                        if (lane == 0) {
+                            float z = sum + bias, zd = sum_d + bias_d;
+                            if (am) { z = GVD_MIN_VALUE; zd = GVD_MIN_VALUE; }
+                            a.z_out[(long long)(b0 + g) * a.z_stride_b + r0 + rl] = (am || om) ? GVD_MIN_VALUE : z;
+                            z_s[g * ATT_MAXC + rl] = z;
+                            z_s[(ATT_GMAX + g) * ATT_MAXC + rl] = zd;
+                        }
+                    }
+                } else {
+                    float4 v4[AJ > 0 ? AJ : 1];
+                    if (AJ > 0) {
+#pragma unroll
+                        for (int j = 0; j < AJ; ++j) v4[j] = *reinterpret_cast<const float4*>(pr + lane * 4 + 128 * j);
+                    }
+                    for (int g = 0; g < G; ++g) {
+                        float sum = att_row_sum_sq<AJ, F>(v4, pr, qs + g * A, w4, ws, A, lane);
+                        sum = warp_sum(sum);
+                        if (lane == 0) {
+                            float z = sum + bias;
+                            if (region) {
+                                if (am) z = GVD_MIN_VALUE;
+                                a.z_out[(long long)(b0 + g) * a.z_stride_b + r0 + rl] = (am || om) ? GVD_MIN_VALUE : z;
+                            }
+                            z_s[g * ATT_MAXC + rl] = z;
+                        }
+                    }
+                }
+            }
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty[s]);
+        }
+    };
+    if (FORM != GVD_REGION_ATTN_MIX && (region || dual)) phase_a(FormTag<FORM>{});
+    else phase_a(FormTag<GVD_REGION_ATTN_MIX>{});
+    consumer_bar();
+    // one warp per (score vector, row): the chunk softmax numerators, max and sum (the out-of-window term with that row's query)
+    for (int k = warp; k < nq * G; k += ATT_CWARPS) {
+        const int qi = k / G, g = k - qi * G;
+        const float* zz = z_s + (qi * ATT_GMAX + g) * ATT_MAXC;
+        float* ee = e_s + (qi * ATT_GMAX + g) * ATT_MAXC;
+        float m = -INFINITY, s0 = -INFINITY;
+        if (n_out > 0) {
+            float4 v4[AJ > 0 ? AJ : 1];
+            if (AJ > 0) {
+#pragma unroll
+                for (int j = 0; j < AJ; ++j) v4[j] = *reinterpret_cast<const float4*>(a.ctx_bias + lane * 4 + 128 * j);
+            }
+            s0 = warp_sum(att_row_sum_sq<AJ, GVD_REGION_ATTN_MIX>(v4, a.ctx_bias, qs + g * A, w4, ws, A, lane)) + bias;
+        }
+        for (int r = lane; r < nrows; r += 32) m = fmaxf(m, zz[r]);
+        m = fmaxf(warp_max(m), s0);
+        float l = 0.f;
+        for (int r = lane; r < nrows; r += 32) {
+            const float e = expf(zz[r] - m);
+            ee[r] = e;
+            l += e;
+        }
+        l = warp_sum(l);
+        if (n_out > 0) l = fmaf((float)n_out, expf(s0 - m), l);
+        if (lane == 0) { ml[2 * k] = m; ml[2 * k + 1] = l; }
+    }
+    consumer_bar();
+
+    // phase B: each row's unnormalised weighted sum from one read of each feature row
+    const int h0 = tid * 4;
+    const bool active = h0 < H;
+    float4 acc[ATT_GMAX], acc_d[ATT_GMAX];
+#pragma unroll
+    for (int g = 0; g < ATT_GMAX; ++g) { acc[g] = make_float4(0.f, 0.f, 0.f, 0.f); acc_d[g] = acc[g]; }
+    for (int j = 0; j < n_pb; ++j) {
+        const int i = n_pa + j, s = i % ATT_NST;
+        const uint32_t ph = (uint32_t)(i / ATT_NST) & 1u;
+        mbar_wait(&full[s], ph);
+        const float* st = reinterpret_cast<const float*>(smem + (size_t)s * ATT_STAGE_BYTES);
+        const int row0 = j * rows_pb, nr = min(rows_pb, nrows - row0);
+        if (active) {
+            for (int rr = 0; rr < nr; ++rr) {
+                const float4 v = *reinterpret_cast<const float4*>(st + (long long)rr * H + h0);
+#pragma unroll
+                for (int g = 0; g < ATT_GMAX; ++g) {
+                    if (g < G) {
+                        const float e = e_s[g * ATT_MAXC + row0 + rr];
+                        acc[g].x = fmaf(e, v.x, acc[g].x); acc[g].y = fmaf(e, v.y, acc[g].y);
+                        acc[g].z = fmaf(e, v.z, acc[g].z); acc[g].w = fmaf(e, v.w, acc[g].w);
+                        if (dual) {
+                            const float ed = e_s[(ATT_GMAX + g) * ATT_MAXC + row0 + rr];
+                            acc_d[g].x = fmaf(ed, v.x, acc_d[g].x); acc_d[g].y = fmaf(ed, v.y, acc_d[g].y);
+                            acc_d[g].z = fmaf(ed, v.z, acc_d[g].z); acc_d[g].w = fmaf(ed, v.w, acc_d[g].w);
+                        }
+                    }
+                }
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[s]);
+    }
+    const int nrec = dual ? 2 * nch_r : nch;
+#pragma unroll
+    for (int g = 0; g < ATT_GMAX; ++g) {
+        if (g < G) {
+            float* out = a.partial + ((long long)(b0 + g) * nrec + c) * (H + 4);
+            if (tid == 0) { out[0] = ml[2 * g]; out[1] = ml[2 * g + 1]; }
+            if (active && !(featmap && region)) *reinterpret_cast<float4*>(out + 4 + h0) = acc[g];
+            if (dual) {
+                float* out_d = a.partial + ((long long)(b0 + g) * nrec + nch_r + c) * (H + 4);
+                if (tid == 0) { out_d[0] = ml[2 * (G + g)]; out_d[1] = ml[2 * (G + g) + 1]; }
+                if (active) *reinterpret_cast<float4*>(out_d + 4 + h0) = acc_d[g];
+            }
+        }
+    }
+    if (a.ticket == nullptr) return;
+    // ---- fused merge by the group's last chunk CTA, row by row in attn_partial_kernel's fixed chunk order
+    __threadfence();
+    consumer_bar();
+    int* flag = reinterpret_cast<int*>(ml + 2 * nq * ATT_GMAX);
+    if (tid == 0) *flag = (atomicAdd(a.ticket + b0, 1) == nch - 1) ? 1 : 0;
+    consumer_bar();
+    if (*flag == 0) return;
+    __threadfence();
+    if (dual) {
+        // g = sigmoid(dual_pointer(h_att)) per row: per-thread partial dot, warp sums, the 8 warp sums added in warp order
+        for (int g = 0; g < G; ++g) {
+            float gd = 0.f;
+            if (active) {
+                const float4 hv = *reinterpret_cast<const float4*>(a.gate_h + (long long)(b0 + g) * a.gate_ld + h0);
+                const float4 wv = __ldg(reinterpret_cast<const float4*>(a.gate_w + h0));
+                gd = fmaf(wv.x, hv.x, gd); gd = fmaf(wv.y, hv.y, gd); gd = fmaf(wv.z, hv.z, gd); gd = fmaf(wv.w, hv.w, gd);
+            }
+            gd = warp_sum(gd);
+            if (lane == 0) red[g * ATT_CWARPS + warp] = gd;
+        }
+        consumer_bar();
+    }
+    for (int g = 0; g < G; ++g) {
+        const int b = b0 + g;
+        const float* base = a.partial + (long long)b * nrec * (H + 4);
+        if (dual) {
+            float glogit = __ldg(a.gate_b);
+            for (int wv = 0; wv < ATT_CWARPS; ++wv) glogit += red[g * ATT_CWARPS + wv];
+            const float gt = sigmoid_acc(glogit);
+            if (active) {
+                const float4 r0v = merge_part(base, 0, nch_r, H, h0), r1v = merge_part(base, nch_r, 2 * nch_r, H, h0);
+                const float h = 1.f - gt;
+                store_x(a, b, h0, make_float4(gt * r0v.x + h * r1v.x, gt * r0v.y + h * r1v.y, gt * r0v.z + h * r1v.z, gt * r0v.w + h * r1v.w));
+            }
+        } else if (active) {
+            float4 res = make_float4(0.f, 0.f, 0.f, 0.f);
+            const float4 t = merge_part(base, nch_r, nch, H, h0);                  // temporal chunks, then region chunks
+            res.x += t.x; res.y += t.y; res.z += t.z; res.w += t.w;
+            if (!featmap) {
+                const float4 r = merge_part(base, 0, nch_r, H, h0);
+                res.x += r.x; res.y += r.y; res.z += r.z; res.w += r.w;
+            }
+            store_x(a, b, h0, res);
+        }
+    }
+    if (tid == 0) a.ticket[b0] = 0;
+}
+
 // merge chunk partials: att = sum_c acc_c e^{m_c - M} / sum_c l_c e^{m_c - M}; x = att(temporal) + att2(region) (featmap: att only)
 __global__ void __launch_bounds__(256) attn_combine_kernel(const float* __restrict__ partial, float* __restrict__ x_out, int H,
                                                            int nch_r, int nch_t, int nparts) {
@@ -714,7 +1096,19 @@ static size_t attn_smem_bytes(int A, bool dual) {
            2 * (size_t)A * sizeof(float) + 16 + (dual ? (2 * (size_t)A + 2 * ATT_MAXC + 4) * sizeof(float) : 0);
 }
 
-int gvd_attn_partial(const AttnArgs& a, cudaStream_t st) {
+// the row-grouped kernel: the ring, [nq][GMAX][MAXC] scores and numerators, [nq][GMAX][2] records + flag, the gate sums, the barriers,
+// [nq][GMAX][A] queries and [nq][A] alpha_net weights (nq = 2 score vectors per row in dual_region)
+static size_t attn_group_smem_bytes(int A, bool dual) {
+    const size_t nq = dual ? 2 : 1;
+    return (size_t)ATT_NST * ATT_STAGE_BYTES + (2 * nq * ATT_GMAX * ATT_MAXC + 2 * nq * ATT_GMAX + 4 + ATT_GMAX * ATT_CWARPS) * sizeof(float) +
+           2 * ATT_NST * sizeof(uint64_t) + (nq * ATT_GMAX + nq) * (size_t)A * sizeof(float);
+}
+
+// The decode runs the per-row kernel at every rows-per-clip: on the same shared features it measured faster than the row-grouped kernel
+// at 2, 3, 5, 16 and 32 rows per clip and within 3 % either way at 8 (DESIGN §3, tools/sample_n_bench.py --part paths)
+int gvd_attn_partial(const AttnArgs& a, cudaStream_t st) { return gvd_attn_partial_path(a, 0, st); }
+
+int gvd_attn_partial_path(const AttnArgs& a, int path, cudaStream_t st) {
     GVD_REQUIRE(a.mode == GVD_ATT_INPUT_BOTH || a.mode == GVD_ATT_INPUT_FEATMAP || a.mode == GVD_ATT_INPUT_DUAL_REGION,
                 "attn: unknown att_input_mode %d", a.mode);
     const bool dual = a.mode == GVD_ATT_INPUT_DUAL_REGION;
@@ -732,14 +1126,24 @@ int gvd_attn_partial(const AttnArgs& a, cudaStream_t st) {
     int nch_r, nch_t;
     gvd_attn_chunks(a.R, a.T, a.RC, a.TC, &nch_r, &nch_t);
     if (dual) nch_t = 0;                         // no temporal attention (AttModel.py:126-128: the frame features are dummies)
-    const size_t smem = attn_smem_bytes(a.A, dual);
-    const unsigned grid = (unsigned)a.B * (unsigned)(nch_r + nch_t);
+    GVD_REQUIRE(path == 0 || path == 1, "attn: unknown path %d", path);
+    const bool grouped = path == 1;
+    const int div = a.feat_div > 1 ? a.feat_div : 1;
+    GVD_REQUIRE(!grouped || a.B % div == 0, "attn: B=%d rows is not a multiple of feat_div=%d", a.B, div);
+    const int ngroups = gvd_cdiv(div, ATT_GMAX);
+    const size_t smem = grouped ? attn_group_smem_bytes(a.A, dual) : attn_smem_bytes(a.A, dual);
+    GVD_REQUIRE(smem <= 227 * 1024, "attn: A=%d needs %zu bytes of shared memory", a.A, smem);
+    const unsigned grid = grouped ? (unsigned)(a.B / div) * (unsigned)ngroups * (unsigned)(nch_r + nch_t) : (unsigned)a.B * (unsigned)(nch_r + nch_t);
     const int aj = (a.A % 128 == 0 && a.A / 128 <= 4) ? a.A / 128 : 0;
-#define GVD_ATT_LAUNCH(AJ, F)                                                                                         \
-    do {                                                                                                              \
-        GVD_CHECK_CUDA(cudaFuncSetAttribute(attn_partial_kernel<AJ, F>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
-                                            (int)smem));                                                              \
-        GVD_CHECK_CUDA(gvd_launch(attn_partial_kernel<AJ, F>, dim3(grid), dim3(ATT_THREADS), smem, st, a, nch_r, nch_t)); \
+#define GVD_ATT_LAUNCH(AJ, F)                                                                                                   \
+    do {                                                                                                                        \
+        if (grouped) {                                                                                                          \
+            GVD_CHECK_CUDA(cudaFuncSetAttribute(attn_group_kernel<AJ, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            GVD_CHECK_CUDA(gvd_launch(attn_group_kernel<AJ, F>, dim3(grid), dim3(ATT_THREADS), smem, st, a, nch_r, nch_t, ngroups)); \
+        } else {                                                                                                                \
+            GVD_CHECK_CUDA(cudaFuncSetAttribute(attn_partial_kernel<AJ, F>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
+            GVD_CHECK_CUDA(gvd_launch(attn_partial_kernel<AJ, F>, dim3(grid), dim3(ATT_THREADS), smem, st, a, nch_r, nch_t));    \
+        }                                                                                                                       \
     } while (0)
 #define GVD_ATT_FORMS(AJ)                                                                   \
     do {                                                                                    \

@@ -82,6 +82,9 @@ struct AttnArgs {
 };
 int gvd_attn_chunks(int R, int T, int RC, int TC, int* nch_r, int* nch_t);
 int gvd_attn_partial(const AttnArgs& a, cudaStream_t st);
+// path 0 = attn_partial_kernel (one CTA per row and chunk, what gvd_attn_partial runs), 1 = attn_group_kernel (one CTA per group of up to 8
+// of a clip's feat_div rows and chunk); both give the same bits per row
+int gvd_attn_partial_path(const AttnArgs& a, int path, cudaStream_t st);
 int gvd_attn_combine(const float* partial, float* x_out, int B, int H, int nch_r, int nch_t, int mode, cudaStream_t st);
 int gvd_greedy_pick(const float* logits, long long ld, int B, int V, int unk_idx, long long* it_out, long long* seq_out,
                     float* logp_out, long long out_stride, const float* embed, float* xt, int E, cudaStream_t st, long long ld_xt = 0);

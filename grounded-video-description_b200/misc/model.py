@@ -30,6 +30,16 @@ def _seq(*mods):
     return nn.Sequential(*mods)
 
 
+def check_sample_n(n):
+    """eval_opt['sample_n'] as an int >= 1 (captions sampled per clip); ValueError for anything else (bool, float, < 1)."""
+    if isinstance(n, bool) or not hasattr(n, "__index__"):
+        raise ValueError("sample_n must be an integer >= 1 (got %r)" % (n,))
+    n = int(n.__index__())
+    if n < 1:
+        raise ValueError("sample_n must be an integer >= 1 (got %r)" % (n,))
+    return n
+
+
 class AttModel(CaptionModel):
     def __init__(self, opt):
         super().__init__()
@@ -199,12 +209,12 @@ class AttModel(CaptionModel):
             return seq, att2, sim_mat
         raise ValueError("unknown forward mode %r (expected 'MLE', 'GRD' or 'sample')" % (opt,))
 
-    def _prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, beam=1, nbox=0, video_idx=None, att2=False):
+    def _prologue(self, segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, beam=1, nbox=0, video_idx=None, att2=False, rows=1):
         nm = self._native_model()
         sim = nm.prologue(segs_feat.float().contiguous(), ppls.float().contiguous(), num.long().contiguous(),
                           ppls_feat.float().contiguous(), sample_idx.long().contiguous(), self._u8(pnt_mask).contiguous(),
                           want_sim=not self.enable_BUTD,       # BUTD (transformer only): nothing reads the similarity, so it is not computed
-                          beam=beam, nbox=nbox, att2=att2,     # the workspace is sized for the decode that follows
+                          beam=beam, nbox=nbox, att2=att2, rows=rows,   # the workspace is sized for the decode that follows
                           video_idx=video_idx.contiguous() if video_idx is not None else None)
         return nm, sim
 
@@ -219,11 +229,26 @@ class AttModel(CaptionModel):
 
         eval_opt['att2_weights'] = True asks for the region-attention logits [B,L,R] of the returned captions as the second output of
         'sample', the input of extract_grounding.  Greedy and multinomial decoding return them anyway; beam search then returns them
-        instead of its region index per word (see _sample_beam)."""
+        instead of its region index per word (see _sample_beam).
+
+        eval_opt['sample_n'] = n (sample_max = 0): n sampled captions per clip from one prologue.  seq, the log-probs and the att2 logits then
+        have B * n rows, caption j of clip b in row b * n + j; sim_mat stays [B, D+1, R], once per clip.  The draws equal the same call on
+        the batch repeated with repeat_interleave(n, 0) under the same seed (gvd_decode_sample_n), and with video_idx the rows are events x n.
+        extract_grounding then takes ppls.repeat_interleave(n, 0).  n = 1 (or no key) is the plain call; n > 1 is refused with sample_max = 1
+        (n identical greedy captions) and with beam_size > 1 (ValueError), and by the transformer captioner (NotImplementedError), which
+        decodes greedily whatever sample_max is."""
         sample_max = opt.get("sample_max", 1)
         beam_size = opt.get("beam_size", 1)
         temperature = opt.get("temperature", 1.0)
         video_idx = opt.get("video_idx")
+        sample_n = check_sample_n(opt.get("sample_n", 1))
+        if sample_n > 1:
+            if beam_size > 1:
+                raise ValueError("sample_n > 1 draws several sampled captions per clip; beam search (beam_size=%r) returns one" % (beam_size,))
+            if self.att_model == "transformer":
+                raise NotImplementedError("sample_n: the transformer captioner decodes greedily whatever sample_max is (model.py:570-578)")
+            if sample_max:
+                raise ValueError("sample_n > 1 needs sample_max = 0: greedy decoding would give %d identical captions per clip" % sample_n)
         if opt.get("att2_weights") and self.att_model == "transformer":
             raise NotImplementedError("att2_weights: the transformer captioner has no region attention to return (its 'sample' returns zeros "
                                       "there, model.py:578)")
@@ -245,10 +270,12 @@ class AttModel(CaptionModel):
             if not (math.isfinite(temperature) and temperature > 0):
                 raise ValueError("temperature must be finite and > 0 (got %r)" % (temperature,))
             seed = int(torch.randint(0, 2 ** 62, (1,)))
-        nm, sim = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, video_idx=video_idx)
+        nm, sim = self._prologue(segs_feat, ppls, num, ppls_feat, sample_idx, pnt_mask, video_idx=video_idx, rows=sample_n)
         mask = self._u8(pnt_mask).contiguous()
         if sample_max:
             seq, logp, att2 = nm.decode_greedy(B, T, mask)
+        elif sample_n > 1:
+            seq, logp, att2 = nm.decode_sample_n(B, T, sample_n, mask, seed, temperature)
         else:
             seq, logp, att2 = nm.decode_sample(B, T, mask, seed, temperature)
         return seq, logp, att2, sim

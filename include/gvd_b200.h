@@ -176,6 +176,25 @@ GVD_API int gvd_decode_sample(gvd_model_t* m, int B, int T, void* workspace, siz
                       float* att2_logits_out,       /* [B,L,R] masked logits (Q8)  */
                       void* stream);
 
+/* ---- n sampled captions per clip from one prologue (sample_max = 0, several candidates per clip).
+ * Rows: caption j of clip b is row b*n + j of seq_out / logprobs_out / att2_logits_out.  Equality: every output equals gvd_decode_sample on
+ * the batch whose clips are repeated n times in place (torch.repeat_interleave(n, 0) of every prologue input) with the same seed and
+ * temperature, bit for bit, given the same prologue outputs: the Philox counter takes the row index b*n + j, and the decode step runs the
+ * same kernels at B*n rows.  The prologue runs once per clip; the n rows of a clip attend over its one copy of the features (feat_div = n,
+ * as the beam rows do).  A prologue on the repeated batch runs its GEMMs with n times the rows, which can change their last bits.
+ * Workspace: gvd_workspace_bytes_sample_n(B, V, T, n) bytes (V = 0 after gvd_prologue_fwd, V > 0 after gvd_prologue_fwd_video): the
+ * prologue's outputs for B clips and decode state for B*n rows; gvd_prologue_fwd / _video must have filled it for the same (B, T).  The loop
+ * is captured as its own graph per (B, T, n); seed and temperature travel in the parameter block as for gvd_decode_sample.  n = 1 is
+ * gvd_decode_sample.  Vocabularies above 6144 words take the sliced tail as there.  Limits: n >= 1, B * n < 2^31. */
+GVD_API size_t gvd_workspace_bytes_sample_n(const gvd_model_t* m, int B, int V, int T, int n);
+GVD_API int gvd_decode_sample_n(gvd_model_t* m, int B, int T, int n, void* workspace, size_t workspace_bytes,
+                      const uint8_t* pnt_mask,      /* [B,R+1] per clip            */
+                      uint64_t seed, float temperature,
+                      int64_t* seq_out,             /* [B*n,L]                     */
+                      float* logprobs_out,          /* [B*n,L] or NULL             */
+                      float* att2_logits_out,       /* [B*n,L,R] masked logits     */
+                      void* stream);
+
 /* ---- S2-S4 one teacher-forced / externally driven step (misc/AttModel.py:134-164).
  * state layout in the workspace; `step` selects the ping-pong parity and must count from 0. */
 GVD_API int gvd_decode_step_fwd(gvd_model_t* m, int B, int T, void* workspace, size_t workspace_bytes, int step,
@@ -384,6 +403,15 @@ GVD_API int gvd_op_attention_video(const float* p_pool, const float* pool, const
                   int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld, int B, int R, int T, int A, int H, int RC, int TC,
                   int feat_div, int att_input_mode, const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld,
                   int region_attn_mode, const int64_t* video_idx, const int64_t* sample_idx, const float* ctx_bias, void* stream);
+/* gvd_op_attention_path: gvd_op_attention_video's arguments (video_idx / sample_idx / ctx_bias NULL: per-clip frame features) and the
+ *   kernel: path 0 = one CTA per (row, chunk), what every decode entry point runs; path 1 = one CTA per (clip, group of up to 8 of its
+ *   feat_div rows, chunk), which streams the chunk's features once for the group.  Both give the same bits per row. */
+GVD_API int gvd_op_attention_path(const float* p_pool, const float* pool, const float* p_conv, const float* conv, const float* q,
+                  const float* q_part, int q_S, const float* q_bias, const float* w1, const float* b1, const float* w2, const float* b2,
+                  const uint8_t* att_mask, const uint8_t* out_mask, int64_t out_mask_stride, float* z_out, int64_t z_stride_b, float* partial,
+                  int* ticket, float* x_out, int64_t x_ld, float* x_pk, int64_t x_pk_ld, int B, int R, int T, int A, int H, int RC, int TC,
+                  int feat_div, int att_input_mode, const float* gate_w, const float* gate_b, const float* gate_h, int64_t gate_ld,
+                  int region_attn_mode, const int64_t* video_idx, const int64_t* sample_idx, const float* ctx_bias, int path, void* stream);
 /* beam_topk: per row of logits [rows, V] (pitch ld) the K <= 8 (K <= V) best words, value descending, ties to the lower index:
  *   topv [rows, K] = their log_softmax, topi [rows, K].  NaN words are skipped; a pick that finds only NaN left takes the lowest untaken
  *   index, so an all-NaN row gives 0 .. K-1 (as a stable torch.sort(descending=True) does).  Rows only partly NaN differ from torch,
